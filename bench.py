@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- series fitted+forecast per second on N B200s (BASELINE.json metric).
+"""bench.py -- series fitted+forecast per second on N H100s (BASELINE.json metric).
 
     python bench.py --gpus 1 --steps 20 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
@@ -28,6 +28,8 @@ if ROOT not in sys.path:
 
 METRIC = "series fitted+forecast/sec"
 UNIT = "series/s"
+L2_BYTES = 50e6                 # H100 L2
+DUMP_BYTES = 32 << 20          # --dump-outputs: the forecast table, or a fixed sample of its rows past this size
 
 
 def parse():
@@ -42,7 +44,7 @@ def parse():
                     help="weak: --series per GPU (driver default); strong: --series in total = BASELINE configs[3] as worded "
                          "(1 M groups over 8 GPUs + one all-gather of the forecast table)")
     ap.add_argument("--tc-variant", type=int, default=0, choices=[0, 1, 2],
-                    help="tcgen05 kernel instantiation: 0 auto, 1 = 10 stages / 1 staging tile, 2 = 8 stages / 2 staging tiles")
+                    help="tensor-core fit kernel instantiation: 0 auto, 1 = 8 stages / 1 staging tile, 2 = 6 stages / 2 staging tiles")
     ap.add_argument("--calendars", type=int, default=0,
                     help="single GPU: ragged batch -- the series are split over this many distinct calendars (start dates "
                          "one day apart, same length) and fit in ONE launch (mmf_fit_forecast_ragged_f32)")
@@ -50,7 +52,7 @@ def parse():
                     help="single GPU diagnostic: store every forecast tile to this many LOCAL copies of the table through the "
                          "multi-destination epilogue (isolates its cost from NVLink)")
     ap.add_argument("--stream-solve", action="store_true",
-                    help="experimental: solve the series with gaps beside the tcgen05 kernel (mmf_config.stream_solve = 1)")
+                    help="experimental: solve the series with gaps beside the tensor-core kernel (mmf_config.stream_solve = 1)")
     ap.add_argument("--no-traffic", action="store_true", help="skip the live ncu DRAM-traffic probe of the dominant kernel")
     ap.add_argument("--traffic-child", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--t", type=int, default=1095)
@@ -73,6 +75,10 @@ def parse():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--ref-groups", type=int, default=0, help="groups per step of the reference arm (0 = 16 x cores)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the forecast table of the last step (rank 0; a fixed, seeded sample of "
+                         "its rows when larger than 32 MB) to DIR/forecast.npy (float32) and the sampled row numbers to "
+                         "DIR/forecast_rows.npy (float64), for comparing two builds output for output")
     return ap.parse_args()
 
 
@@ -81,11 +87,11 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -327,6 +333,19 @@ def live_traffic(args, n, kernel_name):
         return None, f"ncu probe failed: {exc!r}"
 
 
+def dump_outputs(out_dir, table):
+    """The forecast table the timed path left (what a caller of it receives), whole or as a fixed sample of its rows."""
+    import numpy as np
+    import torch
+    n, cols = table.shape
+    k = min(n, max(1, DUMP_BYTES // (4 * cols)))
+    rows = np.arange(n) if k == n else np.sort(np.random.default_rng(0).choice(n, size=k, replace=False))
+    idx = torch.from_numpy(rows).to(table.device)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "forecast.npy"), table.index_select(0, idx).float().cpu().numpy())
+    np.save(os.path.join(out_dir, "forecast_rows.npy"), rows.astype(np.float64))
+
+
 # =========================================================================================
 def run_ours(args):
     import numpy as np
@@ -350,7 +369,7 @@ def run_ours(args):
     n = args.series if args.scaling == "weak" else -(-args.series // world)
     K, W = args.steps, max(args.warmup, 3)
 
-    # ---- inputs: resident in HBM before the timed region; 4.4 GB per pass >> 126 MB L2
+    # ---- inputs: resident in HBM before the timed region; 4.4 GB per pass >> 50 MB L2
     y, start = mmf.synth.daily_store_item_demand_torch(n, t, seed=1234 + rank, nan_frac=args.nan_frac, device=dev,
                                                         ld=args.pitch_floats or None)
     torch.cuda.synchronize()
@@ -390,7 +409,7 @@ def run_ours(args):
 
     # inputs that fit a few L2s are rotated over distinct buffers so that every step streams from HBM
     in_bytes = n * t * 4
-    n_rot = 1 if in_bytes >= 4 * 126e6 else int(min(64, -(-int(5 * 126e6) // in_bytes)))
+    n_rot = 1 if in_bytes >= 4 * L2_BYTES else int(min(64, -(-int(5 * L2_BYTES) // in_bytes)))
     ys = [y] + [mmf.device_packed(y, device=dev) for _ in range(n_rot - 1)]      # same row pitch as y
     graphs = None
     if args.graph:
@@ -475,6 +494,8 @@ def run_ours(args):
     if world > 1:
         dist.all_reduce(tt, op=dist.ReduceOp.MAX)
     total_ms, kern_ms_avg = float(tt[0]), float(tt[1])
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, table)
     clocks = sampler.stop(wall0, wall1) if rank == 0 else None
     value = world * n * K / (total_ms * 1e-3)
     gather_check = None
@@ -616,7 +637,7 @@ def run_ours(args):
         others = {}
         try:
             for name, ns in (("configs[1] 10k x 1095", 10_000), ("configs[2] 100k x 1095", 100_000)):
-                rot = int(min(64, -(-int(5 * 126e6) // (ns * t * 4))))
+                rot = int(min(64, -(-int(5 * L2_BYTES) // (ns * t * 4))))
                 bufs = [mmf.device_packed(y[:ns], device=dev) for _ in range(rot)]       # distinct buffers: > 5x L2 in total
                 o = torch.empty((ns, h), device=dev)
                 k = [0]
@@ -690,9 +711,9 @@ def run_ours(args):
                                          "includes the call's one host synchronisation"} if args.calendars > 0 else {}),
                            "series_per_gpu": n, "t": t, "horizon": h, "nan_frac": args.nan_frac, "mode": args.mode,
                            "kernel": kernel_used,
-                           "l2": (f"inputs {in_bytes / 1e9:.2f} GB per step per GPU > 126 MB L2" if n_rot == 1 else
+                           "l2": (f"inputs {in_bytes / 1e9:.2f} GB per step per GPU > 50 MB L2" if n_rot == 1 else
                                   f"inputs {in_bytes / 1e6:.0f} MB per step: rotating over {n_rot} distinct buffers "
-                                  f"({n_rot * in_bytes / 1e6:.0f} MB > 126 MB L2)"),
+                                  f"({n_rot * in_bytes / 1e6:.0f} MB > 50 MB L2)"),
                            "cuda_graph": bool(args.graph),
                            "parallelism": f"series-sharded x{world}" + (f" + forecast table replicated to every rank via {gather}" if world > 1 else ""),
                            "gather": gather, "gather_max_abs_diff_vs_nccl": gather_check},

@@ -1,9 +1,9 @@
-"""dss-ml-at-scale_b200 -- B200-native many-models fit + forecast engine.
+"""dss-ml-at-scale_b200 -- H100-native many-models fit + forecast engine.
 
 A drop-in for ONE hot path of sebrahimi1988/dss-ml-at-scale: the
 ``groupBy("Product","SKU").applyInPandas(build_tune_and_score_model, ...)`` fan-out of
 group_apply/02_Fine_Grained_Demand_Forecasting.py:417-528.  All groups' series are packed
-into padded device buffers and fitted by hand-written sm_100a kernels in ``libmmf.so``
+into padded device buffers and fitted by hand-written sm_90a kernels in ``libmmf.so``
 (C ABI: ``include/mmf.h``).  There is no CPU implementation in this package.
 
 The directory name is not a Python identifier; import it as ``import mmf`` (alias

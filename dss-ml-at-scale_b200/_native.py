@@ -1,7 +1,7 @@
 """ctypes binding of ``libmmf.so`` (C ABI declared in ``include/mmf.h``).
 
 There is deliberately no CPU implementation behind this module: if the shared
-library is missing, or no B200 is visible, the calls raise.
+library is missing, or no H100 is visible, the calls raise.
 """
 from __future__ import annotations
 
@@ -77,7 +77,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a).  This package has no CPU fallback."
+            "(nvcc, sm_90a).  This package has no CPU fallback."
         )
     lib = C.CDLL(LIB_PATH)
     lib.mmf_version.restype = C.c_int

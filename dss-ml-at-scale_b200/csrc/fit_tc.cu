@@ -1,67 +1,62 @@
-// fit_tc.cu -- the sm_100a fast path: TMA-staged series tiles, tcgen05 moment GEMM with the
-// series tile as the TMEM A operand, TMEM accumulators, per-row epilogue.
+// fit_tc.cu -- the sm_90a fast path: TMA-staged series tiles, wgmma moment GEMM with the
+// centred series as the register A operand, per-row epilogue.
 //
 // What it computes (reference 02_Fine_Grained_Demand_Forecasting.py:435-494 for every group of the
 // applyInPandas fan-out 02:523-528, in the whitened calendar basis of DESIGN.md section 2):
-//     b_i  = A_fit^T (y_i - c_i)          [128 series x T] x [T x 16]  -> tcgen05.mma kind::tf32
+//     b_i  = A_fit^T (y_i - c_i)          [128 series x T] x [T x 16]  -> wgmma tf32
 //     yhat = c_i + A_pred b_i             (fully observed series: G_i = I, gamma_i = b_i)
 // fp32-grade accuracy on the tf32 tensor path comes from an exact 2-term split of both operands
-//     y - c = hi + lo,  A = A_hi + A_lo  ->  D = hi*[A_hi | A_lo] (N = 32)  +  lo*A_hi (N = 16)
+//     y - c = hi + lo,  A = A_hi + A_lo  ->  D = hi*[A_hi | A_lo] + lo*[A_hi | A_lo]   (N = 32 each, b = D[:, p] + D[:, P + p])
+// (lo*A_lo is below fp32 rounding; it is computed only so that both MMAs have the same shape and may chain on one
+// accumulator -- wgmma orders accumulator accesses only between MMAs of the same shape)
 // Rows that contain a non-finite value poison only their own accumulator row (NaN/Inf); the epilogue
 // detects that, marks the row MMF_STATUS_PENDING and the masked warp kernel finishes them.
 //
-// CTA = 14 warps, 1 CTA per SM, persistent over 128-series tiles, every stage decoupled by mbarriers:
+// CTA = 13 warps, 1 CTA per SM, persistent over 128-series tiles, every stage decoupled by mbarriers:
 //   warp 12    TMA producer: y box {32 t x 128 series} + design box {32 t x 32 (hi|lo columns)} per stage.
-//   warps 0-3 / 4-7   two transform groups taking alternate 32-step chunks.  Thread r owns series row r of
-//              the tile == TMEM lane r: LDS.128 its 128-B row of the TMA-swizzled stage, centre, split hi/lo,
-//              tcgen05.st the two 32-column A operands into the group's TMEM slot ring.
-//   warp 13    MMA issuer (warp-converged, elect.sync-predicated tcgen05.mma / commit) + TMEM allocation.
-//   warps 8-11 epilogue: tcgen05.ld the (double-buffered) accumulators of a finished tile, release them at
-//              once, then forecast + store while the next tile is already streaming.
+//   warps 0-3 / 4-7   two consumer warpgroups taking alternate 32-step chunks.  Per chunk each thread first scans
+//              series row r of the tile (r = its index in the warpgroup) for gaps, then loads its m16n8k8 fragments
+//              of both 64-row halves from the TMA-swizzled stage, centres and splits them hi/lo and issues the
+//              wgmma.mma_async chain into register accumulators.  At the end of a tile both warpgroups hand their
+//              partial moments (and gap counts) to the epilogue through a double-buffered shared-memory slot.
+//   warps 8-11 epilogue: sum the two partials of a finished tile, release the slot at once, then forecast + store
+//              while the next tile is already streaming.
 // Algorithmic HBM bytes per series: 4*t_fit read + 4*n_pred written (DESIGN.md section 4).
 #include "mmf_internal.cuh"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace mmf {
 namespace {
 
-using namespace sm100;
+using namespace sm90;
 
-#ifndef MMF_TC_ASLOTS
-#define MMF_TC_ASLOTS 2
-#endif
-constexpr int TILE_M = 128;            // series per tile == TMEM lanes
+constexpr int TILE_M = 128;            // series per tile
 constexpr int KC = 32;                 // time steps per stage == one 128-B swizzle row
 // The shared-memory ring (20 KB per stage) and the number of forecast staging tiles are template parameters of the
-// kernel: <10 stages, 1 staging tile> is the product configuration, <8, 2> (a second staging tile lets tile k+1 be
-// assembled while the NVLink stores of tile k are still reading tile k's) an experiment that did not pay.
-constexpr int NGROUPS = 2;             // transform groups (alternate chunks)
-constexpr int ASLOTS = MMF_TC_ASLOTS;  // TMEM A-operand slots per transform group
+// kernel: <8 stages, 1 staging tile> is the product configuration, <6, 2> (a second staging tile lets tile k+1 be
+// assembled while the NVLink stores of tile k are still reading tile k's) an experiment.
+constexpr int NGROUPS = 2;             // consumer warpgroups (alternate chunks)
 constexpr int MAX_PRED = 64;           // forecast rows the epilogue supports
-constexpr int NM_RING = 8;             // tiles the transform groups may run ahead of the epilogue (2 slots x 2 groups)
 constexpr int BULK_MAX_PRED = 28;      // forecast rows the staged bulk-store epilogue supports (14 KB of smem)
 constexpr int Y_STAGE_BYTES = TILE_M * KC * 4;      // 16384
 constexpr int AT_STAGE_BYTES = 2 * P * KC * 4;      // 4096
-constexpr int THREADS = 448;
-constexpr int WARP_EPI0 = 8, WARP_PROD = 12, WARP_MMA = 13;
-constexpr uint32_t TMEM_COLS = 512;
-constexpr uint32_t ACC_COL0 = 0;                    // 2 accumulator buffers x 32 columns
-constexpr uint32_t ASLOT_COL0 = 64;                 // group g, slot j: hi at 64 + (g*ASLOTS + j)*64, lo 32 further
-static_assert(64 + NGROUPS * ASLOTS * 64 <= 512, "TMEM holds 512 columns");
+constexpr int THREADS = 416;
+constexpr int WARP_EPI0 = 8, WARP_PROD = 12;
+// named barriers: 1-3 epilogue, 4 + g consumer warpgroup g
 
 template <int STAGES, int OBUF>
 struct SmemLayoutT {
-  static_assert(STAGES % NGROUPS == 0, "each transform group must always see the same stages");
   // offsets from the 1024-aligned base
   static constexpr int y = 0;
   static constexpr int at = y + STAGES * Y_STAGE_BYTES;
   static constexpr int apred = at + STAGES * AT_STAGE_BYTES;
   static constexpr int ostage = apred + MAX_PRED * P * 4;            // forecast tile staged for the bulk stores
-  static constexpr int nm = ostage + OBUF * TILE_M * BULK_MAX_PRED * 4;   // per-row missing counts: [NM_RING][2 groups][128] u16
-  static constexpr int bars = nm + NM_RING * NGROUPS * TILE_M * 2;
-  static constexpr int n_bars = 2 * STAGES + 2 * NGROUPS * ASLOTS + 4 + NM_RING;
-  static constexpr int tmem_ptr = bars + n_bars * 8;
-  static constexpr int total = tmem_ptr + 16;
+  static constexpr int acc = ostage + OBUF * TILE_M * BULK_MAX_PRED * 4;   // partial moments: [2 slots][2 groups][128][P] f32
+  static constexpr int nm = acc + 2 * NGROUPS * TILE_M * P * 4;      // gap counts: [2 slots][2 chunk parities][128] u16
+  static constexpr int cc = nm + 2 * NGROUPS * TILE_M * 2;           // centring constants: [2 groups][2 tiles][128] f32
+  static constexpr int bars = cc + NGROUPS * 2 * TILE_M * 4;
+  static constexpr int n_bars = 2 * STAGES + 4;
+  static constexpr int total = bars + n_bars * 8;
   static_assert(total + 1024 <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into");
 };
 
@@ -93,23 +88,22 @@ __device__ __forceinline__ float centring_constant(const float* __restrict__ yro
   return c;
 }
 
+__device__ __forceinline__ bool is_finite_bits(float x) { return (__float_as_uint(x) & 0x7f800000u) != 0x7f800000u; }
+
+__device__ __forceinline__ float lds32(uint32_t addr) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
+  return v;
+}
+
 // MULTI: a ragged launch -- every 128-row tile names its calendar (mv.tiles / mv.cals); `n_chunks` is then only the
 // minimum over the calendars (>= 2).  MULTI == false compiles to the single-calendar kernel.
-// Register budget: ptxas takes 128 registers with __launch_bounds__(448, 1).  -DMMF_TC_MAXNREG=80 caps the kernel so that
-// one 128-thread block of the streaming solve (solve_stream_kernel, 214 registers) fits beside the CTA on an SM -- an
-// experiment that did not pay: at 80 registers the transform loop loses its load/compute overlap and the gap-free step
-// goes from 0.739 to 0.924 ms (2 % NaN: 1.985 ms instead of 1.449), DESIGN.md section 6b.
-#ifdef MMF_TC_MAXNREG
-#define MMF_TC_KERNEL_ATTR __maxnreg__(MMF_TC_MAXNREG)
-#else
-#define MMF_TC_KERNEL_ATTR __launch_bounds__(THREADS, 1)
-#endif
-// BAL (tc_variant = 3, an experiment): a balanced launch -- instead of dealing 128-row tiles round robin (79 tiles
-// leave 69 of the 148 SMs idle), every CTA owns one contiguous range of mv.bal_rows rows (a multiple of 8) and walks it in 128-row tiles; the
-// range's last tile is short and is loaded as 8-row boxes, so no SM streams rows it does not own.
+// BAL (tc_variant = 3, an experiment): a balanced launch -- instead of dealing 128-row tiles round robin, every CTA owns
+// one contiguous range of mv.bal_rows rows (a multiple of 8) and walks it in 128-row tiles; the range's last tile is
+// short and is loaded as 8-row boxes, so no SM streams rows it does not own.
 // Rows are independent in the GEMM, so the forecasts are bit-identical to the round-robin launch's.
 template <int STAGES, int OBUF, bool MULTI, bool BAL>
-__global__ void MMF_TC_KERNEL_ATTR
+__global__ void __launch_bounds__(THREADS, 1)
 fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const FitArgs a,
               uint32_t* __restrict__ pending_count, const int n_tiles_all, const int n_chunks, const MultiView mv) {
   static_assert(!(MULTI && BAL), "ragged launches carry their own tile table");
@@ -140,7 +134,9 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
   const uint32_t s_at = sbase + SmemLayout::at;
   float* s_apred = reinterpret_cast<float*>(smem + SmemLayout::apred);
   float* s_ostage = reinterpret_cast<float*>(smem + SmemLayout::ostage);
+  float* s_acc = reinterpret_cast<float*>(smem + SmemLayout::acc);
   uint16_t* s_nm = reinterpret_cast<uint16_t*>(smem + SmemLayout::nm);
+  float* s_cc = reinterpret_cast<float*>(smem + SmemLayout::cc);
   // series with gaps: substitute the centring constant for missing values (so the moments stay exact), record
   // where they were, and let the epilogue queue a SolveRec for solve_rows_kernel instead of a second pass
 #ifdef MMF_TC_NO_COLLECT
@@ -151,12 +147,8 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
   const uint32_t s_bars = sbase + SmemLayout::bars;
   auto bar_full = [&](int s) { return s_bars + 8u * s; };
   auto bar_empty = [&](int s) { return s_bars + 8u * (STAGES + s); };
-  auto bar_afull = [&](int g, int j) { return s_bars + 8u * (2 * STAGES + g * ASLOTS + j); };
-  auto bar_aempty = [&](int g, int j) { return s_bars + 8u * (2 * STAGES + NGROUPS * ASLOTS + g * ASLOTS + j); };
-  auto bar_accfull = [&](int b) { return s_bars + 8u * (2 * STAGES + 2 * NGROUPS * ASLOTS + b); };
-  auto bar_accempty = [&](int b) { return s_bars + 8u * (2 * STAGES + 2 * NGROUPS * ASLOTS + 2 + b); };
-  auto bar_nm = [&](int i) { return s_bars + 8u * (2 * STAGES + 2 * NGROUPS * ASLOTS + 4 + i); };   // s_nm slot published
-  volatile uint32_t* tmem_ptr_smem = reinterpret_cast<volatile uint32_t*>(smem + SmemLayout::tmem_ptr);
+  auto bar_accfull = [&](int b) { return s_bars + 8u * (2 * STAGES + b); };
+  auto bar_accempty = [&](int b) { return s_bars + 8u * (2 * STAGES + 2 + b); };
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -166,47 +158,31 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
 #pragma unroll
     for (int i = 0; i < CTR_WORDS; ++i) a.zero_next[i] = 0u;
   }
-  if (warp == WARP_MMA) {
+  if (warp == WARP_PROD) {
     if (lane == 0) {
       for (int s = 0; s < STAGES; ++s) {
         mbar_init(bar_full(s), 1);        // producer's expect_tx arrive (+ TMA bytes)
-        mbar_init(bar_empty(s), 5);       // 4 warps of the consuming transform group + 1 tcgen05.commit
+        mbar_init(bar_empty(s), 4);       // 4 warps of the consuming warpgroup, after their MMAs have retired
       }
-      for (int g = 0; g < NGROUPS; ++g)
-        for (int j = 0; j < ASLOTS; ++j) {
-          mbar_init(bar_afull(g, j), 4);  // 4 transform warps
-          mbar_init(bar_aempty(g, j), 1); // tcgen05.commit
-        }
       for (int b = 0; b < 2; ++b) {
-        mbar_init(bar_accfull(b), 1);     // tcgen05.commit after the tile's last chunk
-        mbar_init(bar_accempty(b), 4);    // 4 epilogue warps have read the accumulators
+        // partial moments + gap counts of a tile: every consumer THREAD arrives after writing its entries (release),
+        // the epilogue's wait acquires them (the writer of each entry synchronises with its reader directly)
+        mbar_init(bar_accfull(b), NGROUPS * 128);
+        mbar_init(bar_accempty(b), 4);    // 4 epilogue warps have read the slot
       }
-      // gap counts of a tile: one arrival per transform warp that owns a chunk of it (release) -> epilogue (acquire)
-      // (every THREAD of those warps arrives, not one elected lane after a __syncwarp: the writer of each s_nm entry
-      //  then synchronises with its reader directly, which is also what compute-sanitizer's racecheck can follow)
-      for (int i = 0; i < NM_RING; ++i) mbar_init(bar_nm(i), n_chunks >= 2 ? 256 : 128);
       fence_mbar_init();
-    }
-    __syncwarp();
-    tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_ptr_smem)), TMEM_COLS);
-    tmem_relinquish();
-  } else if (warp == WARP_PROD) {
-    if (lane == 0) {
       prefetch_tensormap(tl.tmap_y);
       prefetch_tensormap(tl.tmap_at);
       if (BAL) prefetch_tensormap(tl.tmap_y8);
     }
-  } else if (warp >= WARP_EPI0 && warp < WARP_PROD) {
+  } else if (warp >= WARP_EPI0) {
     // prediction rows of the whitened design -> shared (broadcast-read in the epilogue); ragged launches reload
     // them whenever the epilogue reaches a tile of another calendar
     if (!a.skip_pred && !MULTI)
       for (int i = threadIdx.x - WARP_EPI0 * 32; i < a.n_pred * P; i += 128)
         s_apred[i] = __ldg(d.apred + (size_t)a.pred_start * P + i);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   // This CTA is resident: a dependent kernel launched behind this one with programmatic stream serialisation may start
   // once EVERY CTA has said so -- the streaming solve then finds all producers running (it never has to wait for a
   // producer that cannot get an SM), the early-exit fix-up kernels hide their launch latency under this kernel's tail.
@@ -228,8 +204,9 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
       const int at_row = MULTI ? tr.cal * 2 * P : 0;
       if (BAL && tr.nrows < TILE_M) {
         // short tile: the design box as usual, the series rows as 8-row boxes (same swizzled layout: a box is one
-        // 1,024-B swizzle atom of the stage); rows beyond the tile keep whatever the stage held -- their lanes compute
-        // garbage that nobody reads.  A box that crosses the end of the buffer is zero-filled and still counts in full.
+        // 1,024-B swizzle atom of the stage); rows beyond the tile keep whatever the stage held -- their accumulator
+        // rows hold garbage that nobody reads.  A box that crosses the end of the buffer is zero-filled and still
+        // counts in full.
         const int nb = (tr.nrows + 7) >> 3;
         for (int ch = 0; ch < tr.n_chunks; ++ch) {
           mbar_wait(bar_empty(stage), phase ^ 1u);
@@ -251,205 +228,153 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
         if (++stage == STAGES) { stage = 0; phase ^= 1u; }
       }
     }
-  } else if (warp == WARP_MMA) {
-    // =========================== MMA issuer ===========================
-    // whole warp converged; tcgen05.mma / commit are predicated on elect.sync inside the wrappers
-    constexpr uint32_t IDESC_N32 = umma_idesc_tf32(TILE_M, 2 * P);
-    constexpr uint32_t IDESC_N16 = umma_idesc_tf32(TILE_M, P);
-    int stage = 0;
-    uint32_t phase = 0;
-    int aslot0 = 0, aslot1 = 0;
-    uint32_t aphase0 = 0u, aphase1 = 0u;
-    int grp = 0;                                     // chunk i of the CTA's stream belongs to group i & 1
-    int lt = 0;                                      // local tile counter -> accumulator buffer lt & 1
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++lt) {
-      const int ab = lt & 1;
-      const int tile_chunks = MULTI ? tile_rec(tile).n_chunks : n_chunks;
-      mbar_wait(bar_accempty(ab), ((lt >> 1) & 1) ^ 1u);    // epilogue of tile lt-2 has drained this buffer
-      tc_fence_after();
-      const uint32_t d_acc = tmem_base + ACC_COL0 + ab * 32;
-      for (int ch = 0; ch < tile_chunks; ++ch) {
-        const int aslot = grp ? aslot1 : aslot0;
-        const uint32_t aphase = grp ? aphase1 : aphase0;
-        mbar_wait(bar_full(stage), phase);                 // design chunk landed (same barrier as the y box)
-        mbar_wait(bar_afull(grp, aslot), aphase);          // A operand written to TMEM by the transform group
-        tc_fence_after();
-        const uint64_t bdesc0 = umma_desc_k_sw128(s_at + stage * AT_STAGE_BYTES);
-        const uint32_t a_hi = tmem_base + ASLOT_COL0 + (grp * ASLOTS + aslot) * 64;
-        const uint32_t a_lo = a_hi + 32;
-#pragma unroll
-        for (int k = 0; k < KC / 8; ++k) {
-          const uint64_t bdesc = bdesc0 + static_cast<uint64_t>(k * 2);       // +32 B (16-B units)
-          umma_tf32_ts_elect(d_acc, a_hi + k * 8, bdesc, IDESC_N32, (ch | k) != 0 ? 1u : 0u);
-#ifndef MMF_TC_NO_LO_TERM      // negative-control build (tests): without lo*A_hi the path is tf32-grade and must FAIL parity
-          umma_tf32_ts_elect(d_acc, a_lo + k * 8, bdesc, IDESC_N16, 1u);
-#endif
-        }
-        umma_commit_elect(bar_aempty(grp, aslot));
-        umma_commit_elect(bar_empty(stage));
-        if (ch == tile_chunks - 1) umma_commit_elect(bar_accfull(ab));
-        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        if (grp) { if (++aslot1 == ASLOTS) { aslot1 = 0; aphase1 ^= 1u; } }
-        else     { if (++aslot0 == ASLOTS) { aslot0 = 0; aphase0 ^= 1u; } }
-        grp ^= 1;
-      }
-    }
   } else if (warp < NGROUPS * 4) {
-    // =========================== transform groups (warps 0-3, 4-7) ===========================
+    // =========================== consumer warpgroups (warps 0-3, 4-7) ===========================
+    // Chunk k of the CTA's stream (counted over all its tiles) sits in stage k % STAGES and belongs to group k & 1.
     const int grp = warp >> 2;
-    const int r = threadIdx.x & 127;                    // row in tile == TMEM lane
-    const uint32_t lane_addr = static_cast<uint32_t>((warp & 3) * 32) << 16;
+    const int r = threadIdx.x & 127;                    // gap scan: row r of the tile
     const uint32_t row_off = static_cast<uint32_t>(r) * 128u;
     const uint32_t sw = static_cast<uint32_t>(r & 7);
-    // this group's chunks are every other chunk of the CTA's stream
-    int stage = grp;                                    // STAGES is even: the group always sees stages of its parity
-    uint32_t phase = 0;
-    int aslot = 0;
-    uint32_t aphase = 0;
+    const int g8 = lane >> 2, t4 = lane & 3;            // MMA fragments: rows 64h + 16*(warp & 3) + g8 (+8), cols t4 (+4)
+    const int frow0 = 16 * (warp & 3) + g8;
+    float* __restrict__ s_c = s_cc + grp * 2 * TILE_M;
+    uint32_t gc = 0;                                    // first chunk of the current tile in the CTA's stream
     int tile = blockIdx.x;
     TileRec tr = tile_rec(tile);
-    int ch = grp;
-    while (tile < n_tiles && ch >= tr.n_chunks) { ch -= tr.n_chunks; tile += gridDim.x; tr = tile_rec(tile); }   // 1-chunk corner
     TileRec trn = tile_rec(tile + (int)gridDim.x);
     auto load_c = [&](int tl_, const TileRec& t) -> float {
       return (d.has_constant && tl_ < n_tiles && r < t.nrows)
                  ? centring_constant(a.y + (int64_t)(t.row0 + r) * a.ld_y, tfit_of(t)) : 0.f;
     };
-    auto finite = [](float x) { return (__float_as_uint(x) & 0x7f800000u) != 0x7f800000u; };
     float c = load_c(tile, tr);
     float c_next = load_c(tile + (int)gridDim.x, trn);  // one tile ahead: the latency hides under the tile
-    bool bad = collect && !finite(c);                   // cannot centre on a missing first value: general path
-    if (bad) c = 0.f;
-    int nm = 0;                                         // missing values this thread saw in the current tile
-    unsigned long long packq = 0ull;                    // the last (nm & 3) gap positions, newest in the top lanes
-    int lt = 0;                                         // local tile counter (s_nm ring slot)
-    while (tile < n_tiles) {
-      mbar_wait(bar_full(stage), phase);
-      const uint32_t rowp = s_y + stage * Y_STAGE_BYTES + row_off;
-      float4 v[8];
+    for (int lt = 0; tile < n_tiles; ++lt) {
+      const bool bad = collect && !is_finite_bits(c);   // cannot centre on a missing first value: general path
+      if (bad) c = 0.f;
+      s_c[(lt & 1) * TILE_M + r] = c;
+      named_bar_sync(4 + grp, 128);
+      float cf[2][2];                                   // centring constants of this thread's four fragment rows
 #pragma unroll
-      for (int q = 0; q < 8; ++q) v[q] = lds128(rowp + ((static_cast<uint32_t>(q) ^ sw) << 4));
-      // (ragged / balanced: rows of a short tile beyond its last row belong to ANOTHER tile -- never touch their records)
-      if (collect && (!(MULTI || BAL) || r < tr.nrows)) {
-        float2 chk2 = make_float2(0.f, 0.f);            // 0 * x is NaN exactly when x is NaN or Inf
-        const float2 zero2 = make_float2(0.f, 0.f);
+      for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          chk2 = fma_f32x2(make_float2(v[q].x, v[q].y), zero2, chk2);
-          chk2 = fma_f32x2(make_float2(v[q].z, v[q].w), zero2, chk2);
-        }
-        const float chk = chk2.x + chk2.y;
-        if (!(chk == 0.f)) {                            // rare: this row has a gap inside this chunk
-          // branch-free substitution + a bit mask of the gap positions, then a short loop over the set bits
-          unsigned gaps = 0u;
+        for (int j = 0; j < 2; ++j) cf[h][j] = s_c[(lt & 1) * TILE_M + 64 * h + frow0 + 8 * j];
+      float acc[2][P];                                  // m64n32 accumulators of the two 64-row halves
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < P; ++i) acc[h][i] = 0.f;
+      const bool scan = collect && (!(MULTI || BAL) || r < tr.nrows);   // short tiles: rows beyond belong to ANOTHER tile
+      // segment = parity of the chunk inside the TILE (all of a group's chunks of one tile share it), not the group:
+      // with an odd chunk count the groups swap roles from tile to tile, and the order in which the solve applies
+      // the gaps -- hence the forecast's last bits -- must not depend on where in a launch the series sits
+      const int seg = (grp ^ (int)gc) & 1;
+      int nm = 0;                                       // missing values this thread saw in the tile
+      unsigned long long packq = 0ull;                  // the last (nm & 3) gap positions, newest in the top lanes
+      for (int ch = seg; ch < tr.n_chunks; ch += NGROUPS) {
+        const uint32_t k = gc + static_cast<uint32_t>(ch);
+        const int stage = static_cast<int>(k % STAGES);
+        mbar_wait(bar_full(stage), (k / STAGES) & 1u);
+        const uint32_t sy = s_y + stage * Y_STAGE_BYTES;
+        if (scan) {
+          const uint32_t rowp = sy + row_off;
+          float4 v[8];
+#pragma unroll
+          for (int q = 0; q < 8; ++q) v[q] = lds128(rowp + ((static_cast<uint32_t>(q) ^ sw) << 4));
+          float chk = 0.f;                              // 0 * x is NaN exactly when x is NaN or Inf
 #pragma unroll
           for (int q = 0; q < 8; ++q) {
-            const bool f0 = finite(v[q].x), f1 = finite(v[q].y), f2 = finite(v[q].z), f3 = finite(v[q].w);
-            gaps |= (f0 ? 0u : 1u << (4 * q)) | (f1 ? 0u : 2u << (4 * q)) | (f2 ? 0u : 4u << (4 * q)) | (f3 ? 0u : 8u << (4 * q));
-            v[q].x = f0 ? v[q].x : c;  v[q].y = f1 ? v[q].y : c;      // contributes (c - c) = 0 to every moment
-            v[q].z = f2 ? v[q].z : c;  v[q].w = f3 ? v[q].w : c;
+            chk = fmaf(v[q].x, 0.f, chk); chk = fmaf(v[q].y, 0.f, chk);
+            chk = fmaf(v[q].z, 0.f, chk); chk = fmaf(v[q].w, 0.f, chk);
           }
-          // positions are shifted into a 64-bit register and leave four at a time (one 8-B store, the unit the
-          // solve kernel reads): a 2-B store per gap made the record traffic the limiter of the gappy case
-          // segment = parity of the chunk inside the TILE (all of a group's chunks of one tile share it), not the group:
-          // with an odd chunk count the groups swap roles from tile to tile, and the order in which the solve applies
-          // the gaps -- hence the forecast's last bits -- must not depend on where in a launch the series sits
-          uint16_t* __restrict__ mt = a.recs[(int64_t)tr.row0 + r].miss_t + (ch & 1) * SOLVE_SEG;
-          const int tbase = ch * KC;
-          while (gaps) {
-            const int pos = __ffs(gaps) - 1;
-            gaps &= gaps - 1u;
-            packq = (packq >> 16) | (static_cast<unsigned long long>(tbase + pos) << 48);
-            ++nm;
-            if ((nm & 3) == 0 && nm <= SOLVE_SEG) *reinterpret_cast<unsigned long long*>(mt + nm - 4) = packq;
-          }
-        }
-      }
-      const float2 c2 = make_float2(c, c);
-      const uint32_t a_hi = tmem_base + lane_addr + ASLOT_COL0 + (grp * ASLOTS + aslot) * 64;
-#ifdef MMF_TC_HALF_ST
-      // register diet (with -DMMF_TC_MAXNREG=80): the chunk leaves in two 16-column halves, so only 32 split values are
-      // live at a time instead of 64
+          if (!(chk == 0.f)) {                          // rare: this row has a gap inside this chunk
+            // a bit mask of the gap positions, then a short loop over the set bits; positions are shifted into a
+            // 64-bit register and leave four at a time (one 8-B store, the unit the solve kernel reads)
+            unsigned gaps = 0u;
 #pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        uint32_t hi[16], lo[16];
-#pragma unroll
-        for (int q4 = 0; q4 < 4; ++q4) {
-          const int q = half * 4 + q4;
-#pragma unroll
-          for (int hlf = 0; hlf < 2; ++hlf) {
-            const float2 e = hlf ? make_float2(v[q].z, v[q].w) : make_float2(v[q].x, v[q].y);
-            const float2 rr = sub_f32x2(e, c2);
-            const uint32_t h0 = __float_as_uint(rr.x) & 0xFFFFE000u, h1 = __float_as_uint(rr.y) & 0xFFFFE000u;
-            const float2 l = sub_f32x2(rr, make_float2(__uint_as_float(h0), __uint_as_float(h1)));
-            hi[q4 * 4 + 2 * hlf] = h0;  hi[q4 * 4 + 2 * hlf + 1] = h1;
-            lo[q4 * 4 + 2 * hlf] = __float_as_uint(l.x);  lo[q4 * 4 + 2 * hlf + 1] = __float_as_uint(l.y);
+            for (int q = 0; q < 8; ++q)
+              gaps |= (is_finite_bits(v[q].x) ? 0u : 1u << (4 * q)) | (is_finite_bits(v[q].y) ? 0u : 2u << (4 * q)) |
+                      (is_finite_bits(v[q].z) ? 0u : 4u << (4 * q)) | (is_finite_bits(v[q].w) ? 0u : 8u << (4 * q));
+            uint16_t* __restrict__ mt = a.recs[(int64_t)tr.row0 + r].miss_t + seg * SOLVE_SEG;
+            const int tbase = ch * KC;
+            while (gaps) {
+              const int pos = __ffs(gaps) - 1;
+              gaps &= gaps - 1u;
+              packq = (packq >> 16) | (static_cast<unsigned long long>(tbase + pos) << 48);
+              ++nm;
+              if ((nm & 3) == 0 && nm <= SOLVE_SEG) *reinterpret_cast<unsigned long long*>(mt + nm - 4) = packq;
+            }
           }
         }
-        if (half == 0) {
-          mbar_wait(bar_aempty(grp, aslot), aphase ^ 1u);   // MMAs that read this A slot have retired
-          tc_fence_after();
-        }
-        tmem_st_32x32b_x16(a_hi + half * 16, hi);
-        tmem_st_32x32b_x16(a_hi + 32 + half * 16, lo);
-      }
-#else
-      uint32_t hi[32], lo[32];
+        // A fragments of both 64-row halves: centre (missing values take the centring constant, so they add
+        // (c - c) = 0 to every moment), split into tf32 hi + fp32 residual lo
+        uint32_t ahi[2][KC / 8][4], alo[2][KC / 8][4];
 #pragma unroll
-      for (int q = 0; q < 8; ++q) {
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int hlf = 0; hlf < 2; ++hlf) {              // packed pairs: FADD2 for the centring and the residual
-          const float2 e = hlf ? make_float2(v[q].z, v[q].w) : make_float2(v[q].x, v[q].y);
-          const float2 rr = sub_f32x2(e, c2);
-          const uint32_t h0 = __float_as_uint(rr.x) & 0xFFFFE000u, h1 = __float_as_uint(rr.y) & 0xFFFFE000u;
-          const float2 l = sub_f32x2(rr, make_float2(__uint_as_float(h0), __uint_as_float(h1)));
-          hi[q * 4 + 2 * hlf] = h0;  hi[q * 4 + 2 * hlf + 1] = h1;
-          lo[q * 4 + 2 * hlf] = __float_as_uint(l.x);  lo[q * 4 + 2 * hlf + 1] = __float_as_uint(l.y);
-        }
-      }
-      mbar_wait(bar_aempty(grp, aslot), aphase ^ 1u);   // MMAs that read this A slot have retired
-      tc_fence_after();
-      tmem_st_32x32b_x32(a_hi, hi);
-      tmem_st_32x32b_x32(a_hi + 32, lo);
+          for (int j = 0; j < 2; ++j) {
+            const uint32_t rowp = sy + static_cast<uint32_t>(64 * h + frow0 + 8 * j) * 128u + t4 * 4;   // row & 7 == g8
+#pragma unroll
+            for (int kk = 0; kk < KC / 8; ++kk)
+#pragma unroll
+              for (int hf = 0; hf < 2; ++hf) {
+                float x = lds32(rowp + ((static_cast<uint32_t>(2 * kk + hf) ^ static_cast<uint32_t>(g8)) << 4));
+                if (collect) x = is_finite_bits(x) ? x : cf[h][j];
+                const float rr = x - cf[h][j];
+                const uint32_t hb = __float_as_uint(rr) & 0xFFFFE000u;
+                ahi[h][kk][j + 2 * hf] = hb;
+                alo[h][kk][j + 2 * hf] = __float_as_uint(rr - __uint_as_float(hb));
+              }
+          }
+        const uint64_t bdesc0 = gmma_desc_k_sw128(s_at + stage * AT_STAGE_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int kk = 0; kk < KC / 8; ++kk) {
+            const uint64_t bdesc = bdesc0 + static_cast<uint64_t>(kk * 2);       // +32 B (16-B units)
+            wgmma_m64n32k8_tf32_rs(acc[h], ahi[h][kk], bdesc);
+#ifndef MMF_TC_NO_LO_TERM      // negative-control build (tests): without the lo term the path is tf32-grade and must FAIL parity
+            wgmma_m64n32k8_tf32_rs(acc[h], alo[h][kk], bdesc);
 #endif
-      const bool last_own = collect && ch + NGROUPS >= tr.n_chunks;    // my last chunk of this tile
-      if (last_own) {
-        if ((nm & 3) != 0 && nm < SOLVE_SEG) {          // flush the partial group (right-aligned: oldest first)
-          uint16_t* __restrict__ mt = a.recs[(int64_t)tr.row0 + r].miss_t + (ch & 1) * SOLVE_SEG;
-          *reinterpret_cast<unsigned long long*>(mt + (nm & ~3)) = packq >> (16 * (4 - (nm & 3)));
-        }
-        const int cnt = nm > 0x7ffe ? 0x7ffe : nm;
-        s_nm[((lt & (NM_RING - 1)) * NGROUPS + (ch & 1)) * TILE_M + r] = static_cast<uint16_t>(cnt | (bad ? 0x8000 : 0));
+          }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc[0]);
+        wgmma_fence_regs(acc[1]);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_empty(stage));   // this warp's MMAs and smem reads of the stage are done
       }
-      tmem_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(bar_afull(grp, aslot));
-        mbar_arrive(bar_empty(stage));                  // this warp's smem reads of the stage are done
+      if (scan && (nm & 3) != 0 && nm < SOLVE_SEG) {    // flush the partial group (right-aligned: oldest first)
+        uint16_t* __restrict__ mt = a.recs[(int64_t)tr.row0 + r].miss_t + seg * SOLVE_SEG;
+        *reinterpret_cast<unsigned long long*>(mt + (nm & ~3)) = packq >> (16 * (4 - (nm & 3)));
       }
-      if (last_own) mbar_arrive(bar_nm(lt & (NM_RING - 1)));       // releases this thread's s_nm entry to the epilogue
-      stage += NGROUPS;
-      if (stage >= STAGES) { stage -= STAGES; phase ^= 1u; }
-      if (++aslot == ASLOTS) { aslot = 0; aphase ^= 1u; }
-      ch += NGROUPS;
-      while (tile < n_tiles && ch >= tr.n_chunks) {     // next tile of this CTA
-        ch -= tr.n_chunks;
-        tile += gridDim.x;
-        ++lt;
-        nm = 0;
-        tr = trn;
-        trn = tile_rec(tile + (int)gridDim.x);
-        c = c_next;
-        c_next = load_c(tile + (int)gridDim.x, trn);
-        bad = collect && !finite(c);
-        if (bad) c = 0.f;
-      }
+      // hand the tile's partial moments (hi and lo columns folded: b = D[:, p] + D[:, P + p]) to the epilogue
+      const int ab = lt & 1;
+      mbar_wait(bar_accempty(ab), ((lt >> 1) & 1) ^ 1u);  // epilogue of tile lt-2 has drained this slot
+      float* __restrict__ sacc = s_acc + (ab * NGROUPS + grp) * TILE_M * P;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const float2 v = make_float2(acc[h][4 * i + 2 * j] + acc[h][4 * (i + 2) + 2 * j],
+                                         acc[h][4 * i + 2 * j + 1] + acc[h][4 * (i + 2) + 2 * j + 1]);
+            *reinterpret_cast<float2*>(sacc + (64 * h + frow0 + 8 * j) * P + 8 * i + 2 * t4) = v;
+          }
+      const int cnt = nm > 0x7ffe ? 0x7ffe : nm;
+      s_nm[(ab * NGROUPS + seg) * TILE_M + r] = static_cast<uint16_t>(cnt | (bad ? 0x8000 : 0));
+      mbar_arrive(bar_accfull(ab));
+      gc += static_cast<uint32_t>(tr.n_chunks);
+      tile += gridDim.x;
+      tr = trn;
+      trn = tile_rec(tile + (int)gridDim.x);
+      c = c_next;
+      c_next = load_c(tile + (int)gridDim.x, trn);
     }
   } else {
     // =========================== epilogue (warps 8-11) ===========================
     const int r = threadIdx.x & 127;
-    const uint32_t lane_addr = static_cast<uint32_t>((warp & 3) * 32) << 16;
     bool vec_out = (a.n_pred % 4 == 0) && (a.ld_out % 4 == 0) && ((reinterpret_cast<uintptr_t>(a.out) & 15u) == 0);
     for (int i = 0; i + 1 < a.n_out; ++i) vec_out = vec_out && ((reinterpret_cast<uintptr_t>(a.out_more[i]) & 15u) == 0);
     // Staged epilogue: the tile's forecasts are one contiguous block of the table (rows are dense), so they are
@@ -485,34 +410,33 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
       }
       float c = (d.has_constant && live) ? centring_constant(a.y + row * a.ld_y, t_fit_c) : 0.f;   // issued before the wait
       mbar_wait(bar_accfull(ab), (lt >> 1) & 1);
-      tc_fence_after();
-      uint32_t acc[32];
-      tmem_ld_32x32b_x32(tmem_base + lane_addr + ACC_COL0 + ab * 32, acc);
-      // gaps the transform groups saw in this tile, by chunk parity
+      float g[P];
+      {
+        const float4* p0 = reinterpret_cast<const float4*>(s_acc + (ab * NGROUPS + 0) * TILE_M * P + r * P);
+        const float4* p1 = reinterpret_cast<const float4*>(s_acc + (ab * NGROUPS + 1) * TILE_M * P + r * P);
+#pragma unroll
+        for (int q = 0; q < P / 4; ++q) {
+          const float4 u = p0[q], w = p1[q];
+          g[4 * q] = u.x + w.x; g[4 * q + 1] = u.y + w.y; g[4 * q + 2] = u.z + w.z; g[4 * q + 3] = u.w + w.w;
+        }
+      }
+      // gaps the consumer warpgroups saw in this tile, by chunk parity
+      const unsigned f0 = s_nm[(ab * NGROUPS + 0) * TILE_M + r], f1 = s_nm[(ab * NGROUPS + 1) * TILE_M + r];
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_accempty(ab));     // the consumers may overwrite this slot now
       int nm0 = 0, nm1 = 0;
       bool general = false;
       if (collect) {
-        mbar_wait(bar_nm(lt & (NM_RING - 1)), (lt / NM_RING) & 1);     // acquire the transform warps' counts
-        const uint16_t* nmrow = s_nm + (lt & (NM_RING - 1)) * NGROUPS * TILE_M + r;
-        const bool has0 = true;                 // entry 0: gaps in the tile's even chunks, entry 1: in its odd chunks
-        const bool has1 = n_chunks >= 2;        // (a one-chunk calendar has no odd chunk; ragged launches: always >= 2)
-        const unsigned f0 = has0 ? nmrow[0] : 0u, f1 = has1 ? nmrow[TILE_M] : 0u;
         nm0 = f0 & 0x7fff; nm1 = f1 & 0x7fff;
         // mostly-missing rows: the downdate I - sum a a^T cancels catastrophically; fit_warp builds their Gram
         // directly over the observed rows (same rule as fit_warp.cu)
         general = ((f0 | f1) & 0x8000u) != 0u || nm0 > SOLVE_SEG || nm1 > SOLVE_SEG || 2 * (nm0 + nm1) > t_fit_c;
         if (general) c = 0.f;
       }
-      tmem_wait_ld();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_accempty(ab));     // the MMA warp may overwrite this buffer now
-      float g[P];
       bool finite = true;
 #pragma unroll
       for (int p = 0; p < P; ++p) {
-        g[p] = __uint_as_float(acc[p]) + __uint_as_float(acc[P + p]);
-        finite = finite && ((__float_as_uint(g[p]) & 0x7f800000u) != 0x7f800000u);
+        finite = finite && is_finite_bits(g[p]);
         if (!((kept_mask >> p) & 1u)) g[p] = 0.f;
       }
       const bool pend = live && (!finite || general);            // -> general warp pass
@@ -539,7 +463,7 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
           const unsigned slot = base + __popc(dm & ((1u << lane) - 1u));
           if (slot < a.rec_cap) {
             if (a.stream_ctl != nullptr) {
-              // publish: the record (this thread's moments, the transform warps' positions acquired through bar_nm) is
+              // publish: the record (this thread's moments, the consumer warps' positions acquired through bar_accfull) is
               // ordered before the work-list entry the consumer polls
               __threadfence();
               st_release_s64(a.rec_rows + slot, row);
@@ -568,7 +492,7 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
           const int64_t off = (int64_t)tr.row0 * a.n_pred;
           const uint32_t src = s_ostage_u32 + static_cast<uint32_t>(ob) * (TILE_M * BULK_MAX_PRED * 4);
           bulk_store_elect(reinterpret_cast<uint64_t>(a.out + off), src, bytes);
-          // peers: every tile starts at another peer, so at any moment this GPU's 148 store queues target all
+          // peers: every tile starts at another peer, so at any moment this GPU's store queues target all
           // peers evenly instead of all hammering the first one in the list (NVLink ingress hot spot)
           const int n_peer = a.n_out - 1;
           int j = n_peer > 1 ? tile % n_peer : 0;
@@ -624,14 +548,6 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
       }
     }
   }
-
-  // ---- teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == WARP_MMA) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
 }
 
 }  // namespace
@@ -659,12 +575,9 @@ static cudaError_t launch_variant(const DesignView& d, const FitArgs& a, const T
   return cudaGetLastError();
 }
 
-// Rows per CTA of a balanced launch (0: deal 128-row tiles round robin).  An experiment that did not pay, built only for
-// tc_variant = 3 (DESIGN.md section 6): with more than one tile per CTA the short tile costs almost a whole tile's
-// pipeline time on EVERY SM, where the round-robin deal leaves the extra tile to a few (100 k series 100.5 -> 103.7 us,
-// 125 k 113.9 -> 121.3 us); a batch of less than one wave (10 k series: 79 tiles -> 139 CTAs x 72 rows) gains 6 % when
-// steps are timed one by one (41.0 -> 38.4 us) and LOSES 30 % when they run back to back (24.0 -> 31.1 us): the idle SMs
-// of the 79-CTA launch are where the next call's kernels start.
+// Rows per CTA of a balanced launch (0: deal 128-row tiles round robin), built only for tc_variant = 3, an
+// experiment: with more than one tile per CTA the short tile costs almost a whole tile's pipeline time on EVERY SM, where
+// the round-robin deal leaves the extra tile to a few; a batch of less than one wave spreads over every SM.
 int fit_tc_balanced_rows(int64_t n, int sm_count, int variant) {
   if (variant != 3) return 0;
   const int64_t per = (n + sm_count - 1) / sm_count;
@@ -675,23 +588,21 @@ cudaError_t launch_fit_tc(const DesignView& d, const FitArgs& a, const TcLaunch&
                           int sm_count, cudaStream_t s, int variant, const MultiView* multi) {
   if (a.n <= 0) return cudaSuccess;
   if (multi != nullptr)      // ragged: the tile table names rows and calendars; d.t_pad / KC is the LONGEST calendar's count
-    return launch_variant<10, 1, true>(d, a, tl, pending_count, sm_count, s, multi->n_tiles, 2, *multi);
+    return launch_variant<8, 1, true>(d, a, tl, pending_count, sm_count, s, multi->n_tiles, 2, *multi);
   const int n_tiles = (int)((a.n + TILE_M - 1) / TILE_M);
   const int n_chunks = d.t_pad / KC;
   const MultiView none{};
-  // variant 0 / 1: ten stages, one staging tile.  The <8 stages, 2 staging tiles> instantiation (tile k+1 staged while
-  // the peer stores of tile k still read theirs) measured no faster at 2, 4 or 8 GPUs -- the multi-destination step
-  // is bound by HBM writes of the incoming copies (N = 4) and by NVLink ingress (N = 8), not by the staging tile
-  // (profiles/r02/multi_gpu.md) -- and 0.9 % slower on one GPU, so it is only built for experiments (variant 2).
+  // variant 0 / 1: eight stages, one staging tile.  Variant 2, <6 stages, 2 staging tiles> (tile k+1 staged while the
+  // peer stores of tile k still read theirs; the second tile costs two stages of the 227 KB), is built for experiments.
   const bool two = variant == 2;
   const int bal = fit_tc_balanced_rows(a.n, sm_count, variant);
   if (bal > 0) {
     MultiView b{};
     b.bal_rows = bal;
-    return launch_variant<10, 1, false, true>(d, a, tl, pending_count, sm_count, s, n_tiles, n_chunks, b);
+    return launch_variant<8, 1, false, true>(d, a, tl, pending_count, sm_count, s, n_tiles, n_chunks, b);
   }
-  return two ? launch_variant<8, 2, false>(d, a, tl, pending_count, sm_count, s, n_tiles, n_chunks, none)
-             : launch_variant<10, 1, false>(d, a, tl, pending_count, sm_count, s, n_tiles, n_chunks, none);
+  return two ? launch_variant<6, 2, false>(d, a, tl, pending_count, sm_count, s, n_tiles, n_chunks, none)
+             : launch_variant<8, 1, false>(d, a, tl, pending_count, sm_count, s, n_tiles, n_chunks, none);
 }
 
 }  // namespace mmf

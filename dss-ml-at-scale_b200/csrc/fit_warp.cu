@@ -13,7 +13,7 @@
 //   yhat_t = c + a_t . gamma                  for the requested rows, again S series per design row
 // It handles everything (NaN masks, any leading dimension, any number of prediction rows: the
 // reference's "Demand_Fitted for every date" contract, 02:484-494) and is also the masked fix-up
-// pass behind the tcgen05 kernel.  Bound: HBM; see DESIGN.md section 4.
+// pass behind the tensor-core kernel.  Bound: HBM; see DESIGN.md section 4.
 #include "mmf_internal.cuh"
 
 namespace mmf {

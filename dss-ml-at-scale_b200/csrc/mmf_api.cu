@@ -164,7 +164,7 @@ struct mmf_ctx {
                                        // eager calls, 2 belongs to captured CUDA graphs (zeroed by a node of the graph)
   int counter_set = 0;                 // set the next eager call uses
   bool set_clean[2] = {true, true};    // the set is known to be zero (cudaMemset at create, or zeroed by the previous
-                                       // eager call's tcgen05 kernel); anything else makes the call memset its set
+                                       // eager call's tensor-core kernel); anything else makes the call memset its set
   int last_set = 0;                    // set the last enqueued call used (stats read n_pending from it)
   int pinned = 0;                      // > 0: a captured CUDA graph holds pointers into the scratch below and into the plan
   bool status_scratch_captured = false;   // some capture ran without a caller-provided status buffer
@@ -321,7 +321,7 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
     a.skip_pred = 1;
   }
   const bool tc_ok = fit_tc_supported(d, a, &why);
-  if (kernel == MMF_KERNEL_TC && !tc_ok) return fail(MMF_E_UNSUPPORTED, "tcgen05 kernel not applicable: %s", why);
+  if (kernel == MMF_KERNEL_TC && !tc_ok) return fail(MMF_E_UNSUPPORTED, "tensor-core kernel not applicable: %s", why);
   if (kernel == MMF_KERNEL_AUTO) kernel = tc_ok ? MMF_KERNEL_TC : MMF_KERNEL_WARP;
   const bool may_mask = !ctx->cfg.assume_finite;
   if (may_mask) {
@@ -337,7 +337,7 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
     a.rec_rows = ctx->d_rec_rows;
     a.rec_cap = (uint32_t)cap;
   }
-  // counters: an eager call uses ping-pong set `cs`; its tcgen05 kernel zeroes the other set for the next eager
+  // counters: an eager call uses ping-pong set `cs`; its tensor-core kernel zeroes the other set for the next eager
   // call, so the common path has no memset node.  A set that is not known to be zero (first use after a warp-only
   // call, after an error, ...) is cleared explicitly.  Under stream capture the launches become a graph that is
   // replayed any number of times, interleaved with eager calls: it gets set 2, zeroed by a memset node of its own,
@@ -351,11 +351,11 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
   if (capturing || !ctx->set_clean[cs]) CU_TRY(cudaMemsetAsync(counters, 0, CTR_WORDS * sizeof(uint32_t), s));
   if (!capturing) ctx->set_clean[cs] = false;             // dirty from here on, whatever happens below
   if (kernel == MMF_KERNEL_TC && !capturing) a.zero_next = ctx->d_pending + CTR_WORDS * (cs ^ 1);
-  // Streaming solve (opt-in, mmf_config.stream_solve = 1): the series with gaps are solved WHILE the tcgen05 kernel is
+  // Streaming solve (opt-in, mmf_config.stream_solve = 1): the series with gaps are solved WHILE the tensor-core kernel is
   // still streaming (solve_stream_kernel launched right behind it with programmatic stream serialisation) instead of in
   // a pass of their own afterwards.  The work list starts out as -1; the producer publishes row indices into it.  It
-  // only overlaps when a consumer block fits beside the fit CTA on an SM, which needs the 80-register build of
-  // fit_tc_kernel -- and that build is slower than what the overlap wins (DESIGN.md section 6b), so it is off by default.
+  // only overlaps when a consumer block fits beside the fit CTA on an SM, which the fit kernel's register and shared
+  // memory use (one CTA per SM) does not leave room for, so it is off by default.
   const bool stream_solve = kernel == MMF_KERNEL_TC && may_mask && !capturing && n >= 32768 && ctx->cfg.stream_solve == 1;
   if (stream_solve) {
     if (!ctx->rec_rows_clean) CU_TRY(cudaMemsetAsync(ctx->d_rec_rows, 0xFF, ctx->rec_rows_cap_bytes, s));
@@ -401,7 +401,7 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
     PredictLaunch pl;
     memcpy(pl.tmap_bhi, ctx->plan.tmap_bhi, 128);
     memcpy(pl.tmap_blo, ctx->plan.tmap_blo, 128);
-    int rc = encode_2d(pl.tmap_out, out, (uint64_t)n_pred, (uint64_t)n, (uint64_t)ld_out * 4, 32, 128);
+    int rc = encode_2d(pl.tmap_out, out, (uint64_t)n_pred, (uint64_t)n, (uint64_t)ld_out * 4, 32, 64);   // one box per warpgroup half
     if (rc != MMF_OK) return rc;
     CU_TRY(launch_predict_tc(d, a, pl, ctx->sm_count, s));
     ++*launches;
@@ -409,7 +409,7 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
   *kernel_used = kernel;
   ctx->last_set = cs;
   if (!capturing) {                                       // toggle only once every launch of the call is enqueued
-    ctx->set_clean[cs ^ 1] = (kernel == MMF_KERNEL_TC);   // zeroed by this call's tcgen05 kernel
+    ctx->set_clean[cs ^ 1] = (kernel == MMF_KERNEL_TC);   // zeroed by this call's tensor-core kernel
     ctx->counter_set = cs ^ 1;
   }
   return MMF_OK;
@@ -510,8 +510,8 @@ int mmf_create(const mmf_config* cfg, mmf_ctx** out) {
   cudaDeviceProp prop;
   if ((e = cudaGetDeviceProperties(&prop, dev)) != cudaSuccess) return bail(e, "cudaGetDeviceProperties");
   ctx->sm_count = prop.multiProcessorCount;
-  if (prop.major != 10) {
-    int rc = fail(MMF_E_UNSUPPORTED, "device %d is sm_%d%d; libmmf is built for sm_100a (B200) only", dev, prop.major,
+  if (prop.major != 9 || prop.minor != 0) {
+    int rc = fail(MMF_E_UNSUPPORTED, "device %d is sm_%d%d; libmmf is built for sm_90a (H100) only", dev, prop.major,
                   prop.minor);
     delete ctx;
     return rc;
@@ -752,10 +752,8 @@ static int fit_forecast_impl(mmf_ctx* ctx, const void* y_any, int32_t dtype, int
       if (want <= 0) {
         cpu_set_t set;
         const int have = (sched_getaffinity(0, sizeof(set), &set) == 0) ? CPU_COUNT(&set) : (int)std::thread::hardware_concurrency();
-        // measured on the 2 x 32-core host of the B200 box (64 logical CPUs local to the GPU): 8 / 16 / 24 / 32 / 48
-        // threads -> 78.8 / 55.7 / 65.2 / 84.7 / 124.6 ms per 1 M x 1,095 step (79 ms without narrowing): past ~16
-        // streaming threads the copy engine's reads of the same memory controllers slow down more than the
-        // conversion speeds up (profiles/r02/README.md)
+        // past ~16 streaming threads the copy engine's reads of the same memory controllers slow down more than the
+        // conversion speeds up
         want = std::max(1, std::min(16, have / 2));
       }
       int ndev_vis = 0;
@@ -764,17 +762,14 @@ static int fit_forecast_impl(mmf_ctx* ctx, const void* y_any, int32_t dtype, int
       if (const char* e = getenv("MMF_HOST_PIN")) pin = atoi(e) != 0;
       ctx->narrow_pool = narrow_pool_create(want - 1, pin);    // the calling thread is the last worker
     }
-    // rows per narrowed sub-chunk and store flavour: measured on the B200 box (16 threads, 1 M x 1,095 per step; float32
-    // copies: 82.4 ms): 1,024 / 2,048 / 4,096 / 8,192 / 32,768 rows with ordinary stores 84.6 / 81.6 / 75.1 / 62.2 /
-    // 63.9 ms, streaming stores 67.1 ms at 4,096 and 63.6 ms at 32,768 -- keeping the slots cache resident (small
-    // sub-chunks, ordinary stores) does not pay for the extra copies and synchronisations; 8,192 rows it is
+    // rows per narrowed sub-chunk and store flavour: keeping the slots cache resident (small sub-chunks, ordinary stores)
+    // does not pay for the extra copies and synchronisations
     int64_t sub_rows = 8192;
     bool stream_stores = true;
     if (const char* e = getenv("MMF_HOST_SUB_ROWS")) sub_rows = std::max<int64_t>(64, atoll(e));   // tuning / experiments
     if (const char* e = getenv("MMF_HOST_STREAM_STORES")) stream_stores = atoi(e) != 0;
     sub_rows = std::min(sub_rows, chunk);
-    // measured (one B200 box, 16 narrowing threads, 1 M x 1,095 per step; float32 copies 82.4 ms): never / every 8th /
-    // 6th / 5th / 4th / 3rd / 2nd chunk direct -> 66.5 / 63.7 / 62.5 / 61.5 / 59.5 / 57.9 / 61.3 ms
+    // every third chunk goes over PCIe as float32 without narrowing: the copy engine and the narrowing threads share the load
     int direct_every = 3;
     if (const char* e = getenv("MMF_HOST_DIRECT_EVERY")) direct_every = atoi(e);
     if (narrow) {
@@ -954,7 +949,7 @@ int mmf_plan_calendars(mmf_ctx* ctx, const double* X_all, int32_t n_cal, const i
   if (n_cal < 1 || n_cal > 65535) return fail(MMF_E_INVALID, "n_cal=%d outside [1,65535]", n_cal);
   if (p < 1 || p > P) return fail(MMF_E_INVALID, "p=%d outside [1,%d]", p, P);
   // one common number of prediction rows <= 64: the forecasts are written by the fit kernel's own epilogue; anything
-  // else (holdout: every date of every calendar) goes through the tcgen05 predict kernel
+  // else (holdout: every date of every calendar) goes through the tensor-core predict kernel
   bool many = false;
   int32_t n_pred = n_pred_cal[0], n_pred_max = 0;
   for (int c = 0; c < n_cal; ++c) {
@@ -1111,7 +1106,7 @@ int mmf_fit_forecast_ragged_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t
       const int64_t r0 = cal_row_start[c], nr = cal_row_start[c + 1] - r0;
       if (nr <= 0) { memset(omaps.data() + (size_t)c * 128, 0, 128); continue; }
       int rc = encode_2d(omaps.data() + (size_t)c * 128, out_pred + r0 * ld_out, (uint64_t)cm.n_pred, (uint64_t)nr,
-                         (uint64_t)ld_out * 4, 32, 128);
+                         (uint64_t)ld_out * 4, 32, 64);
       if (rc != MMF_OK) return rc;
       const int n_ch = (cm.n_pred + 127) / 128;
       for (int64_t r = r0; r < r0 + nr; r += 128)

@@ -13,8 +13,8 @@ constexpr int NPAIR = P * (P + 1) / 2;   // packed symmetric Gram entries (136)
 // A = X W (whitened, float32).  Three layouts of the same numbers:
 //  a4   : column-blocked float4, a4[j*n_rows_pad + t] = A[t][4j..4j+3]   (warp kernel: conflict-free LDS.128)
 //  at   : [2P][t_pad] K-major rows for the tensor-core B operand: row n<P is tf32-hi of column n,
-//         row P+n is the tf32 residual (lo); columns t >= t_fit are zero            (tcgen05 kernel)
-//  apred: [n_rows][P] row-major                                                     (tcgen05 epilogue)
+//         row P+n is the tf32 residual (lo); columns t >= t_fit are zero            (tensor-core kernel)
+//  apred: [n_rows][P] row-major                                                     (wgmma epilogue)
 struct DesignView {
   const float4* a4;
   const float*  at;
@@ -35,7 +35,7 @@ struct DesignView {
 // tile's calendar from the table instead of from launch constants.
 struct CalMeta {                           // one calendar of a ragged plan (32 B)
   int32_t t_fit;
-  int32_t n_chunks;                        // ceil(t_fit / 32): 32-step chunks of the tcgen05 kernel
+  int32_t n_chunks;                        // ceil(t_fit / 32): 32-step chunks of the tensor-core kernel
   int32_t n_rows;                          // design rows planned (fit + forecast rows)
   uint32_t kept_mask;                      // whitened columns retained on this calendar
   int32_t row_off;                         // first row of this calendar in the stacked apred / ap_hi / ap_lo / a4 tables
@@ -62,7 +62,7 @@ struct MultiView {                         // all null / 0 for an ordinary singl
 
 // One series with gaps, handed to the thread-per-series solve kernel (256 B, indexed by row).
 // Missing grid positions come in two segments so that two producers (the two transform groups of the
-// tcgen05 kernel) can append without atomics: segment g holds nm[g] entries at miss_t[g*SOLVE_SEG ...].
+// tensor-core kernel) can append without atomics: segment g holds nm[g] entries at miss_t[g*SOLVE_SEG ...].
 // Segments are a multiple of 4 entries and 8-B aligned: the solve kernel reads the positions four at a time.
 constexpr int SOLVE_SEG = 44;
 constexpr int SOLVE_MISS_CAP = 2 * SOLVE_SEG;
@@ -102,9 +102,9 @@ struct FitArgs {
   uint32_t rec_cap;         //   == n
   int32_t only_pending;     // 1: process only rows whose status == MMF_STATUS_PENDING
   const uint32_t* pending_count;  // nullable; if non-null and *pending_count == 0 the kernel exits at once
-  uint32_t* zero_next;      // nullable: 2 counters of the NEXT call's set, zeroed by the tcgen05 kernel (no memset node)
+  uint32_t* zero_next;      // nullable: 2 counters of the NEXT call's set, zeroed by the tensor-core kernel (no memset node)
   uint32_t* stream_ctl;     // nullable: {claimed, CTAs finished, producer done} of the streaming solve (solve_stream_kernel
-                            // consumes the queued records WHILE the tcgen05 kernel is still producing them)
+                            // consumes the queued records WHILE the tensor-core kernel is still producing them)
   int64_t row_base;         // ragged fallback launches cover one calendar's rows: absolute row of this launch's row 0
   int32_t cal_id;           //   ... and that calendar's index (written into the records the launch queues)
 };
@@ -124,7 +124,7 @@ cudaError_t launch_solve_stream(const DesignView& d, const FitArgs& a, int sm_co
 constexpr int CTR_WORDS = 8;             // one counter set: {pending, records queued, claimed, CTAs finished, producer done, -, -, -}
 
 // fitted values + forecasts for MANY prediction rows (the reference's "Demand_Fitted for every date"
-// contract, 02:484-494): out[n, n_pred] = c + gamma A_pred^T as a tcgen05 GEMM with TMA-stored tiles
+// contract, 02:484-494): out[n, n_pred] = c + gamma A_pred^T as a wgmma GEMM with TMA-stored tiles
 struct PredictLaunch {
   alignas(64) unsigned char tmap_bhi[128];
   alignas(64) unsigned char tmap_blo[128];
@@ -143,7 +143,7 @@ cudaError_t launch_predict_tc(const DesignView& d, const FitArgs& a, const Predi
                               cudaStream_t s, const PredUnit* units = nullptr, int64_t n_units_multi = 0,
                               const unsigned char* tmaps_out = nullptr);
 
-// TMA + tcgen05/TMEM kernel (fully observed fast path).  `tmap_y` / `tmap_at` are CUtensorMap blobs.
+// TMA + wgmma kernel (fully observed fast path).  `tmap_y` / `tmap_at` are CUtensorMap blobs.
 struct TcLaunch {
   alignas(64) unsigned char tmap_y[128];    // box {32 t, 128 series}
   alignas(64) unsigned char tmap_at[128];

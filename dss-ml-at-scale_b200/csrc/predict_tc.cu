@@ -3,42 +3,44 @@
 // The reference's per-group UDF returns Demand_Fitted for EVERY date of the group (in-sample fits for the train
 // dates + the forecast for the held-out dates, group_apply/02_Fine_Grained_Demand_Forecasting.py:484-494).  With
 // T dates per series that is as many bytes out as the fit read in, and 16 FMAs per output element -- too much for
-// the CUDA cores at HBM speed, so it is a second tcgen05 GEMM, the mirror image of fit_tc.cu:
-//   A operand  gamma tile [128 series x 16] (fp32 split hi/lo, written once per tile with tcgen05.st)  -> TMEM
+// the CUDA cores at HBM speed, so it is a second tensor-core GEMM, the mirror image of fit_tc.cu:
+//   A operand  gamma tile [128 series x 16] (fp32 split hi/lo, m16n8k8 register fragments)
 //   B operand  prediction rows of the whitened design, [128 t x 16] K-major tiles (hi and lo), TMA, 64-B swizzle
-//   D          [128 series x 128 t] fp32 in TMEM, double buffered:  hi*Bhi + hi*Blo + lo*Bhi  (fp32-grade)
-//   epilogue   two warp groups on alternate chunks (one per accumulator / staging buffer): tcgen05.ld -> + c ->
-//              128-B-swizzled shared tiles -> TMA 2-D stores (clipped at n / n_pred)
+//   D          [64 series x 128 t] fp32 per warpgroup (registers):  hi*Bhi + hi*Blo + lo*Bhi  (fp32-grade)
+//   epilogue   each warpgroup owns one 64-row half of every tile: D + c -> 128-B-swizzled shared tiles (double
+//              buffered) -> TMA 2-D stores (clipped at n / n_pred)
 // Bound: HBM writes, 4*n_pred bytes per series (DESIGN.md section 4).
 #include "mmf_internal.cuh"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace mmf {
 namespace {
 
-using namespace sm100;
+using namespace sm90;
 
-constexpr int TILE_M = 128;                   // series per tile == TMEM lanes
+constexpr int TILE_M = 128;                   // series per tile
+constexpr int WG_M = 64;                      // series per warpgroup (one wgmma M)
 constexpr int TN = 128;                       // prediction rows per chunk == D columns
 constexpr int SB = 3;                         // B-operand stages
 constexpr int B_TILE_BYTES = TN * P * 4;      // 8192 (hi) ; same for lo
 constexpr int B_STAGE_BYTES = 2 * B_TILE_BYTES;
-constexpr int OUT_SUB_BYTES = TILE_M * 32 * 4;          // one {32 t x 128 series} store box: 16384
-constexpr int OUT_STAGE_BYTES = (TN / 32) * OUT_SUB_BYTES;   // 65536
-constexpr int THREADS = 448;
-constexpr int WARP_LOAD0 = 8, WARP_PROD = 12, WARP_MMA = 13;     // warps 0-3 / 4-7: two epilogue groups
-constexpr uint32_t TMEM_COLS = 512;
-constexpr uint32_t D_COL0 = 0;                // 2 x 128 accumulator columns
-constexpr uint32_t A_COL0 = 256;              // 2 x (16 hi + 16 lo)
+constexpr int OUT_SUB_BYTES = WG_M * 32 * 4;            // one {32 t x 64 series} store box: 8192
+constexpr int OUT_BUF_BYTES = (TN / 32) * OUT_SUB_BYTES;     // 32768
+constexpr int THREADS = 288;
+constexpr int WARP_PROD = 8;                  // warps 0-3 / 4-7: the two warpgroups
 
 struct Smem {
   static constexpr int b = 0;
-  static constexpr int out = b + SB * B_STAGE_BYTES;                // 24576
-  static constexpr int bars = out + 2 * OUT_STAGE_BYTES;            // + 131072
-  static constexpr int n_bars = 2 * SB + 4 + 4;
-  static constexpr int tmem_ptr = bars + n_bars * 8;
-  static constexpr int total = tmem_ptr + 16;
+  static constexpr int out = b + SB * B_STAGE_BYTES;                // 49152
+  static constexpr int bars = out + 2 * 2 * OUT_BUF_BYTES;          // + 2 warpgroups x 2 buffers
+  static constexpr int n_bars = 2 * SB;
+  static constexpr int total = bars + n_bars * 8;
+  static_assert(total + 1024 <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into");
 };
+
+__device__ __forceinline__ void sts64(uint32_t addr, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
+}
 
 // MULTI: a ragged batch (mmf_fit_forecast_ragged_f32, holdout-style requests): the work units come from a table
 // (rows, calendar, chunk of THAT calendar's prediction rows, first row of the chunk in the stacked design table) and the
@@ -68,43 +70,26 @@ predict_tc_kernel(const __grid_constant__ PredictLaunch pl, const DesignView d, 
   const uint32_t s_bars = sbase + Smem::bars;
   auto bar_bfull = [&](int s) { return s_bars + 8u * s; };
   auto bar_bempty = [&](int s) { return s_bars + 8u * (SB + s); };
-  auto bar_afull = [&](int i) { return s_bars + 8u * (2 * SB + i); };
-  auto bar_aempty = [&](int i) { return s_bars + 8u * (2 * SB + 2 + i); };
-  auto bar_dfull = [&](int i) { return s_bars + 8u * (2 * SB + 4 + i); };
-  auto bar_dempty = [&](int i) { return s_bars + 8u * (2 * SB + 6 + i); };
-  volatile uint32_t* tmem_ptr_smem = reinterpret_cast<volatile uint32_t*>(smem + Smem::tmem_ptr);
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == WARP_MMA) {
-    if (lane == 0) {
-      for (int s = 0; s < SB; ++s) { mbar_init(bar_bfull(s), 1); mbar_init(bar_bempty(s), 1); }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(bar_afull(i), 4);    // 4 loader warps
-        mbar_init(bar_aempty(i), 1);   // tcgen05.commit after the tile's last chunk
-        mbar_init(bar_dfull(i), 1);    // tcgen05.commit per chunk
-        mbar_init(bar_dempty(i), 4);   // 4 epilogue warps
-      }
-      fence_mbar_init();
+  if (warp == WARP_PROD && lane == 0) {
+    for (int s = 0; s < SB; ++s) {
+      mbar_init(bar_bfull(s), 1);
+      mbar_init(bar_bempty(s), 8);     // the 8 MMA warps, after their MMAs have retired
     }
-    __syncwarp();
-    tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_ptr_smem)), TMEM_COLS);
-    tmem_relinquish();
-  } else if (warp == WARP_PROD && lane == 0) {
+    fence_mbar_init();
     prefetch_tensormap(pl.tmap_bhi);
     prefetch_tensormap(pl.tmap_blo);
     prefetch_tensormap(pl.tmap_out);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   if (warp == WARP_PROD) {
     // =========================== TMA producer: design rows of the prediction window ===========================
     // Work units are (tile, chunk) pairs in chunk-major order, dealt round-robin to the CTAs: at any moment the
     // CTAs with neighbouring ids write neighbouring 512-B pieces of the SAME 128 rows, i.e. one contiguous region
-    // of the table, instead of 148 unrelated row sets (DRAM write locality).
+    // of the table, instead of unrelated row sets (DRAM write locality).
     int stage = 0;
     uint32_t phase = 0;
     for (int64_t u = blockIdx.x; u < n_units; u += gridDim.x) {
@@ -115,129 +100,80 @@ predict_tc_kernel(const __grid_constant__ PredictLaunch pl, const DesignView d, 
                            s_b + stage * B_STAGE_BYTES + B_TILE_BYTES, pl.tmap_blo, 0, t0, L2_EVICT_LAST);
       if (++stage == SB) { stage = 0; phase ^= 1u; }
     }
-  } else if (warp == WARP_MMA) {
-    // =========================== MMA issuer ===========================
-    constexpr uint32_t IDESC = umma_idesc_tf32(TILE_M, TN);
+  } else {
+    // =========================== warpgroups: gamma fragments -> wgmma -> + c -> swizzled tiles -> TMA store ===========
+    const int wg = warp >> 2;                              // rows 64*wg .. 64*wg + 63 of every tile
+    const int g8 = lane >> 2, t4 = lane & 3;
+    const int frow = 16 * (warp & 3) + g8;                 // fragment rows frow, frow + 8 of the warpgroup's 64
+    const bool leader = (warp & 3) == 0;
     int stage = 0;
     uint32_t phase = 0;
-    int64_t k = 0;                                         // this CTA's unit counter: A / D buffer = k & 1
+    int64_t k = 0;                                         // this CTA's unit counter: staging buffer k & 1
     for (int64_t u = blockIdx.x; u < n_units; u += gridDim.x, ++k) {
-      const int ab = (int)(k & 1);
-      const uint32_t par = (uint32_t)((k >> 1) & 1);
-      mbar_wait(bar_afull(ab), par);
+      const PredUnit pu = unit_at(u);
+      uint32_t ahi[2][4], alo[2][4];                       // [k-step][fragment register]
+      float c[2];
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int rl = WG_M * wg + frow + 8 * j;
+        const bool live = rl < pu.nrows;
+        const float* __restrict__ gp = a.out_gamma + ((int64_t)pu.row0 + rl) * P;
+        c[j] = live ? __ldg(a.out_c + pu.row0 + rl) : 0.f;
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk)
+#pragma unroll
+          for (int hf = 0; hf < 2; ++hf) {
+            const float gv = live ? __ldg(gp + 8 * kk + 4 * hf + t4) : 0.f;
+            const uint32_t h = __float_as_uint(gv) & 0xFFFFE000u;
+            ahi[kk][j + 2 * hf] = h;
+            alo[kk][j + 2 * hf] = __float_as_uint(gv - __uint_as_float(h));
+          }
+      }
+      float acc[TN / 2];
+#pragma unroll
+      for (int i = 0; i < TN / 2; ++i) acc[i] = 0.f;
       mbar_wait(bar_bfull(stage), phase);
-      mbar_wait(bar_dempty(ab), par ^ 1u);
-      tc_fence_after();
-      const uint32_t a_hi = tmem_base + A_COL0 + ab * 32;
-      const uint32_t a_lo = a_hi + 16;
-      const uint64_t bhi = umma_desc_k_sw64(s_b + stage * B_STAGE_BYTES);
-      const uint64_t blo = umma_desc_k_sw64(s_b + stage * B_STAGE_BYTES + B_TILE_BYTES);
-      const uint32_t dcol = tmem_base + D_COL0 + ab * TN;
+      const uint64_t bhi = gmma_desc_k_sw64(s_b + stage * B_STAGE_BYTES);
+      const uint64_t blo = gmma_desc_k_sw64(s_b + stage * B_STAGE_BYTES + B_TILE_BYTES);
+      wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < 2; ++kk) {
-        umma_tf32_ts_elect(dcol, a_hi + kk * 8, bhi + static_cast<uint64_t>(kk * 2), IDESC, kk ? 1u : 0u);
-        umma_tf32_ts_elect(dcol, a_hi + kk * 8, blo + static_cast<uint64_t>(kk * 2), IDESC, 1u);
-        umma_tf32_ts_elect(dcol, a_lo + kk * 8, bhi + static_cast<uint64_t>(kk * 2), IDESC, 1u);
+        wgmma_m64n128k8_tf32_rs(acc, ahi[kk], bhi + static_cast<uint64_t>(kk * 2));
+        wgmma_m64n128k8_tf32_rs(acc, ahi[kk], blo + static_cast<uint64_t>(kk * 2));
+        wgmma_m64n128k8_tf32_rs(acc, alo[kk], bhi + static_cast<uint64_t>(kk * 2));
       }
-      umma_commit_elect(bar_bempty(stage));
-      umma_commit_elect(bar_dfull(ab));
-      umma_commit_elect(bar_aempty(ab));
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_bempty(stage));      // design tile free for the producer
       if (++stage == SB) { stage = 0; phase ^= 1u; }
-    }
-  } else if (warp >= WARP_LOAD0) {
-    // =========================== gamma loaders (warps 8-11): one tcgen05.st pair per tile ===========================
-    const int r = threadIdx.x & 127;
-    const uint32_t lane_addr = static_cast<uint32_t>((warp & 3) * 32) << 16;
-    int64_t k = 0;
-    for (int64_t u = blockIdx.x; u < n_units; u += gridDim.x, ++k) {
-      const int ab = (int)(k & 1);
-      const int lt = (int)k;
-      const PredUnit pu = unit_at(u);
-      const int64_t row = (int64_t)pu.row0 + r;
-      float g[P];
-      if (r < pu.nrows) {
-        const float4* gp = reinterpret_cast<const float4*>(a.out_gamma + row * P);
+
+      const uint32_t obase = s_out + static_cast<uint32_t>(wg * 2 + (int)(k & 1)) * OUT_BUF_BYTES;
+      if (leader) bulk_wait_read1_elect();                 // the stores of unit k - 2 have read this buffer
+      named_bar_sync(1 + wg, 128);
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float4 v = __ldg(gp + q);
-          g[4 * q] = v.x; g[4 * q + 1] = v.y; g[4 * q + 2] = v.z; g[4 * q + 3] = v.w;
-        }
-      } else {
+      for (int i = 0; i < TN / 8; ++i) {                   // n8 block i: columns 8i + 2t4, +1 of rows frow, frow + 8
+        const uint32_t q = static_cast<uint32_t>(2 * (i & 3) + (t4 >> 1));
+        const uint32_t col = obase + (i >> 2) * OUT_SUB_BYTES + ((q ^ static_cast<uint32_t>(g8)) << 4) + (t4 & 1) * 8;
 #pragma unroll
-        for (int p = 0; p < P; ++p) g[p] = 0.f;
+        for (int j = 0; j < 2; ++j)
+          sts64(col + static_cast<uint32_t>(frow + 8 * j) * 128u, acc[4 * i + 2 * j] + c[j], acc[4 * i + 2 * j + 1] + c[j]);
       }
-      uint32_t hi[P], lo[P];
-#pragma unroll
-      for (int p = 0; p < P; ++p) {
-        const uint32_t h = __float_as_uint(g[p]) & 0xFFFFE000u;
-        hi[p] = h;
-        lo[p] = __float_as_uint(g[p] - __uint_as_float(h));
-      }
-      mbar_wait(bar_aempty(ab), ((lt >> 1) & 1) ^ 1u);
-      tc_fence_after();
-      const uint32_t acol = tmem_base + lane_addr + A_COL0 + ab * 32;
-      tmem_st_32x32b_x16(acol, hi);
-      tmem_st_32x32b_x16(acol + 16, lo);
-      tmem_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_afull(ab));
-    }
-  } else {
-    // =========================== epilogue groups (warps 0-3 / 4-7): D -> + c -> swizzled tiles -> TMA store ===========
-    // group g owns accumulator buffer g, staging buffer g and every chunk of the CTA's stream with parity g
-    const int grp = warp >> 2;
-    const int r = threadIdx.x & 127;
-    const uint32_t lane_addr = static_cast<uint32_t>((warp & 3) * 32) << 16;
-    const uint32_t row_off = static_cast<uint32_t>(r) * 128u;
-    const uint32_t sw = static_cast<uint32_t>(r & 7);
-    const uint32_t obase = s_out + grp * OUT_STAGE_BYTES;
-    const bool leader = (warp & 3) == 0;
-    int64_t k = 0;                                         // unit counter: group g owns the units with k & 1 == g
-    for (int64_t u = blockIdx.x; u < n_units; u += gridDim.x, ++k) {
-      if ((int)(k & 1) != grp) continue;
-      const PredUnit pu = unit_at(u);
-      const int64_t row = (int64_t)pu.row0 + r;
-      const float c = (r < pu.nrows) ? __ldg(a.out_c + row) : 0.f;
-      mbar_wait(bar_dfull(grp), (uint32_t)((k >> 1) & 1));
-      tc_fence_after();
-      if (leader) bulk_wait_read_elect();                  // this group's previous stores have read the staging tile
-      named_bar_sync(1 + grp, 128);
-#pragma unroll
-      for (int j = 0; j < TN / 32; ++j) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_base + lane_addr + D_COL0 + grp * TN + j * 32, v);
-        tmem_wait_ld();
-        const uint32_t rowp = obase + j * OUT_SUB_BYTES + row_off;
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const float4 o = make_float4(__uint_as_float(v[4 * q]) + c, __uint_as_float(v[4 * q + 1]) + c,
-                                       __uint_as_float(v[4 * q + 2]) + c, __uint_as_float(v[4 * q + 3]) + c);
-          sts128(rowp + ((static_cast<uint32_t>(q) ^ sw) << 4), o);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_dempty(grp));        // accumulator buffer free for the MMA warp
       fence_proxy_async_smem();
-      named_bar_sync(1 + grp, 128);
+      named_bar_sync(1 + wg, 128);
       if (leader) {
-        const void* tmo = MULTI ? static_cast<const void*>(tmaps_out + (size_t)pu.cal * 128) : static_cast<const void*>(pl.tmap_out);
-        if (MULTI) fence_tensormap_acquire(tmo);
+        if (WG_M * wg < pu.nrows) {
+          const void* tmo = MULTI ? static_cast<const void*>(tmaps_out + (size_t)pu.cal * 128) : static_cast<const void*>(pl.tmap_out);
+          if (MULTI) fence_tensormap_acquire(tmo);
 #pragma unroll
-        for (int j = 0; j < TN / 32; ++j)
-          tma_store_2d_elect(tmo, obase + j * OUT_SUB_BYTES, pu.ch * TN + j * 32, pu.row_in_map);
+          for (int j = 0; j < TN / 32; ++j)
+            tma_store_2d_elect(tmo, obase + j * OUT_SUB_BYTES, pu.ch * TN + j * 32, pu.row_in_map + WG_M * wg);
+        }
         bulk_commit_elect();
       }
     }
     if (leader) bulk_wait_all_elect();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == WARP_MMA) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
   }
 }
 

@@ -41,7 +41,7 @@ select_kernel(const DesignView d, const FitArgs a, const SelectArgs sel) {
     // partial sum IS the prediction of the model made of columns 0..p, so each held-out row costs 16 FMAs for the
     // predictions and 16 for the squared errors of all 16 prefix lengths (statically indexed registers); the
     // candidates' scores are picked out of those 16 at the end.  (Testing every column against every candidate
-    // inside the loop made this kernel issue-bound at ~4x the instructions: profiles/r02/ncu_select.txt.)
+    // inside the loop made this kernel issue-bound at ~4x the instructions.)
     float sse[P];
 #pragma unroll
     for (int p = 0; p < P; ++p) sse[p] = 0.f;

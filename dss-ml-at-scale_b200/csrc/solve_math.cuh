@@ -12,10 +12,9 @@ namespace mmf {
 
 __device__ __forceinline__ constexpr int tri(int i, int j) { return i * (i + 1) / 2 + j; }   // i >= j
 
-__device__ __forceinline__ void ldg256_nc(const float* p, float4& lo, float4& hi) {      // p: 32-B aligned
-  asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(lo.x), "=f"(lo.y), "=f"(lo.z), "=f"(lo.w), "=f"(hi.x), "=f"(hi.y), "=f"(hi.z), "=f"(hi.w)
-               : "l"(p));
+__device__ __forceinline__ void ldg32b_nc(const float* p, float4& lo, float4& hi) {      // p: 32-B aligned (one sector)
+  lo = __ldg(reinterpret_cast<const float4*>(p));
+  hi = __ldg(reinterpret_cast<const float4*>(p) + 1);
 }
 
 // b (moments over the observed rows) -> gamma, in place.  `load_group(seg, gi)` returns the gi-th 8-B group of four
@@ -30,11 +29,11 @@ __device__ __forceinline__ unsigned masked_solve(const DesignView& d, float (&b)
   for (int j = 0; j < P; ++j) G[tri(j, j)] = ((d.kept_mask >> j) & 1u) ? 1.f : 0.f;
   // software-pipelined: gap positions arrive four at a time (one 8-B load, two groups ahead) and the design row
   // of the next gap is in flight while the 136 FMAs of the current one issue.  Every lane gathers a different
-  // 64-B design row: two 256-bit loads (one 32-B sector each) instead of four LDG.128.
+  // 64-B design row (two 32-B sectors).
   auto design_row = [&](int t, float4& r0, float4& r1, float4& r2, float4& r3) {
     const float* ap = d.apred + (size_t)t * P;
-    ldg256_nc(ap, r0, r1);
-    ldg256_nc(ap + 8, r2, r3);
+    ldg32b_nc(ap, r0, r1);
+    ldg32b_nc(ap + 8, r2, r3);
   };
   // (one flat loop over both segments, to pay the warp's max-over-lanes trip count once, measured slower:
   //  the segment-switch bookkeeping costs more issue slots than the shorter trip count saves)

@@ -25,7 +25,7 @@ __device__ __forceinline__ float widen_one(T x) {
 
 // 8 values per 16-B (int16) / 32-B (int32) load, two 16-B stores.  A 64-thread quarter of the block owns a row at a time
 // and strides over its groups of 8 (no integer division per element: the first version computed row = i / groups in 64
-// bits for every group and ran at 1.3 TB/s whatever the unrolling, profiles/r02/ncu_widen*.txt); the loads of a row are
+// bits for every group and ran at 1.3 TB/s whatever the unrolling); the loads of a row are
 // issued before its stores.  Rows are walked with a pitch, so a group never straddles a row; the tail of a row (t % 8)
 // takes the scalar path.
 constexpr int QUART = 64;                      // threads per row

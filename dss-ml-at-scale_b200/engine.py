@@ -107,7 +107,7 @@ def release_pinned_pool() -> None:
 
 def device_packed(y, device="cuda"):
     """Copy packed series (NumPy [n,t] or torch) into a CUDA tensor whose row pitch is a multiple of
-    4 floats -- the layout the TMA/tcgen05 fast path needs.  Returns the [n, t] view."""
+    4 floats -- the layout the TMA/wgmma fast path needs.  Returns the [n, t] view."""
     import torch
 
     src = torch.from_numpy(np.ascontiguousarray(y)) if isinstance(y, np.ndarray) else y
@@ -249,7 +249,7 @@ class ForecastEngine:
         ``mode="future"``: every series is fit on its whole history and forecast ``horizon`` rows past its end;
         ``mode="holdout"`` (the reference's contract, 02:372-380 + 484-494): the last ``horizon`` rows are held out and a
         value is produced for EVERY date of the calendar.  One host call whitens every calendar (``mmf_plan_calendars``);
-        ``fit_forecast_ragged`` then fits all groups in one pass of the tcgen05 kernel (+ one of the predict kernel in
+        ``fit_forecast_ragged`` then fits all groups in one pass of the tensor-core kernel (+ one of the predict kernel in
         holdout mode).  Returns the prediction dates per calendar: ``[n_cal, horizon]`` datetime64[D] (future) or a list
         of ``t_lens[c]``-long arrays (holdout)."""
         starts = [np.datetime64(s, "D") for s in starts]

@@ -298,7 +298,7 @@ RAGGED_MIN_BUCKETS = 2        # from this many calendars on, a batch goes throug
 def _fit_buckets_ragged(buckets, eng, freq, horizon, mode, design, on_device):
     """All calendars of the batch in one launch (``mmf_plan_calendars`` + ``mmf_fit_forecast_ragged_f32``): the groups'
     rows are laid out calendar after calendar in one device buffer, each calendar's design is whitened in the same
-    host call, and one pass of the tcgen05 kernel fits every group against its own calendar (02:422-423 per group);
+    host call, and one pass of the tensor-core kernel fits every group against its own calendar (02:422-423 per group);
     in holdout mode one pass of the predict kernel then writes a value for every date of every group (02:484-494)."""
     import torch
 

@@ -3,9 +3,9 @@
 The reference spreads groups with ``repartition(n_tasks, "Product", "SKU")`` -- a hash
 shuffle of the key columns -- and then runs one task per group
 (group_apply/02_Fine_Grained_Demand_Forecasting.py:520-528).  Groups are independent, so
-the B200 analogue is: ``owner = hash(key) mod world_size`` at pack time, every rank fits
+the H100 analogue is: ``owner = hash(key) mod world_size`` at pack time, every rank fits
 its own series (no data-path collective), and exactly one ``all_gather`` of the
-``[per_rank, n_pred]`` float32 forecast table over NCCL (NVLink 5 / NVSwitch) gives every
+``[per_rank, n_pred]`` float32 forecast table over NCCL (NVLink / NVSwitch) gives every
 rank the whole table.  One process per GPU; ``torch.distributed`` is the plumbing.
 """
 from __future__ import annotations

@@ -1,5 +1,5 @@
 /*
- * mmf.h -- C ABI of libmmf.so, the B200-native many-models fit+forecast engine.
+ * mmf.h -- C ABI of libmmf.so, the H100-native many-models fit+forecast engine.
  *
  * This is the drop-in boundary for ONE hot path of sebrahimi1988/dss-ml-at-scale:
  * the per-(Product,SKU) fit + predict that the reference fans out with
@@ -58,9 +58,9 @@ extern "C" {
 #define MMF_DT_I32 3             /* int32,   INT32_MIN   = missing; exact for |v| < 2^24  */
 
 /* kernel selection */
-#define MMF_KERNEL_AUTO 0        /* tcgen05 fast path + masked fix-up where eligible, else warp kernel */
+#define MMF_KERNEL_AUTO 0        /* tensor-core fast path + masked fix-up where eligible, else warp kernel */
 #define MMF_KERNEL_WARP 1        /* warp-per-series CUDA-core kernel (general: masks, any ld, any n_pred) */
-#define MMF_KERNEL_TC 2          /* TMA + tcgen05/TMEM kernel (fully observed rows; others -> masked pass) */
+#define MMF_KERNEL_TC 2          /* TMA + wgmma kernel (fully observed rows; others -> masked pass) */
 
 typedef struct mmf_ctx mmf_ctx;
 
@@ -68,16 +68,16 @@ typedef struct mmf_config {
   int32_t device;          /* CUDA device ordinal, -1 = current device */
   int32_t kernel;          /* MMF_KERNEL_* */
   int32_t assume_finite;   /* 1: caller guarantees y has no NaN/Inf, skip the masked fix-up pass */
-  int32_t tc_variant;      /* tuning of the tcgen05 kernel, same results whichever: 0 / 1 = the product (128-row tiles dealt
-                              round robin over the SMs), 2 = the experimental <8-stage, 2 staging tiles> instantiation,
-                              3 = the experimental balanced launch (one row range per SM) -- DESIGN.md section 6 */
+  int32_t tc_variant;      /* tuning of the tensor-core kernel, same results whichever: 0 / 1 = the product (128-row tiles dealt
+                              round robin over the SMs), 2 = the experimental <6-stage, 2 staging tiles> instantiation,
+                              3 = the experimental balanced launch (one row range per SM) */
   int64_t chunk_series;    /* host-buffer path: series per pipelined chunk (0 = library default) */
   void*   stream;          /* cudaStream_t to enqueue on (NULL = library-owned stream) */
   int32_t host_narrow;     /* host-buffer path: 0 = automatic, 1 = always try, 2 = never: narrow float32 chunks to
                               uint16 on host threads when every value is an integer in [0, 65534] (exactly, or the
                               chunk goes as float32), so that half the bytes cross PCIe; widened back on the device */
   int32_t host_threads;    /* threads of that narrowing pool (0 = half of the process's cores, at most 16) */
-  int32_t stream_solve;    /* series with gaps: 0 = solved in a pass of their own after the tcgen05 kernel (default), 1 = by a
+  int32_t stream_solve;    /* series with gaps: 0 = solved in a pass of their own after the tensor-core kernel (default), 1 = by a
                               consumer kernel launched BESIDE it (experimental: pays only with a register-capped build) */
   int32_t reserved1;
 } mmf_config;
@@ -118,7 +118,7 @@ int mmf_plan_design(mmf_ctx* ctx, const double* X, int32_t n_rows, int32_t p,
  * mmf_pin_scratch(ctx, +1) after a capture makes every later call that would have to move that memory (a larger
  * batch, mmf_plan_design) fail with MMF_E_UNSUPPORTED instead of leaving the graph with dangling pointers;
  * mmf_pin_scratch(ctx, -1) when the graph is destroyed.  Counted: one +1 per live graph.
- * replaces: nothing in the reference (Spark re-launches a Python task per group, 02:523-528); it is the B200
+ * replaces: nothing in the reference (Spark re-launches a Python task per group, 02:523-528); it is the H100
  * answer to that per-task launch overhead for small batches.                                                   */
 int mmf_pin_scratch(mmf_ctx* ctx, int32_t delta);
 /* W [MMF_P*MMF_P] row-major (beta = W gamma), kept[MMF_P] 0/1; either may be NULL */
@@ -158,12 +158,12 @@ int mmf_fit_forecast_int(mmf_ctx* ctx, const void* y, int32_t dtype, int64_t n, 
  * The reference re-indexes every group on its own calendar (sort_values + asfreq per group, 02:422-423), so one
  * batch may hold groups with different first dates and lengths.  Planning and fitting them calendar by calendar
  * costs a launch sequence per distinct calendar; a ragged plan whitens all calendars in one host call and ONE pass
- * of the tcgen05 kernel fits every group, each 128-row tile against its own calendar's design.
+ * of the tensor-core kernel fits every group, each 128-row tile against its own calendar's design.
  *   X_all        the calendars' design matrices back to back: calendar c contributes n_rows[c] rows of p doubles
  *   t_fit[c]     fit rows of calendar c (33 .. 65535); rows [pred_start[c], pred_start[c] + n_pred[c]) are evaluated
  *   n_pred[c]    per calendar.  One common value <= 64 (future mode: pred_start[c] = t_fit[c], n_pred[c] = horizon): the fit
  *                kernel's own epilogue writes the forecasts.  Anything else (holdout, the reference's contract: pred_start[c]
- *                = 0, n_pred[c] = every date of calendar c, 02:484-494): the fit hands gamma / c to the tcgen05 predict
+ *                = 0, n_pred[c] = every date of calendar c, 02:484-494): the fit hands gamma / c to the tensor-core predict
  *                kernel, which writes each calendar's block of the table through that calendar's own tensor map.
  * mmf_fit_forecast_ragged_f32: y [n, ld_y] device, rows grouped by calendar: calendar c owns rows
  * [cal_row_start[c], cal_row_start[c+1]) (host array of n_cal + 1 entries, 0 .. n); columns >= t_fit[c] of a row

@@ -135,7 +135,7 @@ print(json.dumps({{"lib": mmf.LIB_PATH, "max_err": float(err.max()), "p99_row_er
 
 def test_negative_control_without_lo_term_fails_config2():
     """BASELINE configs[1] (10k x 1,095, all rows) through two builds of the same ABI: the product library must pass
-    the stated tolerance, and tests/_build/libmmf_negctl.so -- the tcgen05 kernel compiled WITHOUT the lo*A_hi MMA of
+    the stated tolerance, and tests/_build/libmmf_negctl.so -- the tensor-core kernel compiled WITHOUT the lo*A_hi MMA of
     the 3-term tf32 split (-DMMF_TC_NO_LO_TERM) -- must FAIL it.  If the second half ever passes, the tolerance no
     longer guards the property that makes the tensor-core path legitimate."""
     neg = os.path.join(ROOT, "tests", "_build", "libmmf_negctl.so")
@@ -162,7 +162,7 @@ def test_negative_control_without_lo_term_fails_config2():
 
 # ---- the fused multi-GPU path against the oracle -------------------------------------------------------------
 @pytest.mark.parametrize("mode", ["p2p", "multicast-bulk"])
-def test_symmetric_table_fused_gather_matches_oracle(mode):
+def test_symmetric_table_fused_gather_matches_oracle(mode, tmp_path):
     """world_size >= 2 (one process per GPU, torchrun): every rank fits its shard and the fit kernel's epilogue
     stores each forecast tile into every rank's copy of the table (NVLink P2P bulk stores / NVLS multicast); every
     rank's whole table must equal the ORACLE's forecasts of all shards (not just NCCL's gather of the same numbers),
@@ -171,9 +171,7 @@ def test_symmetric_table_fused_gather_matches_oracle(mode):
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
     world = min(torch.cuda.device_count(), 8)
-    out = os.path.join(ROOT, "gpurun_out", f"symm_{mode}.json")
-    if os.path.exists(out):
-        os.remove(out)
+    out = str(tmp_path / f"symm_{mode}.json")
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}",
            "--master-addr", "127.0.0.1", "--master-port", "29617", os.path.join(ROOT, "tests", "_symm_worker.py"),
            "--mode", mode, "--out", out]
@@ -487,7 +485,7 @@ def test_host_narrowing_is_exact_or_not_used():
 
 def test_streaming_solve_matches_the_separate_pass():
     """mmf_config.stream_solve = 1: the queued records of series with gaps are consumed by solve_stream_kernel while
-    the tcgen05 kernel is still producing them (release/acquire work list, PDL launch).  Same records, same arithmetic:
+    the tensor-core kernel is still producing them (release/acquire work list, PDL launch).  Same records, same arithmetic:
     bit-equal forecasts and statuses to the default (a solve pass after the streaming kernel), also on a second call
     (the work list must be left clean) and when the default path runs in between."""
     import torch
@@ -616,7 +614,7 @@ def test_balanced_launch_is_bit_equal_to_round_robin_tiles(n, mode):
 
 def test_gappy_rows_do_not_depend_on_their_position_in_the_launch():
     """A series' forecast must not depend on which tile of which SM it lands in.  With an odd number of 32-step chunks
-    (t_fit = 400 -> 13) the two transform groups of the tcgen05 kernel swap roles from one tile of a CTA to the next;
+    (t_fit = 400 -> 13) the two transform groups of the tensor-core kernel swap roles from one tile of a CTA to the next;
     the gap positions are therefore filed by the chunk's parity inside the tile, not by the group that saw them, so the
     solve applies them in one canonical order.  Rows of a CTA's SECOND tile, fit again as a batch of their own (first
     tile of another CTA), must come out bit-identical -- with gaps."""

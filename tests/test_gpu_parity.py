@@ -14,7 +14,7 @@ pytestmark = pytest.mark.gpu
 
 
 def _le(err, tol, what=""):
-    """assert err <= tol, leaving the measured error in gpurun_out/parity_errors.jsonl"""
+    """assert err <= tol, leaving the measured error in the scratch log of conftest.record_err"""
     import os
     name = os.environ.get("PYTEST_CURRENT_TEST", "?").split("::")[-1].split(" ")[0]
     record_err(name, err, tol, what=str(what))
@@ -92,7 +92,7 @@ def test_parity_full_series(engines, kernel, n, t):
 
 
 def test_parity_config2_10k_by_1095(engines):
-    """BASELINE.json configs[1]: 10k groups x 1,095 days fp32, single B200, parity on ALL series."""
+    """BASELINE.json configs[1]: 10k groups x 1,095 days fp32, single H100, parity on ALL series."""
     y, start = mmf.synth.daily_store_item_demand(10_000, 1095, seed=1234)
     want, _ = _oracle(y, start, "D", 28, "future")
     for k in ("tc", "warp"):
@@ -119,12 +119,12 @@ def test_parity_masked_series(engines, kernel):
     assert np.array_equal(status, wst)
     if kernel != "warp":
         # rows whose first value is missing (or with > 44 gaps per transform group) take the general pass;
-        # every other gappy row is solved from the record the tcgen05 kernel queued
+        # every other gappy row is solved from the record the tensor-core kernel queued
         assert 0 < res["stats"].n_pending < 300
 
 
 def test_gap_counts_around_record_capacity(engines):
-    """The tcgen05 kernel notes gap positions per transform group (alternate 32-step chunks) in two 44-entry
+    """The tensor-core kernel notes gap positions per transform group (alternate 32-step chunks) in two 44-entry
     segments that the solve kernel reads four at a time: every count 0..48 in one group (all tails of the 4-wide
     groups, the capacity edge and the overflow to the general pass), both groups, must match the oracle."""
     t, h = 1095, 28
@@ -367,7 +367,7 @@ def test_broadcast_stores_write_every_replica(engines):
 @pytest.mark.parametrize("n,t", [(300, 1095), (1000, 400), (129, 157), (5, 130)])
 def test_holdout_on_tensor_cores_matches_oracle_and_warp(engines, n, t):
     """Reference contract (02:484-494): a value for EVERY grid date.  auto/tc = fit kernels + predict_tc_kernel
-    (tcgen05 GEMM + TMA stores), warp = CUDA-core path; both against the float64 oracle, incl. rows with gaps."""
+    (wgmma GEMM + TMA stores), warp = CUDA-core path; both against the float64 oracle, incl. rows with gaps."""
     y, start = mmf.synth.daily_store_item_demand(n, t, seed=300 + n)
     y[1, 10:40] = np.nan
     y[2, :] = np.nan                                  # empty row -> NaN everywhere, status 1

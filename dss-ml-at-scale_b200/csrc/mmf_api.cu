@@ -166,7 +166,9 @@ struct mmf_ctx {
   bool set_clean[2] = {true, true};    // the set is known to be zero (cudaMemset at create, or zeroed by the previous
                                        // eager call's tensor-core kernel); anything else makes the call memset its set
   int last_set = 0;                    // set the last enqueued call used (stats read n_pending from it)
-  int pinned = 0;                      // > 0: a captured CUDA graph holds pointers into the scratch below and into the plan
+  uint32_t* d_slab_pending = nullptr;  // n_pending of every slab of a multi-slab call with stats (grown on demand)
+  size_t slab_pending_cap = 0;
+  int pinned = 0;                     // > 0: a captured CUDA graph holds pointers into the scratch below and into the plan
   bool status_scratch_captured = false;   // some capture ran without a caller-provided status buffer
   SolveRec* d_recs = nullptr;          // deferred masked series (grown on demand, capped)
   size_t recs_cap_bytes = 0;
@@ -420,10 +422,7 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
 // slab, not to the batch.  One slab for batches up to a million rows; beyond that the slab is sized so the scratch
 // stays under ~5 % of the input (10 M x 365: 4 slabs, 0.7 GB instead of 2.6 GB).  Slabs run back to back on the
 // stream; the scratch of slab i is free again when slab i+1 starts (stream order).
-int run_device(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pred_start, int32_t n_pred,
-               float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s, int* launches,
-               int* kernel_used, float* const* out_more = nullptr, int n_out = 1, int multimem = 0,
-               const SelectArgs* sel = nullptr) {
+int64_t slab_rows(const mmf_ctx* ctx, int64_t n) {
   int64_t slab = n;
   if (n > (int64_t)1 << 20) {
     const double input_bytes = (double)n * (double)ctx->plan.t_fit * 4.0;
@@ -432,7 +431,17 @@ int run_device(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pr
     const int64_t n_slabs = (n + slab - 1) / slab;
     slab = (((n + n_slabs - 1) / n_slabs) + 127) & ~(int64_t)127;     // equal slabs
   }
-  for (int64_t off = 0; off < n; off += slab) {
+  return slab;
+}
+
+// slab_pending (nullable, one word per slab): each slab's count of rows handed to the general pass is copied there
+// before the next slab's tensor-core kernel zeroes the counter set it was kept in (0 for a slab fit by the warp kernel).
+int run_device(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pred_start, int32_t n_pred,
+               float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s, int* launches,
+               int* kernel_used, float* const* out_more = nullptr, int n_out = 1, int multimem = 0,
+               const SelectArgs* sel = nullptr, uint32_t* slab_pending = nullptr) {
+  const int64_t slab = slab_rows(ctx, n);
+  for (int64_t off = 0, i = 0; off < n; off += slab, ++i) {
     const int64_t m = std::min(slab, n - off);
     float* more[MAX_OUT - 1] = {};
     for (int i = 0; i + 1 < n_out && i < MAX_OUT - 1; ++i) more[i] = out_more[i] + off * ld_out;
@@ -446,6 +455,13 @@ int run_device(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pr
                                    beta ? beta + off * P : nullptr, status + off, s, launches, kernel_used, more, n_out,
                                    multimem, sel != nullptr ? &sel_slab : nullptr);
     if (rc != MMF_OK) return rc;
+    if (slab_pending != nullptr) {
+      if (*kernel_used == MMF_KERNEL_TC)
+        CU_TRY(cudaMemcpyAsync(slab_pending + i, ctx->d_pending + CTR_WORDS * ctx->last_set, sizeof(uint32_t),
+                               cudaMemcpyDeviceToDevice, s));
+      else
+        CU_TRY(cudaMemsetAsync(slab_pending + i, 0, sizeof(uint32_t), s));
+    }
   }
   return MMF_OK;
 }
@@ -555,6 +571,7 @@ int mmf_destroy(mmf_ctx* ctx) {
     if (ctx->hslot[i].ev) cudaEventDestroy(ctx->hslot[i].ev);
   }
   cudaFree(ctx->d_pending);
+  cudaFree(ctx->d_slab_pending);
   cudaFree(ctx->d_recs);
   cudaFree(ctx->d_rec_rows);
   cudaFree(ctx->d_gamma);
@@ -714,18 +731,39 @@ static int fit_forecast_impl(mmf_ctx* ctx, const void* y_any, int32_t dtype, int
       if (rc != MMF_OK) return rc;
       status = ctx->d_status_scratch;
     }
+    // Several slabs: every slab's tensor-core kernel zeroes the counter set the slab before it used, so the pending
+    // count of each slab is copied aside as it completes and summed here.  A call with stats synchronises and so is
+    // never captured: this scratch is not part of any graph and may grow while one is pinned.
+    const int64_t slab = slab_rows(ctx, n);
+    const int64_t n_slabs = (n + slab - 1) / slab;
+    uint32_t* slab_pending = nullptr;
+    if (stats && n_slabs > 1) {
+      const mmf_ctx* saved = g_grow_ctx;
+      g_grow_ctx = nullptr;
+      const int rc = grow((void**)&ctx->d_slab_pending, &ctx->slab_pending_cap, (size_t)n_slabs * sizeof(uint32_t));
+      g_grow_ctx = saved;
+      if (rc != MMF_OK) return rc;
+      slab_pending = ctx->d_slab_pending;
+    }
     if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, ctx->stream));
     int rc = run_device(ctx, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_beta, status, ctx->stream,
-                        &launches, &kernel_used);
+                        &launches, &kernel_used, nullptr, 1, 0, nullptr, slab_pending);
     if (rc != MMF_OK) return rc;
     if (stats) {
       CU_TRY(cudaEventRecord(ctx->ev_k1, ctx->stream));
       CU_TRY(cudaEventSynchronize(ctx->ev_k1));
       CU_TRY(cudaEventElapsedTime(&stats->kernel_ms, ctx->ev_k0, ctx->ev_k1));
       stats->total_ms = stats->kernel_ms;
-      uint32_t pend = 0;
-      CU_TRY(cudaMemcpy(&pend, ctx->d_pending + CTR_WORDS * ctx->last_set, sizeof(pend), cudaMemcpyDeviceToHost));
-      stats->n_pending = (kernel_used == MMF_KERNEL_TC) ? pend : 0;
+      if (slab_pending != nullptr) {
+        std::vector<uint32_t> pend((size_t)n_slabs);
+        CU_TRY(cudaMemcpy(pend.data(), slab_pending, pend.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+        stats->n_pending = 0;
+        for (uint32_t v : pend) stats->n_pending += v;
+      } else {
+        uint32_t pend = 0;
+        CU_TRY(cudaMemcpy(&pend, ctx->d_pending + CTR_WORDS * ctx->last_set, sizeof(pend), cudaMemcpyDeviceToHost));
+        stats->n_pending = (kernel_used == MMF_KERNEL_TC) ? pend : 0;
+      }
     }
   } else {
     // ------------------------------------------------ host buffers (or an integer series buffer): pipelined chunks

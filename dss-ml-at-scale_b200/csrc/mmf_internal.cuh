@@ -149,7 +149,7 @@ struct TcLaunch {
   alignas(64) unsigned char tmap_at[128];
   alignas(64) unsigned char tmap_y8[128];   // box {32 t, 8 series}: the short last tile of a balanced launch's CTA
 };
-// variant: 0 / 1 = <10 smem stages, 1 forecast staging tile>, tiles dealt round robin (the product), 2 = <8 stages,
+// variant: 0 / 1 = <8 smem stages, 1 forecast staging tile>, tiles dealt round robin (the product), 2 = <6 stages,
 // 2 staging tiles>, 3 = balanced row ranges per CTA (both experiments that did not pay, kept for the record)
 int fit_tc_balanced_rows(int64_t n, int sm_count, int variant);
 cudaError_t launch_fit_tc(const DesignView& d, const FitArgs& a, const TcLaunch& tl,

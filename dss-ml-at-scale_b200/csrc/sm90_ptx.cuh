@@ -153,6 +153,15 @@ __device__ __forceinline__ void bulk_store_elect(uint64_t dst_global, uint32_t s
       ::"l"(dst_global), "r"(src_smem), "r"(bytes)
       : "memory");
 }
+// the same with an L2 cache-eviction policy for the written lines (L2_EVICT_*)
+__device__ __forceinline__ void bulk_store_hint_elect(uint64_t dst_global, uint32_t src_smem, uint32_t bytes, uint64_t hint) {
+  asm volatile(
+      "{\n\t.reg .pred pe;\n\t"
+      "elect.sync _|pe, 0xffffffff;\n\t"
+      "@pe cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;\n\t}"
+      ::"l"(dst_global), "r"(src_smem), "r"(bytes), "l"(hint)
+      : "memory");
+}
 __device__ __forceinline__ void bulk_commit_elect() {
   asm volatile(
       "{\n\t.reg .pred pe;\n\t"

@@ -36,6 +36,12 @@ constexpr int KC = 32;                 // time steps per stage == one 128-B swiz
 // kernel: <8 stages, 1 staging tile> is the product configuration, <6, 2> (a second staging tile lets tile k+1 be
 // assembled while the NVLink stores of tile k are still reading tile k's) an experiment.
 constexpr int NGROUPS = 2;             // consumer warpgroups (alternate chunks)
+// A wgmma accumulator rounds every addition relative to the running partial sum, which grows with the fit window, so
+// summing a long window in one accumulator has an error that grows linearly with t_fit (36x the parity tolerance at
+// 70,001 rows).  Each consumer group therefore adds its accumulator into a running fp32 sum (kept in the tile's slot
+// of partial moments in shared memory) and restarts it after every FOLD_CHUNKS of its chunks.  Tiles of up to 2 * 18 chunks (t_fit <= 1,152) never fold and are summed exactly as
+// without folding.
+constexpr int FOLD_CHUNKS = 18;
 constexpr int MAX_PRED = 64;           // forecast rows the epilogue supports
 constexpr int BULK_MAX_PRED = 28;      // forecast rows the staged bulk-store epilogue supports (14 KB of smem)
 constexpr int Y_STAGE_BYTES = TILE_M * KC * 4;      // 16384
@@ -270,6 +276,15 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
       const int seg = (grp ^ (int)gc) & 1;
       int nm = 0;                                       // missing values this thread saw in the tile
       unsigned long long packq = 0ull;                  // the last (nm & 3) gap positions, newest in the top lanes
+      // the tile's slot of partial moments for the epilogue; a long tile keeps the folded sums of its restarted
+      // accumulators there (each thread its own entries), which costs no registers
+      const int ab = lt & 1;
+      float* __restrict__ sacc = s_acc + (ab * NGROUPS + grp) * TILE_M * P;
+      auto sacc_at = [&](int h, int j, int i) {
+        return reinterpret_cast<float2*>(sacc + (64 * h + frow0 + 8 * j) * P + 8 * i + 2 * t4);
+      };
+      bool folded = false;
+      int since_fold = 0;
       for (int ch = seg; ch < tr.n_chunks; ch += NGROUPS) {
         const uint32_t k = gc + static_cast<uint32_t>(ch);
         const int stage = static_cast<int>(k % STAGES);
@@ -343,24 +358,43 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
         wgmma_fence_regs(acc[1]);
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_empty(stage));   // this warp's MMAs and smem reads of the stage are done
+        if (++since_fold == FOLD_CHUNKS && ch + NGROUPS < tr.n_chunks) {   // more chunks follow: fold and restart
+          if (!folded) mbar_wait(bar_accempty(ab), ((lt >> 1) & 1) ^ 1u);  // epilogue of tile lt-2 has drained the slot
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int j = 0; j < 2; ++j)
+#pragma unroll
+              for (int i = 0; i < 2; ++i) {
+                const int q = 4 * i + 2 * j;            // acc[h][q + 8] is the lo column of acc[h][q]
+                float2 f = make_float2(acc[h][q] + acc[h][q + P / 2], acc[h][q + 1] + acc[h][q + 1 + P / 2]);
+                if (folded) { const float2 o = *sacc_at(h, j, i); f.x = o.x + f.x; f.y = o.y + f.y; }
+                *sacc_at(h, j, i) = f;
+              }
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int i = 0; i < P; ++i) acc[h][i] = 0.f;
+          folded = true;
+          since_fold = 0;
+        }
       }
       if (scan && (nm & 3) != 0 && nm < SOLVE_SEG) {    // flush the partial group (right-aligned: oldest first)
         uint16_t* __restrict__ mt = a.recs[(int64_t)tr.row0 + r].miss_t + seg * SOLVE_SEG;
         *reinterpret_cast<unsigned long long*>(mt + (nm & ~3)) = packq >> (16 * (4 - (nm & 3)));
       }
       // hand the tile's partial moments (hi and lo columns folded: b = D[:, p] + D[:, P + p]) to the epilogue
-      const int ab = lt & 1;
-      mbar_wait(bar_accempty(ab), ((lt >> 1) & 1) ^ 1u);  // epilogue of tile lt-2 has drained this slot
-      float* __restrict__ sacc = s_acc + (ab * NGROUPS + grp) * TILE_M * P;
+      if (!folded) mbar_wait(bar_accempty(ab), ((lt >> 1) & 1) ^ 1u);  // epilogue of tile lt-2 has drained this slot
 #pragma unroll
       for (int h = 0; h < 2; ++h)
 #pragma unroll
         for (int j = 0; j < 2; ++j)
 #pragma unroll
           for (int i = 0; i < 2; ++i) {
-            const float2 v = make_float2(acc[h][4 * i + 2 * j] + acc[h][4 * (i + 2) + 2 * j],
-                                         acc[h][4 * i + 2 * j + 1] + acc[h][4 * (i + 2) + 2 * j + 1]);
-            *reinterpret_cast<float2*>(sacc + (64 * h + frow0 + 8 * j) * P + 8 * i + 2 * t4) = v;
+            const int q = 4 * i + 2 * j;                // acc[h][q + 8] is the lo column of acc[h][q]
+            float2 v = make_float2(acc[h][q] + acc[h][q + P / 2], acc[h][q + 1] + acc[h][q + 1 + P / 2]);
+            if (folded) { const float2 o = *sacc_at(h, j, i); v.x = o.x + v.x; v.y = o.y + v.y; }
+            *sacc_at(h, j, i) = v;
           }
       const int cnt = nm > 0x7ffe ? 0x7ffe : nm;
       s_nm[(ab * NGROUPS + seg) * TILE_M + r] = static_cast<uint16_t>(cnt | (bad ? 0x8000 : 0));

@@ -118,9 +118,20 @@ __device__ __noinline__ int solve_masked(const DesignView& d, const ARows& A, co
       for (int k = 0; k < DPL; ++k) dacc[k] = fmaf(A.elem(tt, pi[k]), A.elem(tt, pj[k]), dacc[k]);
     }
   } else {
-    // second pass over the row (L2-hot), 8 independent 128-B loads in flight per trip
+    // second pass over the row (L2-hot), 8 independent 128-B loads in flight per trip.  Every lane sums its entries
+    // over the whole row; for a long row (a mostly-missing one sums every observed position) the partial sums grow and
+    // so does the rounding of each addition, so the sums restart every FOLD_T positions and are added up in dsum.  Rows
+    // of up to FOLD_T fit values are summed exactly as without folding.
+    constexpr int FOLD_T = 2048;
+    float dsum[DPL];
+    bool folded = false;
 #pragma unroll 1
     for (int t0 = 0; t0 < t_fit; t0 += 256) {
+      if (t0 > 0 && t0 % FOLD_T == 0) {
+#pragma unroll
+        for (int k = 0; k < DPL; ++k) { dsum[k] = folded ? dsum[k] + dacc[k] : dacc[k]; dacc[k] = 0.f; }
+        folded = true;
+      }
       float v[8];
 #pragma unroll
       for (int u = 0; u < 8; ++u) {
@@ -141,6 +152,10 @@ __device__ __noinline__ int solve_masked(const DesignView& d, const ARows& A, co
           for (int k = 0; k < DPL; ++k) dacc[k] = fmaf(A.elem(tt, pi[k]), A.elem(tt, pj[k]), dacc[k]);
         }
       }
+    }
+    if (folded) {
+#pragma unroll
+      for (int k = 0; k < DPL; ++k) dacc[k] = dsum[k] + dacc[k];
     }
   }
   __syncwarp();

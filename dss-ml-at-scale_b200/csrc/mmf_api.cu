@@ -403,7 +403,11 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
     PredictLaunch pl;
     memcpy(pl.tmap_bhi, ctx->plan.tmap_bhi, 128);
     memcpy(pl.tmap_blo, ctx->plan.tmap_blo, 128);
-    int rc = encode_2d(pl.tmap_out, out, (uint64_t)n_pred, (uint64_t)n, (uint64_t)ld_out * 4, 32, 64);   // one box per warpgroup half
+    // the map stops at the last whole 16 B of a row (TMA clips with 16-B granularity); the kernel stores the
+    // n_pred % 4 columns behind it itself, so the caller's columns from n_pred on are never written
+    pl.n_tma = n_pred & ~3;
+    int rc = encode_2d(pl.tmap_out, out, (uint64_t)(pl.n_tma > 0 ? pl.n_tma : n_pred), (uint64_t)n, (uint64_t)ld_out * 4,
+                       32, 64);   // one box per warpgroup half
     if (rc != MMF_OK) return rc;
     CU_TRY(launch_predict_tc(d, a, pl, ctx->sm_count, s));
     ++*launches;
@@ -1233,6 +1237,7 @@ int mmf_fit_forecast_ragged_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t
     memcpy(pl.tmap_bhi, m.tmap_bhi, 128);
     memcpy(pl.tmap_blo, m.tmap_blo, 128);
     memcpy(pl.tmap_out, m.tmap_bhi, 128);                  // unused by the ragged kernel (per-calendar maps instead)
+    pl.n_tma = 0;                                          // unused as well: each calendar's map clips its own block
     CU_TRY(launch_predict_tc(d, a, pl, ctx->sm_count, s, m.d_units, m.n_units, m.d_tmaps_out));
     ++launches;
   }

@@ -129,6 +129,8 @@ struct PredictLaunch {
   alignas(64) unsigned char tmap_bhi[128];
   alignas(64) unsigned char tmap_blo[128];
   alignas(64) unsigned char tmap_out[128];
+  int32_t n_tma;                           // single calendar: columns [0, n_tma) leave through tmap_out, [n_tma, n_pred)
+                                           // through plain stores (TMA clips with 16-B granularity, n_tma = n_pred & ~3)
 };
 struct PredUnit {                          // one (tile, chunk) work unit of a ragged predict launch (32 B)
   int32_t row0, nrows;                     // series rows of the tile inside one calendar

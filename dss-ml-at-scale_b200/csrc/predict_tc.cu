@@ -157,8 +157,21 @@ predict_tc_kernel(const __grid_constant__ PredictLaunch pl, const DesignView d, 
         const uint32_t q = static_cast<uint32_t>(2 * (i & 3) + (t4 >> 1));
         const uint32_t col = obase + (i >> 2) * OUT_SUB_BYTES + ((q ^ static_cast<uint32_t>(g8)) << 4) + (t4 & 1) * 8;
 #pragma unroll
-        for (int j = 0; j < 2; ++j)
-          sts64(col + static_cast<uint32_t>(frow + 8 * j) * 128u, acc[4 * i + 2 * j] + c[j], acc[4 * i + 2 * j + 1] + c[j]);
+        for (int j = 0; j < 2; ++j) {
+          const float v0 = acc[4 * i + 2 * j] + c[j], v1 = acc[4 * i + 2 * j + 1] + c[j];
+          sts64(col + static_cast<uint32_t>(frow + 8 * j) * 128u, v0, v1);
+          if (!MULTI) {
+            // the table's last n_pred % 4 columns: a TMA store would also write the caller's columns up to the next
+            // multiple of 4, so these few go out as plain stores
+            const int tcol = pu.ch * TN + 8 * i + 2 * t4;
+            const int rl = WG_M * wg + frow + 8 * j;
+            if (tcol + 1 >= pl.n_tma && tcol < a.n_pred && rl < pu.nrows) {
+              float* __restrict__ orow = a.out + ((int64_t)pu.row0 + rl) * a.ld_out;
+              if (tcol >= pl.n_tma) orow[tcol] = v0;
+              if (tcol + 1 < a.n_pred) orow[tcol + 1] = v1;
+            }
+          }
+        }
       }
       fence_proxy_async_smem();
       named_bar_sync(1 + wg, 128);
@@ -168,7 +181,8 @@ predict_tc_kernel(const __grid_constant__ PredictLaunch pl, const DesignView d, 
           if (MULTI) fence_tensormap_acquire(tmo);
 #pragma unroll
           for (int j = 0; j < TN / 32; ++j)
-            tma_store_2d_elect(tmo, obase + j * OUT_SUB_BYTES, pu.ch * TN + j * 32, pu.row_in_map + WG_M * wg);
+            if (MULTI || pu.ch * TN + j * 32 < pl.n_tma)
+              tma_store_2d_elect(tmo, obase + j * OUT_SUB_BYTES, pu.ch * TN + j * 32, pu.row_in_map + WG_M * wg);
         }
         bulk_commit_elect();
       }

@@ -133,6 +133,9 @@ int mmf_get_whitening(mmf_ctx* ctx, double* W, int32_t* kept);
  * out_pred [n, ld_out] float32, host or device (same side as y not required)
  * out_beta [n, MMF_P]  nullable: coefficients on the raw X columns
  * out_status [n]       nullable
+ * Only columns [0, n_pred) of each out_pred row are written: columns [n_pred, ld_out) keep what the caller left
+ * there, whatever the kernel (any ld_out >= n_pred and any base pointer; 16-B aligned tables with ld_out % 4 == 0
+ * take the tensor-core store path, others the CUDA-core kernels).
  * Device-pointer calls are enqueued on the ctx stream and return without
  * synchronising unless `stats` is non-NULL.  Host-pointer calls pipeline
  * H2D / kernel / D2H in chunks and return when the results are in host memory.

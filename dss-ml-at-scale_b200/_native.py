@@ -25,7 +25,7 @@ INT_MISSING = {"int16": -32768, "uint16": 65535, "int32": -2147483648}     # the
 EXPORTS = (
     "mmf_version", "mmf_last_error", "mmf_device_count", "mmf_create", "mmf_destroy",
     "mmf_set_stream", "mmf_synchronize", "mmf_plan_design", "mmf_pin_scratch", "mmf_get_whitening",
-    "mmf_fit_forecast_f32", "mmf_fit_forecast_int", "mmf_plan_calendars", "mmf_fit_forecast_ragged_f32",
+    "mmf_fit_forecast_f32", "mmf_fit_forecast_int", "mmf_fit_forecast_se_f32", "mmf_plan_calendars", "mmf_fit_forecast_ragged_f32",
     "mmf_fit_forecast_bcast_f32", "mmf_fit_select_forecast_f32", "mmf_pack_hash_utf8", "mmf_pack_hash_i32",
     "mmf_pack_group_codes", "mmf_pack_verify_utf8", "mmf_pack_verify_i32", "mmf_pack_minmax", "mmf_pack_scatter_f32", "mmf_alloc_pinned", "mmf_free_pinned",
     "mmf_host_register", "mmf_host_unregister",
@@ -97,6 +97,10 @@ def load() -> C.CDLL:
     lib.mmf_fit_forecast_int.argtypes = [
         C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_int64, C.c_int32, C.c_int32,
         C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.POINTER(MmfStats),
+    ]
+    lib.mmf_fit_forecast_se_f32.argtypes = [
+        C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32,
+        C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(MmfStats),
     ]
     lib.mmf_plan_calendars.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_int32, C.c_int32]

@@ -50,7 +50,7 @@ constexpr int THREADS = 416;
 constexpr int WARP_EPI0 = 8, WARP_PROD = 12;
 // named barriers: 1-3 epilogue, 4 + g consumer warpgroup g
 
-template <int STAGES, int OBUF>
+template <int STAGES, int OBUF, bool SE = false>
 struct SmemLayoutT {
   // offsets from the 1024-aligned base
   static constexpr int y = 0;
@@ -62,7 +62,10 @@ struct SmemLayoutT {
   static constexpr int cc = nm + 2 * NGROUPS * TILE_M * 2;           // centring constants: [2 groups][2 tiles][128] f32
   static constexpr int bars = cc + NGROUPS * 2 * TILE_M * 4;
   static constexpr int n_bars = 2 * STAGES + 4;
-  static constexpr int total = bars + n_bars * 8;
+  // SE only: S per row, [2 slots][2 groups][128] f64, and sqrt(1 + h_t) of the prediction rows
+  static constexpr int ss = bars + n_bars * 8;
+  static constexpr int sfac = ss + (SE ? 2 * NGROUPS * TILE_M * 8 : 0);
+  static constexpr int total = sfac + (SE ? MAX_PRED * 4 : 0);
   static_assert(total + 1024 <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into");
 };
 
@@ -108,12 +111,16 @@ __device__ __forceinline__ float lds32(uint32_t addr) {
 // one contiguous range of mv.bal_rows rows (a multiple of 8) and walks it in 128-row tiles; the range's last tile is
 // short and is loaded as 8-row boxes, so no SM streams rows it does not own.
 // Rows are independent in the GEMM, so the forecasts are bit-identical to the round-robin launch's.
-template <int STAGES, int OBUF, bool MULTI, bool BAL>
+// SE (standard-error calls, single calendar): the consumers also sum S = sum (y - c)^2 of their fragment rows and the
+// epilogue writes sigma / dof (and the se row in future mode) of the gap-free rows; the MMA inputs are unchanged.
+template <int STAGES, int OBUF, bool MULTI, bool BAL, bool SE = false>
 __global__ void __launch_bounds__(THREADS, 1)
 fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const FitArgs a,
-              uint32_t* __restrict__ pending_count, const int n_tiles_all, const int n_chunks, const MultiView mv) {
+              uint32_t* __restrict__ pending_count, const int n_tiles_all, const int n_chunks, const MultiView mv,
+              const SeArgs se) {
   static_assert(!(MULTI && BAL), "ragged launches carry their own tile table");
-  using SmemLayout = SmemLayoutT<STAGES, OBUF>;
+  static_assert(!SE || !(MULTI || BAL), "standard errors are built for the single-calendar round-robin launch");
+  using SmemLayout = SmemLayoutT<STAGES, OBUF, SE>;
   // BAL: this CTA's rows; its k-th tile keeps the round-robin loop index blockIdx.x + k * gridDim.x
   const int64_t cta_row0 = BAL ? (int64_t)blockIdx.x * mv.bal_rows : 0;
   const int cta_rows = BAL ? (int)(a.n - cta_row0 < mv.bal_rows ? a.n - cta_row0 : mv.bal_rows) : 0;
@@ -143,6 +150,8 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
   float* s_acc = reinterpret_cast<float*>(smem + SmemLayout::acc);
   uint16_t* s_nm = reinterpret_cast<uint16_t*>(smem + SmemLayout::nm);
   float* s_cc = reinterpret_cast<float*>(smem + SmemLayout::cc);
+  double* s_ss = reinterpret_cast<double*>(smem + SmemLayout::ss);
+  float* s_sfac = reinterpret_cast<float*>(smem + SmemLayout::sfac);
   // series with gaps: substitute the centring constant for missing values (so the moments stay exact), record
   // where they were, and let the epilogue queue a SolveRec for solve_rows_kernel instead of a second pass
 #ifdef MMF_TC_NO_COLLECT
@@ -187,6 +196,8 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
     if (!a.skip_pred && !MULTI)
       for (int i = threadIdx.x - WARP_EPI0 * 32; i < a.n_pred * P; i += 128)
         s_apred[i] = __ldg(d.apred + (size_t)a.pred_start * P + i);
+    if (SE && !a.skip_pred)
+      for (int i = threadIdx.x - WARP_EPI0 * 32; i < a.n_pred; i += 128) s_sfac[i] = __ldg(se.sfac + a.pred_start + i);
   }
   __syncthreads();
   // This CTA is resident: a dependent kernel launched behind this one with programmatic stream serialisation may start
@@ -285,6 +296,9 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
       };
       bool folded = false;
       int since_fold = 0;
+      // SE: S of the four fragment rows over this thread's columns.  A chunk's 8 squares are summed in fp32 and the
+      // chunk sums in f64, so the rounding does not grow with the fit window (the moments restart for the same reason)
+      double ssq[2][2] = {{0.0, 0.0}, {0.0, 0.0}};
       for (int ch = seg; ch < tr.n_chunks; ch += NGROUPS) {
         const uint32_t k = gc + static_cast<uint32_t>(ch);
         const int stage = static_cast<int>(k % STAGES);
@@ -323,11 +337,13 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
         // A fragments of both 64-row halves: centre (missing values take the centring constant, so they add
         // (c - c) = 0 to every moment), split into tf32 hi + fp32 residual lo
         uint32_t ahi[2][KC / 8][4], alo[2][KC / 8][4];
+        const int lim = d.t_fit - ch * KC;              // SE: columns from t_fit on arrive as zeros (TMA clip), not c
 #pragma unroll
         for (int h = 0; h < 2; ++h)
 #pragma unroll
           for (int j = 0; j < 2; ++j) {
             const uint32_t rowp = sy + static_cast<uint32_t>(64 * h + frow0 + 8 * j) * 128u + t4 * 4;   // row & 7 == g8
+            float part = 0.f;
 #pragma unroll
             for (int kk = 0; kk < KC / 8; ++kk)
 #pragma unroll
@@ -338,7 +354,12 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
                 const uint32_t hb = __float_as_uint(rr) & 0xFFFFE000u;
                 ahi[h][kk][j + 2 * hf] = hb;
                 alo[h][kk][j + 2 * hf] = __float_as_uint(rr - __uint_as_float(hb));
+                if (SE) {
+                  const float rs = 4 * (2 * kk + hf) + t4 < lim ? rr : 0.f;
+                  part = fmaf(rs, rs, part);
+                }
               }
+            if (SE) ssq[h][j] += static_cast<double>(part);
           }
         const uint64_t bdesc0 = gmma_desc_k_sw128(s_at + stage * AT_STAGE_BYTES);
         wgmma_fence();
@@ -396,6 +417,17 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
             if (folded) { const float2 o = *sacc_at(h, j, i); v.x = o.x + v.x; v.y = o.y + v.y; }
             *sacc_at(h, j, i) = v;
           }
+      if (SE) {                                         // the quad's four column sets -> one S per fragment row
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            double v = ssq[h][j];
+            v += __shfl_xor_sync(0xffffffffu, v, 1);
+            v += __shfl_xor_sync(0xffffffffu, v, 2);
+            if (t4 == 0) s_ss[(ab * NGROUPS + grp) * TILE_M + 64 * h + frow0 + 8 * j] = v;
+          }
+      }
       const int cnt = nm > 0x7ffe ? 0x7ffe : nm;
       s_nm[(ab * NGROUPS + seg) * TILE_M + r] = static_cast<uint16_t>(cnt | (bad ? 0x8000 : 0));
       mbar_arrive(bar_accfull(ab));
@@ -420,6 +452,9 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
     const bool bulk = !a.skip_pred && vec_out && a.out_multimem != 1 && a.ld_out == a.n_pred && a.n_pred <= BULK_MAX_PRED;
 #endif
     const uint32_t s_ostage_u32 = smem_u32(s_ostage);
+    // SE: 16-B stores of the se rows when the table allows them (the same test as vec_out)
+    const bool se_vec = SE && (a.n_pred % 4 == 0) && (se.ld_se % 4 == 0) &&
+                        ((reinterpret_cast<uintptr_t>(se.out_se) & 15u) == 0);
     int lt = 0;
     int cur_cal = MULTI ? -1 : 0;
     uint32_t kept_mask = d.kept_mask;
@@ -456,6 +491,7 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
       }
       // gaps the consumer warpgroups saw in this tile, by chunk parity
       const unsigned f0 = s_nm[(ab * NGROUPS + 0) * TILE_M + r], f1 = s_nm[(ab * NGROUPS + 1) * TILE_M + r];
+      const double ss = SE ? s_ss[(ab * NGROUPS + 0) * TILE_M + r] + s_ss[(ab * NGROUPS + 1) * TILE_M + r] : 0.0;
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_accempty(ab));     // the consumers may overwrite this slot now
       int nm0 = 0, nm1 = 0;
@@ -491,6 +527,7 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
           bp[0] = make_float4(g[0], g[1], g[2], g[3]);    bp[1] = make_float4(g[4], g[5], g[6], g[7]);
           bp[2] = make_float4(g[8], g[9], g[10], g[11]);  bp[3] = make_float4(g[12], g[13], g[14], g[15]);
           rec.c = c;
+          if (SE) rec.ss = static_cast<float>(ss);
           rec.nm[0] = static_cast<uint16_t>(nm0);
           rec.nm[1] = static_cast<uint16_t>(nm1);
           rec.cal = tr.cal;
@@ -568,6 +605,26 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
               br[p] = s;
             }
           }
+          if (SE) {
+            // gap-free: G_i = I, so b'gamma = |gamma|^2, every kept column is used and h_t = |a_t|^2
+            double bg = 0.0;
+#pragma unroll
+            for (int p = 0; p < P; ++p) bg = fma(static_cast<double>(g[p]), static_cast<double>(g[p]), bg);
+            const int dof = t_fit_c - __popc(kept_mask);
+            const double rss = fmax(ss - bg, 0.0);
+            const float sig = dof > 0 ? static_cast<float>(sqrt(rss / dof)) : __int_as_float(0x7fc00000);
+            se.sigma[row] = sig;
+            if (se.dof != nullptr) se.dof[row] = dof;
+            if (se.out_se != nullptr && !a.skip_pred) {
+              float* __restrict__ srow = se.out_se + row * se.ld_se;
+              int k = 0;
+              if (se_vec)
+                for (; k < a.n_pred; k += 4)
+                  __stcs(reinterpret_cast<float4*>(srow + k),
+                         make_float4(sig * s_sfac[k], sig * s_sfac[k + 1], sig * s_sfac[k + 2], sig * s_sfac[k + 3]));
+              for (; k < a.n_pred; ++k) __stcs(srow + k, sig * s_sfac[k]);
+            }
+          }
           a.status[row] = MMF_STATUS_OK;
         } else {
           a.status[row] = pend ? MMF_STATUS_PENDING : MMF_STATUS_DEFERRED;
@@ -600,14 +657,15 @@ bool fit_tc_supported(const DesignView& d, const FitArgs& a, const char** why) {
   return w == nullptr;
 }
 
-template <int STAGES, int OBUF, bool MULTI, bool BAL = false>
+template <int STAGES, int OBUF, bool MULTI, bool BAL = false, bool SE = false>
 static cudaError_t launch_variant(const DesignView& d, const FitArgs& a, const TcLaunch& tl, uint32_t* pending_count,
-                                  int sm_count, cudaStream_t s, int n_tiles, int n_chunks, const MultiView& mv) {
-  const size_t smem = SmemLayoutT<STAGES, OBUF>::total + 1024;
-  cudaError_t e = cudaFuncSetAttribute(fit_tc_kernel<STAGES, OBUF, MULTI, BAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+                                  int sm_count, cudaStream_t s, int n_tiles, int n_chunks, const MultiView& mv,
+                                  const SeArgs& se = SeArgs{}) {
+  const size_t smem = SmemLayoutT<STAGES, OBUF, SE>::total + 1024;
+  cudaError_t e = cudaFuncSetAttribute(fit_tc_kernel<STAGES, OBUF, MULTI, BAL, SE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   const int grid = BAL ? (int)((a.n + mv.bal_rows - 1) / mv.bal_rows) : (n_tiles < sm_count ? n_tiles : sm_count);
-  fit_tc_kernel<STAGES, OBUF, MULTI, BAL><<<grid, THREADS, smem, s>>>(tl, d, a, pending_count, n_tiles, n_chunks, mv);
+  fit_tc_kernel<STAGES, OBUF, MULTI, BAL, SE><<<grid, THREADS, smem, s>>>(tl, d, a, pending_count, n_tiles, n_chunks, mv, se);
   return cudaGetLastError();
 }
 
@@ -639,6 +697,14 @@ cudaError_t launch_fit_tc(const DesignView& d, const FitArgs& a, const TcLaunch&
   }
   return two ? launch_variant<6, 2, false>(d, a, tl, pending_count, sm_count, s, n_tiles, n_chunks, none)
              : launch_variant<8, 1, false>(d, a, tl, pending_count, sm_count, s, n_tiles, n_chunks, none);
+}
+
+cudaError_t launch_fit_tc_se(const DesignView& d, const FitArgs& a, const TcLaunch& tl, uint32_t* pending_count,
+                             int sm_count, cudaStream_t s, const SeArgs& se) {
+  if (a.n <= 0) return cudaSuccess;
+  const int n_tiles = (int)((a.n + TILE_M - 1) / TILE_M);
+  return launch_variant<8, 1, false, false, true>(d, a, tl, pending_count, sm_count, s, n_tiles, d.t_pad / KC,
+                                                  MultiView{}, se);
 }
 
 }  // namespace mmf

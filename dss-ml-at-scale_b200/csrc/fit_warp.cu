@@ -87,12 +87,20 @@ __device__ __forceinline__ float dot16(const float4& a0, const float4& a1, const
   return s;
 }
 
+__device__ __forceinline__ double warp_sum_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
 // One masked series: Gram (down)date over the row, in-order Cholesky with pivot dropping, two solves.
 // `b` (moments, identical in every lane) in, gamma out; returns the status.  Deliberately not inlined
 // into the S-unrolled paths: it is the rare path and would quadruple the hot loop's I-cache footprint.
+// SE: zz = |z|^2 of the forward solve (= b'gamma); the factor stays in scr.G for the se rows.
+template <bool SE>
 __device__ __noinline__ int solve_masked(const DesignView& d, const ARows& A, const float* __restrict__ yr,
                                          int nmiss, const unsigned short* __restrict__ miss_list,
-                                         WarpScratch& scr, float (&g)[P], int lane) {
+                                         WarpScratch& scr, float (&g)[P], int lane, float& zz, unsigned& omask) {
   const int t_fit = d.t_fit;
   int pi[DPL], pj[DPL];
 #pragma unroll
@@ -180,13 +188,14 @@ __device__ __noinline__ int solve_masked(const DesignView& d, const ARows& A, co
   __syncwarp();
   // right-looking Cholesky, lane -> (row i = lane&15, column half h = lane>>4)
   const int ri = lane & 15, ch = lane >> 4;
-  unsigned dropped = 0u;
+  unsigned dropped = 0u, kept_cols = 0u;
 #pragma unroll 1
   for (int j = 0; j < P; ++j) {
     const float dj = scr.G[j][j];
     const float d0 = scr.diag0[j];
     const bool globally_out = !((d.kept_mask >> j) & 1u);
     const bool keep = !globally_out && d0 > 0.f && dj > MMF_PIVOT_TOL * d0;
+    if (SE && keep) kept_cols |= 1u << j;
     __syncwarp();
     if (keep) {
       const float inv = rsqrtf(dj);
@@ -213,6 +222,7 @@ __device__ __noinline__ int solve_masked(const DesignView& d, const ARows& A, co
     __syncwarp();
   }
   const unsigned outmask = dropped | ~d.kept_mask;
+  if (SE) omask = ~kept_cols & 0xFFFFu;              // also the columns no observed row touches (pivot 0)
 #pragma unroll 1
   for (int j = 0; j < P; ++j) {                                   // forward solve L z = b
     float zj = 0.f;
@@ -220,6 +230,13 @@ __device__ __noinline__ int solve_masked(const DesignView& d, const ARows& A, co
     __syncwarp();
     if (lane == j) scr.b[j] = zj;
     if (lane > j && lane < P) scr.b[lane] = fmaf(-scr.G[lane][j], zj, scr.b[lane]);
+    __syncwarp();
+  }
+  if (SE) {
+    float s = 0.f;
+#pragma unroll
+    for (int j = 0; j < P; ++j) s = fmaf(scr.b[j], scr.b[j], s);
+    zz = s;
     __syncwarp();
   }
 #pragma unroll 1
@@ -237,8 +254,39 @@ __device__ __noinline__ int solve_masked(const DesignView& d, const ARows& A, co
   return dropped ? MMF_STATUS_RANKDEF : MMF_STATUS_OK;
 }
 
+// se row of one series after solve_masked: h_t = |L^-1 a_t|^2 with the factor in scr.G, lanes over the rows
+__device__ __forceinline__ void se_row_masked(const DesignView& d, const FitArgs& a, const SeArgs& se, const ARows& A,
+                                              const WarpScratch& scr, unsigned outmask, float sig, int64_t row,
+                                              int lane) {
+  float rinv[P];                                  // 1 / L_jj once per series: no division per prediction row
+#pragma unroll
+  for (int j = 0; j < P; ++j) rinv[j] = ((outmask >> j) & 1u) ? 0.f : 1.f / scr.G[j][j];
+#pragma unroll 1
+  for (int k = lane; k < a.n_pred; k += 32) {
+    const int t = a.pred_start + k;
+    const float4 a0 = A.vec(0, t), a1 = A.vec(1, t), a2 = A.vec(2, t), a3 = A.vec(3, t);
+    const float av[P] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w, a2.x, a2.y, a2.z, a2.w, a3.x, a3.y, a3.z, a3.w};
+    float w[P];
+    float h = 0.f;
+#pragma unroll
+    for (int j = 0; j < P; ++j) {
+      float s = av[j];
+#pragma unroll
+      for (int q = 0; q < j; ++q) s = fmaf(-scr.G[j][q], w[q], s);
+      w[j] = s * rinv[j];
+      h = fmaf(w[j], w[j], h);
+    }
+    se.out_se[row * se.ld_se + k] = sig * sqrtf(1.f + h);
+  }
+}
+
+__device__ __forceinline__ float sigma_of(double ss, double bg, int dof) {
+  return dof > 0 ? static_cast<float>(sqrt(fmax(ss - bg, 0.0) / dof)) : __int_as_float(0x7fc00000);
+}
+
+template <bool SE>
 __global__ void __launch_bounds__(THREADS, 1)
-fit_warp_kernel(const DesignView d, const FitArgs a, const int smem_rows) {
+fit_warp_kernel(const DesignView d, const FitArgs a, const int smem_rows, const SeArgs se) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   // programmatic dependent launch: this kernel may have been scheduled before its producer finished; its work starts
   // once the producer has completed.  (Releasing ITS dependent -- solve_rows_kernel -- early as well was measured: the
@@ -302,11 +350,13 @@ fit_warp_kernel(const DesignView d, const FitArgs a, const int smem_rows) {
     // ---- moments of the S series
     float acc[S][P];
     int miss[S];
+    double ssq[S];                                   // SE: S = sum (y - c)^2 over the observed rows (f64: no restarts)
     if (lane < S) scr.miss_n[lane] = 0;
     __syncwarp();
 #pragma unroll
     for (int s = 0; s < S; ++s) {
       miss[s] = 0;
+      ssq[s] = 0.0;
 #pragma unroll
       for (int p = 0; p < P; ++p) acc[s][p] = 0.f;
     }
@@ -336,6 +386,7 @@ fit_warp_kernel(const DesignView d, const FitArgs a, const int smem_rows) {
               if (pos < MISS_CAP) scr.miss_t[s][pos] = (unsigned short)t;
             }
             MMF_DOT16(acc[s], a0, a1, a2, a3, r)
+            if (SE) ssq[s] = fma(static_cast<double>(r), static_cast<double>(r), ssq[s]);
           }
         }
       }
@@ -348,14 +399,16 @@ fit_warp_kernel(const DesignView d, const FitArgs a, const int smem_rows) {
         if (!((d.kept_mask >> p) & 1u)) acc[s][p] = 0.f;         // fully observed: G_i = I, gamma = b
       }
       miss[s] = __reduce_add_sync(0xffffffffu, miss[s]);
+      if (SE) ssq[s] = warp_sum_d(ssq[s]);
     }
 
     __syncwarp();                                    // missing positions recorded by other lanes are visible now
     // ---- series with gaps: per-series normal equations (rare path, one copy of the code)
     int st[S];
     bool deferred[S];
+    bool se_done[S];                                 // SE: sigma / dof / se row already written by the masked solve
 #pragma unroll
-    for (int s = 0; s < S; ++s) { st[s] = any[s] ? MMF_STATUS_OK : MMF_STATUS_EMPTY; deferred[s] = false; }
+    for (int s = 0; s < S; ++s) { st[s] = any[s] ? MMF_STATUS_OK : MMF_STATUS_EMPTY; deferred[s] = false; se_done[s] = false; }
 #pragma unroll 1
     for (int s = 0; s < S; ++s) {
       bool need = false;
@@ -379,6 +432,12 @@ fit_warp_kernel(const DesignView d, const FitArgs a, const int smem_rows) {
         if (lane < P) rec.b[lane] = bl;
         if (lane == P) {
           rec.c = cs;
+          if (SE) {
+            double sq = ssq[0];
+#pragma unroll
+            for (int q = 1; q < S; ++q) sq = (q == s) ? ssq[q] : sq;
+            rec.ss = static_cast<float>(sq);
+          }
           rec.nm[0] = (uint16_t)(nm < SOLVE_SEG ? nm : SOLVE_SEG);
           rec.nm[1] = (uint16_t)(nm < SOLVE_SEG ? 0 : nm - SOLVE_SEG);
           rec.cal = a.cal_id;
@@ -399,7 +458,9 @@ fit_warp_kernel(const DesignView d, const FitArgs a, const int smem_rows) {
         for (int q = 1; q < S; ++q) x = (q == s) ? acc[q][p] : x;
         g[p] = x;
       }
-      const int rs = solve_masked(d, A, yr0 + s * a.ld_y, nm, scr.miss_t[s], scr, g, lane);
+      float zz = 0.f;
+      unsigned outmask = 0u;
+      const int rs = solve_masked<SE>(d, A, yr0 + s * a.ld_y, nm, scr.miss_t[s], scr, g, lane, zz, outmask);
 #pragma unroll
       for (int q = 0; q < S; ++q) {
         if (q == s) {
@@ -407,6 +468,21 @@ fit_warp_kernel(const DesignView d, const FitArgs a, const int smem_rows) {
 #pragma unroll
           for (int p = 0; p < P; ++p) acc[q][p] = g[p];
         }
+      }
+      if (SE) {                                      // the factor is still in scr.G: this series' se row now
+        double sq = ssq[0];
+#pragma unroll
+        for (int q = 1; q < S; ++q) sq = (q == s) ? ssq[q] : sq;
+        const int dof = t_fit - nm - __popc(~outmask & 0xFFFFu);
+        const float sg = sigma_of(sq, static_cast<double>(zz), dof);
+        if (se.out_se != nullptr) se_row_masked(d, a, se, A, scr, outmask, sg, row0 + s, lane);
+        if (lane == 0) {
+          se.sigma[row0 + s] = sg;
+          if (se.dof != nullptr) se.dof[row0 + s] = dof;
+        }
+#pragma unroll
+        for (int q = 0; q < S; ++q) if (q == s) se_done[q] = true;
+        __syncwarp();                                // scr.G is read until here; the next series overwrites it
       }
     }
 
@@ -433,6 +509,24 @@ fit_warp_kernel(const DesignView d, const FitArgs a, const int smem_rows) {
         if (act[s] && !deferred[s]) {
           const float yhat = any[s] ? dot16(a0, a1, a2, a3, acc[s], c[s]) : qnan;
           store_out1(a, off0 + s * a.ld_out + k, yhat);
+        }
+      }
+    }
+    if (SE) {                                      // fully observed (G_i = I, b'gamma = |gamma|^2) and empty rows
+#pragma unroll
+      for (int s = 0; s < S; ++s) {
+        if (!act[s] || deferred[s] || se_done[s]) continue;
+        double bg = 0.0;
+#pragma unroll
+        for (int p = 0; p < P; ++p) bg = fma(static_cast<double>(acc[s][p]), static_cast<double>(acc[s][p]), bg);
+        const int dof = any[s] ? t_fit - __popc(d.kept_mask) : 0;
+        const float sg = sigma_of(ssq[s], bg, dof);
+        if (se.out_se != nullptr)
+          for (int k = lane; k < a.n_pred; k += 32)
+            se.out_se[(row0 + s) * se.ld_se + k] = sg * __ldg(se.sfac + a.pred_start + k);
+        if (lane == 0) {
+          se.sigma[row0 + s] = sg;
+          if (se.dof != nullptr) se.dof[row0 + s] = dof;
         }
       }
     }
@@ -468,14 +562,15 @@ size_t fit_warp_smem_bytes(const DesignView& d, int* smem_rows) {
   return (size_t)rows * 4 * sizeof(float4) + scratch;
 }
 
-cudaError_t launch_fit_warp(const DesignView& d, const FitArgs& a, int sm_count, cudaStream_t s) {
+cudaError_t launch_fit_warp(const DesignView& d, const FitArgs& a, int sm_count, cudaStream_t s, const SeArgs* se) {
   if (a.n <= 0) return cudaSuccess;
   int smem_rows = 0;
   const size_t smem = fit_warp_smem_bytes(d, &smem_rows);
-  cudaError_t e = cudaFuncSetAttribute(fit_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  auto kern = se != nullptr ? fit_warp_kernel<true> : fit_warp_kernel<false>;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   int per_sm = 0;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fit_warp_kernel, THREADS, smem);
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, THREADS, smem);
   if (e != cudaSuccess) return e;
   if (per_sm < 1) per_sm = 1;
   const int64_t groups = (a.n + S - 1) / S;
@@ -492,7 +587,7 @@ cudaError_t launch_fit_warp(const DesignView& d, const FitArgs& a, int sm_count,
   attr[0].val.programmaticStreamSerializationAllowed = a.only_pending ? 1 : 0;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, fit_warp_kernel, d, a, smem_rows);
+  return cudaLaunchKernelEx(&cfg, kern, d, a, smem_rows, se != nullptr ? *se : SeArgs{});
 }
 
 }  // namespace mmf

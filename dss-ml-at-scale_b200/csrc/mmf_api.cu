@@ -95,6 +95,7 @@ struct Plan {
   float* d_w = nullptr;
   float* d_ap_hi = nullptr;   // [n_rows][P] tf32-hi / tf32-lo of A: B operand of predict_tc_kernel
   float* d_ap_lo = nullptr;
+  float* d_sfac = nullptr;    // [n_rows] sqrt(1 + |a_t|^2) (float64 on the host): se of gap-free rows / sigma
   alignas(64) unsigned char tmap_at[128];
   alignas(64) unsigned char tmap_bhi[128];
   alignas(64) unsigned char tmap_blo[128];
@@ -179,6 +180,8 @@ struct mmf_ctx {
   size_t gamma_cap_bytes = 0;
   float* d_c = nullptr;
   size_t c_cap_bytes = 0;
+  float* d_sigma_scratch = nullptr;    // sigma of a standard-error call that did not ask for it (the holdout se rows need it)
+  size_t sigma_scratch_cap = 0;
   int32_t* d_status_scratch = nullptr;
   size_t status_scratch_cap = 0;
   void* d_pack_scratch = nullptr;      // sort / scan work space of the packer (grown on demand, kept)
@@ -202,6 +205,7 @@ void free_multi(MultiPlan& m) {
 
 void free_plan(Plan& p) {
   cudaFree(p.d_a4); cudaFree(p.d_at); cudaFree(p.d_apred); cudaFree(p.d_w); cudaFree(p.d_ap_hi); cudaFree(p.d_ap_lo);
+  cudaFree(p.d_sfac);
   p = Plan{};
 }
 
@@ -297,7 +301,8 @@ inline void split_tf32(float v, float* hi, float* lo) {
 // Enqueue the fit of ONE slab of device-resident rows on `s`.  status must be non-null.
 int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pred_start, int32_t n_pred,
                     float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s, int* launches,
-                    int* kernel_used, float* const* out_more, int n_out, int multimem, const SelectArgs* sel) {
+                    int* kernel_used, float* const* out_more, int n_out, int multimem, const SelectArgs* sel,
+                    const SeArgs* se = nullptr) {
   const DesignView d = view_of(ctx->plan);
   FitArgs a{};
   a.y = y; a.n = n; a.ld_y = ld_y; a.pred_start = pred_start; a.n_pred = n_pred;
@@ -358,7 +363,9 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
   // a pass of their own afterwards.  The work list starts out as -1; the producer publishes row indices into it.  It
   // only overlaps when a consumer block fits beside the fit CTA on an SM, which the fit kernel's register and shared
   // memory use (one CTA per SM) does not leave room for, so it is off by default.
-  const bool stream_solve = kernel == MMF_KERNEL_TC && may_mask && !capturing && n >= 32768 && ctx->cfg.stream_solve == 1;
+  // (standard-error calls always take the product configuration and the post-pass solve)
+  const bool stream_solve = kernel == MMF_KERNEL_TC && may_mask && !capturing && n >= 32768 && ctx->cfg.stream_solve == 1 &&
+                            se == nullptr;
   if (stream_solve) {
     if (!ctx->rec_rows_clean) CU_TRY(cudaMemsetAsync(ctx->d_rec_rows, 0xFF, ctx->rec_rows_cap_bytes, s));
     ctx->rec_rows_clean = true;                            // the call's closing solve_rows pass resets what it consumed
@@ -373,8 +380,17 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
       rc = encode_2d(tl.tmap_y8, y, (uint64_t)d.t_fit, (uint64_t)n, (uint64_t)ld_y * 4, 32, 8);
     if (rc != MMF_OK) return rc;
     memcpy(tl.tmap_at, ctx->plan.tmap_at, 128);
-    CU_TRY(launch_fit_tc(d, a, tl, counters, ctx->sm_count, s, ctx->cfg.tc_variant));
-    ++*launches;
+    if (se != nullptr) {
+      CU_TRY(launch_fit_tc_se(d, a, tl, counters, ctx->sm_count, s, *se));
+      ++*launches;
+      if (many_pred) {          // se rows of the rows fit_tc finished, before the passes behind it change any status
+        CU_TRY(launch_se_outer(a, *se, ctx->sm_count, s));
+        ++*launches;
+      }
+    } else {
+      CU_TRY(launch_fit_tc(d, a, tl, counters, ctx->sm_count, s, ctx->cfg.tc_variant));
+      ++*launches;
+    }
     if (may_mask) {
       FitArgs m = a;
       m.only_pending = 1;
@@ -383,15 +399,15 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
         CU_TRY(launch_solve_stream(d, m, ctx->sm_count, s));
         ++*launches;
       }
-      CU_TRY(launch_fit_warp(d, m, ctx->sm_count, s));
-      CU_TRY(launch_solve_rows(d, m, ctx->sm_count, s));    // records the general pass queued (and, without the
+      CU_TRY(launch_fit_warp(d, m, ctx->sm_count, s, se));
+      CU_TRY(launch_solve_rows(d, m, ctx->sm_count, s, nullptr, se));   // records the general pass queued (and, without the
       *launches += 2;                                        // streaming solve, all of them)
     }
   } else {
-    CU_TRY(launch_fit_warp(d, a, ctx->sm_count, s));
+    CU_TRY(launch_fit_warp(d, a, ctx->sm_count, s, se));
     ++*launches;
     if (may_mask) {
-      CU_TRY(launch_solve_rows(d, a, ctx->sm_count, s));
+      CU_TRY(launch_solve_rows(d, a, ctx->sm_count, s, nullptr, se));
       ++*launches;
     }
   }
@@ -443,7 +459,7 @@ int64_t slab_rows(const mmf_ctx* ctx, int64_t n) {
 int run_device(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pred_start, int32_t n_pred,
                float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s, int* launches,
                int* kernel_used, float* const* out_more = nullptr, int n_out = 1, int multimem = 0,
-               const SelectArgs* sel = nullptr, uint32_t* slab_pending = nullptr) {
+               const SelectArgs* sel = nullptr, uint32_t* slab_pending = nullptr, const SeArgs* se = nullptr) {
   const int64_t slab = slab_rows(ctx, n);
   for (int64_t off = 0, i = 0; off < n; off += slab, ++i) {
     const int64_t m = std::min(slab, n - off);
@@ -455,9 +471,16 @@ int run_device(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pr
       if (sel_slab.out_choice) sel_slab.out_choice += off;
       if (sel_slab.out_mse) sel_slab.out_mse += off;
     }
+    SeArgs se_slab{};
+    if (se != nullptr) {
+      se_slab = *se;
+      if (se_slab.out_se) se_slab.out_se += off * se_slab.ld_se;
+      se_slab.sigma += off;
+      if (se_slab.dof) se_slab.dof += off;
+    }
     const int rc = run_device_slab(ctx, y + off * ld_y, m, ld_y, pred_start, n_pred, out + off * ld_out, ld_out,
                                    beta ? beta + off * P : nullptr, status + off, s, launches, kernel_used, more, n_out,
-                                   multimem, sel != nullptr ? &sel_slab : nullptr);
+                                   multimem, sel != nullptr ? &sel_slab : nullptr, se != nullptr ? &se_slab : nullptr);
     if (rc != MMF_OK) return rc;
     if (slab_pending != nullptr) {
       if (*kernel_used == MMF_KERNEL_TC)
@@ -580,6 +603,7 @@ int mmf_destroy(mmf_ctx* ctx) {
   cudaFree(ctx->d_rec_rows);
   cudaFree(ctx->d_gamma);
   cudaFree(ctx->d_c);
+  cudaFree(ctx->d_sigma_scratch);
   cudaFree(ctx->d_status_scratch);
   cudaFree(ctx->d_pack_scratch);
   if (ctx->ev_a) cudaEventDestroy(ctx->ev_a);
@@ -673,6 +697,15 @@ int mmf_plan_design(mmf_ctx* ctx, const double* X, int32_t n_rows, int32_t p, in
   CU_TRY(cudaMalloc(&pl.d_ap_lo, A.size() * sizeof(float)));
   CU_TRY(cudaMemcpy(pl.d_ap_hi, ap_hi.data(), A.size() * sizeof(float), cudaMemcpyHostToDevice));
   CU_TRY(cudaMemcpy(pl.d_ap_lo, ap_lo.data(), A.size() * sizeof(float), cudaMemcpyHostToDevice));
+  // leverage of a gap-free series (G_i = I): h_t = |a_t|^2 over the kept columns (the others are zero in A)
+  std::vector<float> sfac(n_rows);
+  for (int32_t t = 0; t < n_rows; ++t) {
+    double h = 0.0;
+    for (int q = 0; q < P; ++q) h += (double)A[(size_t)t * P + q] * (double)A[(size_t)t * P + q];
+    sfac[t] = (float)std::sqrt(1.0 + h);
+  }
+  CU_TRY(cudaMalloc(&pl.d_sfac, sfac.size() * sizeof(float)));
+  CU_TRY(cudaMemcpy(pl.d_sfac, sfac.data(), sfac.size() * sizeof(float), cudaMemcpyHostToDevice));
   int rc = encode_2d(pl.tmap_at, pl.d_at, (uint64_t)pl.t_pad, (uint64_t)(2 * P), (uint64_t)pl.t_pad * 4, 32, 2 * P);
   if (rc != MMF_OK) return rc;
   rc = encode_2d(pl.tmap_bhi, pl.d_ap_hi, (uint64_t)P, (uint64_t)n_rows, (uint64_t)P * 4, P, 128, CU_TENSOR_MAP_SWIZZLE_64B);
@@ -981,6 +1014,77 @@ int mmf_fit_forecast_int(mmf_ctx* ctx, const void* y, int32_t dtype, int64_t n, 
                          mmf_stats* stats) {
   if (dtype == MMF_DT_F32) return fail(MMF_E_INVALID, "mmf_fit_forecast_int takes MMF_DT_I16 / U16 / I32; use mmf_fit_forecast_f32");
   return fit_forecast_impl(ctx, y, dtype, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_beta, out_status, stats);
+}
+
+int mmf_fit_forecast_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pred_start, int32_t n_pred,
+                            float* out_pred, int64_t ld_out, float* out_se, int64_t ld_se, float* out_sigma,
+                            int32_t* out_dof, int32_t* out_status, mmf_stats* stats) {
+  if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
+  GrowScope grow_scope(ctx);
+  if (!ctx->plan.valid) return fail(MMF_E_NOPLAN, "mmf_plan_design has not been called");
+  const Plan& pl = ctx->plan;
+  if (n < 0) return fail(MMF_E_INVALID, "n < 0");
+  if (n > 0 && (!y || !out_pred)) return fail(MMF_E_INVALID, "y or out_pred is NULL");
+  if (!out_se && !out_sigma && !out_dof)
+    return fail(MMF_E_INVALID, "out_se, out_sigma and out_dof are all NULL: use mmf_fit_forecast_f32");
+  if (ld_y < pl.t_fit) return fail(MMF_E_INVALID, "ld_y=%lld < t_fit=%d", (long long)ld_y, pl.t_fit);
+  if (n_pred < 1 || pred_start < 0 || (int64_t)pred_start + n_pred > pl.n_rows)
+    return fail(MMF_E_INVALID, "prediction rows [%d,%d) outside the planned design (%d rows)", pred_start,
+                pred_start + n_pred, pl.n_rows);
+  if (ld_out < n_pred) return fail(MMF_E_INVALID, "ld_out=%lld < n_pred=%d", (long long)ld_out, n_pred);
+  if (out_se && ld_se < n_pred) return fail(MMF_E_INVALID, "ld_se=%lld < n_pred=%d", (long long)ld_se, n_pred);
+  if (stats) memset(stats, 0, sizeof(*stats));
+  if (n == 0) return MMF_OK;
+  CU_TRY(cudaSetDevice(ctx->device));
+  if (!is_device_ptr(y) || !is_device_ptr(out_pred) || (out_se && !is_device_ptr(out_se)) ||
+      (out_sigma && !is_device_ptr(out_sigma)) || (out_dof && !is_device_ptr(out_dof)) ||
+      (out_status && !is_device_ptr(out_status)))
+    return fail(MMF_E_UNSUPPORTED, "mmf_fit_forecast_se_f32 takes device buffers only");
+  int32_t* status = out_status;
+  if (!status) {
+    int rc = grow_status_scratch(ctx, n, ctx->stream);
+    if (rc != MMF_OK) return rc;
+    status = ctx->d_status_scratch;
+  }
+  SeArgs se{};
+  se.out_se = out_se; se.ld_se = ld_se; se.sigma = out_sigma; se.dof = out_dof; se.sfac = pl.d_sfac;
+  if (!se.sigma) {
+    int rc = grow((void**)&ctx->d_sigma_scratch, &ctx->sigma_scratch_cap, (size_t)n * sizeof(float));
+    if (rc != MMF_OK) return rc;
+    se.sigma = ctx->d_sigma_scratch;
+  }
+  const int64_t slab = slab_rows(ctx, n);
+  const int64_t n_slabs = (n + slab - 1) / slab;
+  uint32_t* slab_pending = nullptr;
+  if (stats && n_slabs > 1) {
+    const mmf_ctx* saved = g_grow_ctx;
+    g_grow_ctx = nullptr;
+    const int rc = grow((void**)&ctx->d_slab_pending, &ctx->slab_pending_cap, (size_t)n_slabs * sizeof(uint32_t));
+    g_grow_ctx = saved;
+    if (rc != MMF_OK) return rc;
+    slab_pending = ctx->d_slab_pending;
+  }
+  int launches = 0, kernel_used = 0;
+  if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, ctx->stream));
+  int rc = run_device(ctx, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, nullptr, status, ctx->stream, &launches,
+                      &kernel_used, nullptr, 1, 0, nullptr, slab_pending, &se);
+  if (rc != MMF_OK) return rc;
+  if (stats) {
+    CU_TRY(cudaEventRecord(ctx->ev_k1, ctx->stream));
+    CU_TRY(cudaEventSynchronize(ctx->ev_k1));
+    CU_TRY(cudaEventElapsedTime(&stats->kernel_ms, ctx->ev_k0, ctx->ev_k1));
+    stats->total_ms = stats->kernel_ms;
+    std::vector<uint32_t> pend((size_t)n_slabs, 0u);
+    if (slab_pending != nullptr)
+      CU_TRY(cudaMemcpy(pend.data(), slab_pending, pend.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    else if (kernel_used == MMF_KERNEL_TC)
+      CU_TRY(cudaMemcpy(pend.data(), ctx->d_pending + CTR_WORDS * ctx->last_set, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    for (uint32_t v : pend) stats->n_pending += v;
+    stats->n_series = n;
+    stats->kernel_launches = launches;
+    stats->kernel_used = kernel_used;
+  }
+  return MMF_OK;
 }
 
 

@@ -72,7 +72,7 @@ struct SolveRec {
   uint16_t nm[2];                          // entries in each segment
   uint16_t miss_t[SOLVE_MISS_CAP];         // grid positions of the missing fit rows (byte offset 72)
   int32_t cal;                             // ragged launches: the series' calendar (index into MultiView::cals)
-  uint16_t pad_[2];
+  float ss;                                // standard-error calls: S = sum over the observed rows of (y - c)^2
 };
 static_assert(sizeof(SolveRec) == 256, "SolveRec is one 256-B record");
 static_assert(SOLVE_SEG % 4 == 0 && offsetof(SolveRec, miss_t) % 8 == 0, "position groups are aligned 8-B words");
@@ -109,14 +109,28 @@ struct FitArgs {
   int32_t cal_id;           //   ... and that calendar's index (written into the records the launch queues)
 };
 
+// Outputs of a standard-error call (mmf_fit_forecast_se_f32, DESIGN.md section 2 item 7).  Kernels take it as their
+// last parameter and read it only in their SE instantiation, so the plain instantiations are unchanged.
+struct SeArgs {
+  float* out_se;            // nullable [n, ld_se]: sigma * sqrt(1 + h_t) for the requested rows
+  int64_t ld_se;
+  float* sigma;             // [n] residual scale (never null inside the library: scratch if the caller passed NULL)
+  int32_t* dof;             // nullable [n]: n_obs - used columns
+  const float* sfac;        // [n_rows] sqrt(1 + |a_t|^2) of the planned design (gap-free rows: G_i = I)
+};
+
 // warp-per-series CUDA-core kernel (general path)
-cudaError_t launch_fit_warp(const DesignView& d, const FitArgs& a, int sm_count, cudaStream_t s);
+cudaError_t launch_fit_warp(const DesignView& d, const FitArgs& a, int sm_count, cudaStream_t s,
+                            const SeArgs* se = nullptr);
 size_t fit_warp_smem_bytes(const DesignView& d, int* smem_rows);
 
 // thread-per-series normal equations for the deferred masked rows: Gram downdate, in-order Cholesky with
 // pivot dropping and both triangular solves entirely in registers, then the forecasts
 cudaError_t launch_solve_rows(const DesignView& d, const FitArgs& a, int sm_count, cudaStream_t s,
-                              const CalMeta* cals = nullptr);
+                              const CalMeta* cals = nullptr, const SeArgs* se = nullptr);
+// se rows of the gap-free rows of a fit + predict_tc call: out_se[i, k] = sigma_i * sfac[pred_start + k] for every row
+// whose status is MMF_STATUS_OK right after fit_tc_kernel (launched before the passes that finish the other rows)
+cudaError_t launch_se_outer(const FitArgs& a, const SeArgs& se, int sm_count, cudaStream_t s);
 // the same solve as a CONSUMER that runs beside fit_tc_kernel (launched right behind it with programmatic stream
 // serialisation; fit_tc_kernel releases it once all its CTAs are resident): records are solved as the epilogue
 // publishes them, the kernel retires when the producer has finished and the work list is drained
@@ -157,6 +171,9 @@ int fit_tc_balanced_rows(int64_t n, int sm_count, int variant);
 cudaError_t launch_fit_tc(const DesignView& d, const FitArgs& a, const TcLaunch& tl,
                           uint32_t* pending_count, int sm_count, cudaStream_t s, int variant = 0,
                           const MultiView* multi = nullptr);
+// the product configuration <8, 1> with the standard-error outputs (SE instantiation)
+cudaError_t launch_fit_tc_se(const DesignView& d, const FitArgs& a, const TcLaunch& tl, uint32_t* pending_count,
+                             int sm_count, cudaStream_t s, const SeArgs& se);
 bool fit_tc_supported(const DesignView& d, const FitArgs& a, const char** why);
 
 // per-series model selection by hold-out MSE over nested whitened designs (select.cu)

@@ -191,7 +191,31 @@ predict_tc_kernel(const __grid_constant__ PredictLaunch pl, const DesignView d, 
   }
 }
 
+// Standard errors of the gap-free rows of a fit + predict_tc call: se[i, k] = sigma_i * sqrt(1 + h_{pred_start+k}), an
+// outer product and a pure HBM write (one warp per row, coalesced).  It runs right after fit_tc_kernel: MMF_STATUS_OK
+// then marks exactly the rows that kernel finished; the passes behind it write the se rows of all the others.
+__global__ void __launch_bounds__(256)
+se_outer_kernel(const int32_t* __restrict__ status, const float* __restrict__ sigma, const float* __restrict__ sfac,
+                int32_t pred_start, int32_t n_pred, int64_t n, float* __restrict__ out_se, int64_t ld_se) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warps = (int64_t)gridDim.x * 8;
+  for (int64_t row = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5); row < n; row += warps) {
+    if (status[row] != MMF_STATUS_OK) continue;
+    const float sg = sigma[row];
+    float* __restrict__ o = out_se + row * ld_se;
+    for (int k = lane; k < n_pred; k += 32) __stcs(o + k, sg * __ldg(sfac + pred_start + k));
+  }
+}
+
 }  // namespace
+
+cudaError_t launch_se_outer(const FitArgs& a, const SeArgs& se, int sm_count, cudaStream_t s) {
+  if (a.n <= 0 || se.out_se == nullptr) return cudaSuccess;
+  const int64_t want = (a.n + 7) / 8, cap = (int64_t)sm_count * 8;
+  se_outer_kernel<<<(unsigned)(want < cap ? want : cap), 256, 0, s>>>(a.status, se.sigma, se.sfac, a.pred_start, a.n_pred,
+                                                                     a.n, se.out_se, se.ld_se);
+  return cudaGetLastError();
+}
 
 cudaError_t launch_predict_tc(const DesignView& d, const FitArgs& a, const PredictLaunch& pl, int sm_count,
                               cudaStream_t s, const PredUnit* units, int64_t n_units_multi, const unsigned char* tmaps_out) {

@@ -19,9 +19,11 @@ __device__ __forceinline__ void ldg32b_nc(const float* p, float4& lo, float4& hi
 
 // b (moments over the observed rows) -> gamma, in place.  `load_group(seg, gi)` returns the gi-th 8-B group of four
 // gap positions of segment seg (SolveRec layout).  Returns the bit mask of columns dropped for rank deficiency.
-template <class LoadGroup>
+// `tail(G, outmask, zz)` runs last with the factor L still in G (packed, dropped columns: L_jj = 1, rest 0), the mask
+// of unused columns and zz = |z|^2 = b'gamma of the forward solve L z = b (what the standard errors need).
+template <class LoadGroup, class Tail>
 __device__ __forceinline__ unsigned masked_solve(const DesignView& d, float (&b)[P], int nm0, int nm1,
-                                                 LoadGroup load_group) {
+                                                 LoadGroup load_group, Tail tail) {
   float G[NPAIR];
 #pragma unroll
   for (int e = 0; e < NPAIR; ++e) G[e] = 0.f;
@@ -97,6 +99,9 @@ __device__ __forceinline__ unsigned masked_solve(const DesignView& d, float (&b)
     for (int q = 0; q < j; ++q) s = fmaf(-G[tri(j, q)], b[q], s);
     b[j] = ((outmask >> j) & 1u) ? 0.f : s / G[tri(j, j)];
   }
+  float zz = 0.f;
+#pragma unroll
+  for (int j = 0; j < P; ++j) zz = fmaf(b[j], b[j], zz);
 #pragma unroll
   for (int j = P - 1; j >= 0; --j) {
     float s = b[j];
@@ -104,7 +109,24 @@ __device__ __forceinline__ unsigned masked_solve(const DesignView& d, float (&b)
     for (int r = j + 1; r < P; ++r) s = fmaf(-G[tri(r, j)], b[r], s);
     b[j] = ((outmask >> j) & 1u) ? 0.f : s / G[tri(j, j)];
   }
+  tail(G, outmask, zz);
   return dropped;
+}
+
+// h = |L^-1 a|^2 over the used columns (G as handed to masked_solve's tail; rinv[j] = 1 / L_jj, 0 for an unused column):
+// one forward substitution, no division (the reciprocals are taken once per series, not once per prediction row)
+__device__ __forceinline__ float leverage_packed(const float (&G)[NPAIR], const float (&rinv)[P], const float (&av)[P]) {
+  float w[P];
+  float h = 0.f;
+#pragma unroll
+  for (int j = 0; j < P; ++j) {
+    float s = av[j];
+#pragma unroll
+    for (int q = 0; q < j; ++q) s = fmaf(-G[tri(j, q)], w[q], s);
+    w[j] = s * rinv[j];
+    h = fmaf(w[j], w[j], h);
+  }
+  return h;
 }
 
 }  // namespace mmf

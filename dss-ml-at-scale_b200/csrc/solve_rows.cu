@@ -25,9 +25,10 @@ __device__ __forceinline__ void prefetch_rec(const SolveRec* r) {
 }
 
 // One queued series: Gram downdate, Cholesky with pivot dropping, both solves, forecasts, status.
-template <bool MULTI>
+// SE: also sigma / dof from S (rec.ss) and |z|^2, and the se row with h_t = |L^-1 a_t|^2 from the row's own factor.
+template <bool MULTI, bool SE = false>
 __device__ __forceinline__ void solve_one(const DesignView& d0, const FitArgs& a, const CalMeta* __restrict__ cals,
-                                          const int64_t row, const bool vec_out) {
+                                          const int64_t row, const bool vec_out, const SeArgs& se = SeArgs{}) {
   const SolveRec& rec = a.recs[row];
   float b[P];
   {
@@ -53,9 +54,29 @@ __device__ __forceinline__ void solve_one(const DesignView& d0, const FitArgs& a
   }
 
   // ---- G_i = I - sum over the missing rows of a_t a_t^T, Cholesky with pivot dropping, both solves (solve_math.cuh)
-  const unsigned dropped = masked_solve(d, b, nm0, nm1, [&](int seg, int gi) {
+  auto load_group = [&](int seg, int gi) {
     return reinterpret_cast<const unsigned long long*>(rec.miss_t + seg * SOLVE_SEG)[gi];
-  });
+  };
+  auto se_tail = [&](const float (&G)[NPAIR], unsigned outmask, float zz) {
+    if (!SE) return;
+    const int dof = d.t_fit - nm0 - nm1 - __popc(~outmask & 0xFFFFu);
+    const double rss = fmax(static_cast<double>(rec.ss) - static_cast<double>(zz), 0.0);
+    const float sig = dof > 0 ? static_cast<float>(sqrt(rss / dof)) : __int_as_float(0x7fc00000);
+    se.sigma[row] = sig;
+    if (se.dof != nullptr) se.dof[row] = dof;
+    if (se.out_se == nullptr) return;
+    float rinv[P];
+#pragma unroll
+    for (int j = 0; j < P; ++j) rinv[j] = ((outmask >> j) & 1u) ? 0.f : 1.f / G[tri(j, j)];
+#pragma unroll 1
+    for (int k = 0; k < a.n_pred; ++k) {
+      const float4* ap = reinterpret_cast<const float4*>(d.apred + (size_t)(pred_start + k) * P);
+      const float4 a0 = __ldg(ap), a1 = __ldg(ap + 1), a2 = __ldg(ap + 2), a3 = __ldg(ap + 3);
+      const float av[P] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w, a2.x, a2.y, a2.z, a2.w, a3.x, a3.y, a3.z, a3.w};
+      se.out_se[row * se.ld_se + k] = sig * sqrtf(1.f + leverage_packed(G, rinv, av));
+    }
+  };
+  const unsigned dropped = masked_solve(d, b, nm0, nm1, load_group, se_tail);
 
   if (a.out_gamma != nullptr) {
     float4* gp = reinterpret_cast<float4*>(a.out_gamma + row * P);
@@ -104,9 +125,9 @@ __device__ __forceinline__ bool vec_out_ok(const FitArgs& a) {
 
 // The pass over the whole work list, after the producers have finished.  A record whose series is no longer
 // MMF_STATUS_DEFERRED was already solved by the streaming consumer below.
-template <bool MULTI>
+template <bool MULTI, bool SE = false>
 __global__ void __launch_bounds__(THREADS, 2)
-solve_rows_kernel(const DesignView d0, const FitArgs a, const CalMeta* __restrict__ cals) {
+solve_rows_kernel(const DesignView d0, const FitArgs a, const CalMeta* __restrict__ cals, const SeArgs se) {
   asm volatile("griddepcontrol.wait;" ::: "memory");    // programmatic dependent launch: the producer kernels are done
   const uint32_t count = min(*a.rec_count, a.rec_cap);
   const uint32_t stride = gridDim.x * THREADS;
@@ -124,7 +145,7 @@ solve_rows_kernel(const DesignView d0, const FitArgs a, const CalMeta* __restric
       a.rec_rows[i] = -1;                               // the work list of a streaming call is left as it was found: all -1
       if (a.status[row] != MMF_STATUS_DEFERRED) continue;
     }
-    solve_one<MULTI>(d0, a, cals, row, vec_out);
+    solve_one<MULTI, SE>(d0, a, cals, row, vec_out, se);
   }
 }
 
@@ -184,7 +205,8 @@ solve_stream_kernel(const DesignView d0, const FitArgs a) {
 
 }  // namespace
 
-cudaError_t launch_solve_rows(const DesignView& d, const FitArgs& a, int sm_count, cudaStream_t s, const CalMeta* cals) {
+cudaError_t launch_solve_rows(const DesignView& d, const FitArgs& a, int sm_count, cudaStream_t s, const CalMeta* cals,
+                              const SeArgs* se) {
   if (a.recs == nullptr || a.rec_cap == 0) return cudaSuccess;
   const int64_t want = ((int64_t)a.rec_cap + THREADS - 1) / THREADS;
   const int64_t cap = (int64_t)sm_count * 8;
@@ -199,8 +221,10 @@ cudaError_t launch_solve_rows(const DesignView& d, const FitArgs& a, int sm_coun
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  return cals != nullptr ? cudaLaunchKernelEx(&cfg, solve_rows_kernel<true>, d, a, cals)
-                         : cudaLaunchKernelEx(&cfg, solve_rows_kernel<false>, d, a, cals);
+  const SeArgs none{};
+  if (se != nullptr) return cudaLaunchKernelEx(&cfg, solve_rows_kernel<false, true>, d, a, cals, *se);
+  return cals != nullptr ? cudaLaunchKernelEx(&cfg, solve_rows_kernel<true>, d, a, cals, none)
+                         : cudaLaunchKernelEx(&cfg, solve_rows_kernel<false>, d, a, cals, none);
 }
 
 cudaError_t launch_solve_stream(const DesignView& d, const FitArgs& a, int sm_count, cudaStream_t s) {

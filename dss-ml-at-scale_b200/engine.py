@@ -387,6 +387,37 @@ class ForecastEngine:
                                  {N.KERNEL_WARP: "warp", N.KERNEL_TC: "tc"}.get(st.kernel_used, "?"))
         return res
 
+    def fit_forecast_se(self, y, pred_start: int, n_pred: int, want_stats: bool = False):
+        """``fit_forecast`` with prediction standard errors (``mmf_fit_forecast_se_f32``): ``y`` is a float32 CUDA
+        tensor.  Returns ``{"pred", "se", "sigma", "dof", "status"}`` (torch tensors on y's device): ``sigma[i]`` the
+        residual scale sqrt(RSS / dof), ``se[i, j] = sigma[i] * sqrt(1 + h)`` the standard error of a new observation
+        at design row ``pred_start + j`` (NaN where dof <= 0).  ``pred`` / ``status`` are bit-equal to ``fit_forecast``."""
+        import torch
+        if self.t_fit is None:
+            raise RuntimeError("plan()/plan_calendar() must be called first")
+        yp, n, t_have, ld_y = _describe(y, "y")
+        if not (_is_torch(y) and y.is_cuda and y.dtype == torch.float32) or t_have < self.t_fit:
+            raise ValueError(f"y must be a float32 CUDA tensor with at least t_fit={self.t_fit} columns")
+        self.set_stream(torch.cuda.current_stream(y.device).cuda_stream)
+
+        def table():            # 16-B row pitch: the tensor-core store paths
+            return torch.empty((n, (n_pred + 3) & ~3), device=y.device, dtype=torch.float32)[:, :n_pred]
+
+        out, se = table(), table()
+        sigma = torch.empty(n, device=y.device, dtype=torch.float32)
+        dof = torch.empty(n, device=y.device, dtype=torch.int32)
+        status = torch.empty(n, device=y.device, dtype=torch.int32)
+        st = N.MmfStats() if want_stats else None
+        N.check(self._lib.mmf_fit_forecast_se_f32(self._h, yp, n, ld_y, int(pred_start), int(n_pred), out.data_ptr(),
+                                                  out.stride(0), se.data_ptr(), se.stride(0), sigma.data_ptr(),
+                                                  dof.data_ptr(), status.data_ptr(),
+                                                  C.byref(st) if st is not None else None))
+        res = {"pred": out, "se": se, "sigma": sigma, "dof": dof, "status": status}
+        if st is not None:
+            self.launches += st.kernel_launches
+            res["stats"] = Stats(st.kernel_ms, st.total_ms, st.n_series, st.n_pending, st.h2d_bytes, st.d2h_bytes,
+                                 st.kernel_launches, {N.KERNEL_WARP: "warp", N.KERNEL_TC: "tc"}.get(st.kernel_used, "?"))
+        return res
 
     def capture(self, y, pred_start: int, n_pred: int, out=None, status=None):
         """Record one device-resident ``fit_forecast`` call as a CUDA graph.  Small batches are launch-bound (three

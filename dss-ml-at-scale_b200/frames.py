@@ -30,11 +30,15 @@ EXO_FIELDS = ("covid", "christmas", "new_year")   # 02:431
 
 
 # ---- schemas (02:360-370, 02:498-506) as pyarrow; pyspark StructTypes on demand ---------
-def tuning_schema(keys=DEFAULT_KEYS, date_col="Date", value_col="Demand"):
+def tuning_schema(keys=DEFAULT_KEYS, date_col="Date", value_col="Demand", interval: bool = False):
+    """``interval=True``: the schema of ``forecast_groups(..., interval=level)``, with ``{value}_Lower`` /
+    ``{value}_Upper`` float32 columns behind ``{value}_Fitted``."""
     import pyarrow as pa
 
+    extra = [(value_col + "_Lower", pa.float32()), (value_col + "_Upper", pa.float32())] if interval else []
     return pa.schema([(k, pa.string()) for k in keys]
-                     + [(date_col, pa.date32()), (value_col, pa.float32()), (value_col + "_Fitted", pa.float32())])
+                     + [(date_col, pa.date32()), (value_col, pa.float32()), (value_col + "_Fitted", pa.float32())]
+                     + extra)
 
 
 def enriched_schema(keys=DEFAULT_KEYS, date_col="Date", value_col="Demand"):
@@ -314,19 +318,32 @@ def _fit_buckets_ragged(buckets, eng, freq, horizon, mode, design, on_device):
     for i, b in enumerate(buckets):
         y_host = b.y.cpu().numpy() if on_device else b.y
         n_pred = horizon if mode == "future" else b.t_len
-        yield b, dates[i], n_pred, y_host, np.ascontiguousarray(pred[int(rows[i]):int(rows[i + 1]), :n_pred])
+        yield b, dates[i], n_pred, y_host, np.ascontiguousarray(pred[int(rows[i]):int(rows[i + 1]), :n_pred]), None
 
 
-def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device):
-    """Run the engine over every bucket: yields (bucket, out_days, n_pred, y_host, pred_host)."""
+def _host(x):
+    return x.cpu().numpy() if hasattr(x, "cpu") else np.asarray(x)
+
+
+def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, interval=False):
+    """Run the engine over every bucket: yields (bucket, out_days, n_pred, y_host, pred_host, se_host or None).
+    ``interval``: prediction standard errors too (``fit_forecast_se``), one call per calendar bucket."""
+    if interval and select is not None:
+        raise ValueError("interval= is not offered with select= (model selection returns point forecasts)")
     t_fit_min = min((b.t_len - (horizon if mode == "holdout" else 0)) for b in buckets) if buckets else 0
-    if (select is None and len(buckets) >= RAGGED_MIN_BUCKETS and (mode == "holdout" or 1 <= horizon <= 64)
+    if (select is None and not interval and len(buckets) >= RAGGED_MIN_BUCKETS and (mode == "holdout" or 1 <= horizon <= 64)
             and hasattr(eng, "fit_forecast_ragged") and t_fit_min >= 33 and all(b.t_len <= 65535 for b in buckets)):
         yield from _fit_buckets_ragged(buckets, eng, freq, horizon, mode, design, on_device)
         return
     for b in buckets:
         out_days, pred_start, n_pred = eng.plan_calendar(b.start, b.t_len, freq, horizon, mode, design)
-        if select is not None:
+        se = None
+        if interval:
+            from .engine import device_packed
+            yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
+            res = eng.fit_forecast_se(yd, pred_start, n_pred)
+            pred, se = _host(res["pred"]), _host(res["se"])
+        elif select is not None:
             if mode != "holdout":
                 raise ValueError("select= needs mode='holdout' (the held-out rows score the candidates)")
             from .engine import device_packed
@@ -337,7 +354,25 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device):
             if on_device:
                 pred = pred.cpu().numpy()
         y_host = b.y.cpu().numpy() if on_device else b.y
-        yield b, out_days, n_pred, y_host, pred
+        yield b, out_days, n_pred, y_host, pred, se
+
+
+def _z_of(interval):
+    """normal quantile of a two-sided interval at level ``interval`` (what SARIMAX's conf_int uses); None: no interval"""
+    if interval is None:
+        return None
+    from statistics import NormalDist
+    level = float(interval)
+    if not 0.0 < level < 1.0:
+        raise ValueError(f"interval must be a level in (0, 1), got {interval!r}")
+    return NormalDist().inv_cdf(0.5 + level / 2.0)
+
+
+def _bounds(pred, se, z):
+    """(lower, upper) float32 rows of pred -+ z * se"""
+    p = np.asarray(pred, dtype=np.float64).reshape(-1)
+    s = np.asarray(se, dtype=np.float64).reshape(-1)
+    return (p - z * s).astype(np.float32), (p + z * s).astype(np.float32)
 
 
 def _global_order(buckets, keys, lengths):
@@ -436,7 +471,7 @@ def _single_group_fast(pdf, keys, date_col, value_col, freq, horizon, mode, desi
 def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Demand",
                     freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                     engine: ForecastEngine | None = None, pack: str = "host", select=None,
-                    null_keys_on_gaps: bool = False) -> pd.DataFrame:
+                    null_keys_on_gaps: bool = False, interval=None) -> pd.DataFrame:
     """Fit + forecast every group in ``pdf``; returns ``tuning_schema`` rows
     (keys..., Date, Demand, Demand_Fitted), groups in key order, dates ascending.
 
@@ -456,17 +491,24 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     key columns from the re-indexed frame (02:490), so rows that ``asfreq`` inserted for missing dates carry NaN in
     ``Product`` / ``SKU``.  By default the keys are filled on every row (a grid row without a ``Demand`` is still
     that group's row); with the option, rows whose ``Demand`` is missing get null keys.
+
+    ``interval=0.9`` appends float32 ``Demand_Lower`` / ``Demand_Upper`` = ``Demand_Fitted -+ z * se`` with the normal
+    quantile ``z = NormalDist().inv_cdf(0.5 + level / 2)`` and ``se`` the prediction standard error of each row
+    (``ForecastEngine.fit_forecast_se``; NaN where a series has no residual degrees of freedom).  Every calendar bucket
+    then takes its own call.  ``interval=None`` leaves the frame as it was.
     """
     eng = engine or default_engine()
     keys = list(keys)
     fitted_col = value_col + "_Fitted"
-    if pack == "host" and select is None and isinstance(pdf, pd.DataFrame):
+    z = _z_of(interval)
+    if pack == "host" and select is None and z is None and isinstance(pdf, pd.DataFrame):
         one = _single_group_fast(pdf, keys, date_col, value_col, freq, horizon, mode, design, eng, null_keys_on_gaps)
         if one is not None:
             return one
     buckets = _buckets_for(pdf, keys, date_col, value_col, freq, pack, eng)
     parts, lengths = [], []
-    for b, out_days, n_pred, y_host, pred in _fit_buckets(buckets, eng, freq, horizon, mode, design, select, pack == "device"):
+    for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
+                                                              pack == "device", z is not None):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n), n_pred)
         # key columns keep the dtype they came in with (no per-row string inference on N x T values)
@@ -477,6 +519,8 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
         else:
             frame[value_col] = np.full(n * n_pred, np.nan, dtype=np.float32)
         frame[fitted_col] = pred.reshape(-1)
+        if z is not None:
+            frame[value_col + "_Lower"], frame[value_col + "_Upper"] = _bounds(pred, se, z)
         if null_keys_on_gaps and mode == "holdout":
             gap = np.isnan(frame[value_col])
             if gap.any():
@@ -485,9 +529,11 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
         parts.append(pd.DataFrame(frame))
         lengths.append(n_pred)
     if not parts:
+        bounds = ({value_col + "_Lower": pd.Series(dtype=np.float32), value_col + "_Upper": pd.Series(dtype=np.float32)}
+                  if z is not None else {})
         return pd.DataFrame({**{k: pd.Series(dtype=object) for k in keys},
                              date_col: pd.Series(dtype="datetime64[ns]"),
-                             value_col: pd.Series(dtype=np.float32), fitted_col: pd.Series(dtype=np.float32)})
+                             value_col: pd.Series(dtype=np.float32), fitted_col: pd.Series(dtype=np.float32), **bounds})
     if len(parts) == 1:
         return parts[0]
     out = pd.concat(parts, ignore_index=True)
@@ -497,20 +543,24 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
 def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Demand",
                    freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                    engine: ForecastEngine | None = None, pack: str = "host", select=None,
-                   null_keys_on_gaps: bool = False):
+                   null_keys_on_gaps: bool = False, interval=None):
     """Arrow ``Table``/``RecordBatch`` in -> Arrow ``Table`` with ``tuning_schema`` out (the ``mapInArrow``
     flavour of the boundary).  No pandas frame of the rows on either side: keys are dictionary-encoded on the way
-    in and expanded from a dictionary on the way out, dates and values are NumPy views of Arrow buffers."""
+    in and expanded from a dictionary on the way out, dates and values are NumPy views of Arrow buffers.
+    ``interval=level`` adds the ``{value}_Lower`` / ``{value}_Upper`` columns of ``forecast_groups`` (schema:
+    ``tuning_schema(..., interval=True)``)."""
     import pyarrow as pa
 
     if isinstance(table, pa.RecordBatch):
         table = pa.Table.from_batches([table])
     eng = engine or default_engine()
     keys = list(keys)
-    schema = tuning_schema(keys, date_col, value_col)
+    z = _z_of(interval)
+    schema = tuning_schema(keys, date_col, value_col, interval=z is not None)
     buckets = _buckets_for(table, keys, date_col, value_col, freq, pack, eng)
     parts, lengths = [], []
-    for b, out_days, n_pred, y_host, pred in _fit_buckets(buckets, eng, freq, horizon, mode, design, select, pack == "device"):
+    for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
+                                                              pack == "device", z is not None):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n, dtype=np.int32), n_pred)
         cols = []
@@ -528,6 +578,8 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
         cols.append(pa.array(np.tile(day32, n)).cast(pa.date32()))
         cols.append(pa.array(demand, from_pandas=True))               # NaN -> null, like the pandas route
         cols.append(pa.array(np.ascontiguousarray(pred).reshape(-1), from_pandas=True))
+        if z is not None:
+            cols.extend(pa.array(v, from_pandas=True) for v in _bounds(pred, se, z))
         parts.append(pa.Table.from_arrays(cols, schema=schema))
         lengths.append(n_pred)
     if not parts:

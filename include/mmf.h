@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define MMF_VERSION 102          /* 0.1.2 */
+#define MMF_VERSION 103          /* 0.1.3 */
 #define MMF_P 16                 /* design columns (zero-pad narrower designs) */
 #define MMF_PIVOT_TOL 1e-3f      /* per-series relative Cholesky pivot threshold */
 #define MMF_CAL_TOL 1e-10        /* aliasing threshold on the float64 calendar Gram */
@@ -156,6 +156,25 @@ int mmf_fit_forecast_int(mmf_ctx* ctx, const void* y, int32_t dtype, int64_t n, 
                          int32_t pred_start, int32_t n_pred,
                          float* out_pred, int64_t ld_out,
                          float* out_beta, int32_t* out_status, mmf_stats* stats);
+
+/* The same fit with prediction standard errors for forecast intervals (DESIGN.md section 2 item 7).  For series i,
+ * with n_obs its finite fit values, k the whitened columns its fit uses and S = sum over them of (y_t - c_i)^2:
+ *   out_sigma[i] = sqrt(RSS / dof), RSS = S - b'gamma (clamped at 0), out_dof[i] = dof = n_obs - k;
+ *                  NaN (and dof <= 0) when dof <= 0, in particular for empty series (status 1: dof = 0)
+ *   out_se[i, j] = sigma_i * sqrt(1 + h_t), h_t = a_t' G_i^-1 a_t over the used columns, t = pred_start + j:
+ *                  the least-squares standard error of a new observation at design row t (leverage included)
+ * out_pred and out_status are bit-equal to mmf_fit_forecast_f32 on the same inputs.  out_se [n, ld_se] (ld_se >=
+ * n_pred; only columns [0, n_pred) of a row are written), out_sigma [n], out_dof [n] are each nullable, but not all
+ * three.  Device buffers only (host pointers: MMF_E_UNSUPPORTED); enqueue-only unless `stats` is non-NULL.  The
+ * call always runs the product tensor-core configuration and solves series with gaps in a pass of their own after
+ * it, whatever mmf_config.tc_variant and stream_solve say; mmf_config.kernel is honoured.
+ * replaces: the forecast variance / conf_int() the reference's per-group SARIMAX model offers beside the mean. */
+int mmf_fit_forecast_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y,
+                            int32_t pred_start, int32_t n_pred,
+                            float* out_pred, int64_t ld_out,
+                            float* out_se, int64_t ld_se,
+                            float* out_sigma, int32_t* out_dof,
+                            int32_t* out_status, mmf_stats* stats);
 
 /* ---- ragged batches: groups on MANY calendars in one launch ---------------------------------------------
  * The reference re-indexes every group on its own calendar (sort_values + asfreq per group, 02:422-423), so one

@@ -13,8 +13,8 @@ from . import design, synth, sharding, packer, sink         # noqa: F401
 from ._native import LIB_PATH, MmfError, device_count, load as load_library   # noqa: F401
 from .engine import (ForecastEngine, Stats, alloc_packed, bind_to_gpu_numa, default_engine, device_packed, forecast_packed,
                      pinned_empty, release_pinned_pool, to_integer_demand)  # noqa: F401
-from .frames import (DEFAULT_KEYS, EXO_FIELDS, FORECAST_HORIZON, add_exo_variables, enriched_schema,   # noqa: F401
-                     forecast_arrow_batches, forecast_groups, forecast_table, pack_groups, spark_schemas,
-                     split_train_score_data, tuning_schema)
+from .frames import (DEFAULT_KEYS, EXO_FIELDS, FORECAST_HORIZON, add_exo_variables, backtest_groups,  # noqa: F401
+                     backtest_schema, enriched_schema, forecast_arrow_batches, forecast_groups, forecast_table,
+                     pack_groups, spark_schemas, split_train_score_data, tuning_schema)
 
 __version__ = "0.1.0"

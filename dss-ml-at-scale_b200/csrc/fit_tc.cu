@@ -99,6 +99,30 @@ __device__ __forceinline__ float centring_constant(const float* __restrict__ yro
 
 __device__ __forceinline__ bool is_finite_bits(float x) { return (__float_as_uint(x) & 0x7f800000u) != 0x7f800000u; }
 
+// Backtest: a consumer group's running moments of its four fragment rows at origin k -> bt.mom, folded (hi + lo
+// columns, plus the restarted accumulators' sum in the tile's slot) exactly like the tile's hand-off to the epilogue.
+__device__ __forceinline__ void bt_write_moments(const BtArgs& bt, int k, int grp, int64_t n, const TileRec& tr, int frow0,
+                                                 int t4, const float (&acc)[2][P], bool folded, const float* sacc) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int rt = 64 * h + frow0 + 8 * j;
+      if (rt >= tr.nrows) continue;
+      float* __restrict__ dst = bt.mom + (((int64_t)k * 2 + grp) * n + tr.row0 + rt) * P + 2 * t4;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int q = 4 * i + 2 * j;                    // acc[h][q + 8] is the lo column of acc[h][q]
+        float2 v = make_float2(acc[h][q] + acc[h][q + P / 2], acc[h][q + 1] + acc[h][q + 1 + P / 2]);
+        if (folded) {
+          const float2 o = *reinterpret_cast<const float2*>(sacc + rt * P + 8 * i + 2 * t4);
+          v.x = o.x + v.x; v.y = o.y + v.y;
+        }
+        *reinterpret_cast<float2*>(dst + 8 * i) = v;
+      }
+    }
+}
+
 __device__ __forceinline__ float lds32(uint32_t addr) {
   float v;
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
@@ -113,13 +137,17 @@ __device__ __forceinline__ float lds32(uint32_t addr) {
 // Rows are independent in the GEMM, so the forecasts are bit-identical to the round-robin launch's.
 // SE (standard-error calls, single calendar): the consumers also sum S = sum (y - c)^2 of their fragment rows and the
 // epilogue writes sigma / dof (and the se row in future mode) of the gap-free rows; the MMA inputs are unchanged.
-template <int STAGES, int OBUF, bool MULTI, bool BAL, bool SE = false>
+// BT (backtest calls, single calendar, d = the longest window t_K): a consumer group writes its running moments to
+// bt.mom at every earlier origin t_k -- a chunk that contains t_k is issued twice, first with its values at t >= t_k
+// zeroed, then with the complementary ones -- and the epilogue finishes every origin of a row (DESIGN.md section 4.12).
+template <int STAGES, int OBUF, bool MULTI, bool BAL, bool SE = false, bool BT = false>
 __global__ void __launch_bounds__(THREADS, 1)
 fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const FitArgs a,
               uint32_t* __restrict__ pending_count, const int n_tiles_all, const int n_chunks, const MultiView mv,
-              const SeArgs se) {
+              const SeArgs se, const BtArgs bt) {
   static_assert(!(MULTI && BAL), "ragged launches carry their own tile table");
   static_assert(!SE || !(MULTI || BAL), "standard errors are built for the single-calendar round-robin launch");
+  static_assert(!BT || !(MULTI || BAL || SE), "backtests are built for the single-calendar round-robin launch");
   using SmemLayout = SmemLayoutT<STAGES, OBUF, SE>;
   // BAL: this CTA's rows; its k-th tile keeps the round-robin loop index blockIdx.x + k * gridDim.x
   const int64_t cta_row0 = BAL ? (int64_t)blockIdx.x * mv.bal_rows : 0;
@@ -331,6 +359,10 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
               packq = (packq >> 16) | (static_cast<unsigned long long>(tbase + pos) << 48);
               ++nm;
               if ((nm & 3) == 0 && nm <= SOLVE_SEG) *reinterpret_cast<unsigned long long*>(mt + nm - 4) = packq;
+              // BT: the first position the segment cannot hold, so that the epilogue can tell for every origin whether
+              // more than SOLVE_SEG of its gaps fall into the segment (kept in the record's `ss` word, unused here)
+              if constexpr (BT) if (nm == SOLVE_SEG + 1)
+                reinterpret_cast<uint16_t*>(&a.recs[(int64_t)tr.row0 + r].ss)[seg] = static_cast<uint16_t>(tbase + pos);
             }
           }
         }
@@ -362,6 +394,64 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
             if (SE) ssq[h][j] += static_cast<double>(part);
           }
         const uint64_t bdesc0 = gmma_desc_k_sw128(s_at + stage * AT_STAGE_BYTES);
+        uint32_t bt_in = 0;                             // BT: earlier origins strictly inside this chunk
+        if constexpr (BT) {
+          // origins in [start - 32, start]: this group's previous chunk ended at or below them and the other group's
+          // chunk lies in between, so the accumulator holds exactly this group's share of their moments (origins
+          // inside a chunk of this group are split below, origins beyond its last chunk written at the tile's end)
+          const int s0 = ch * KC;
+          uint32_t pre = 0;
+#pragma unroll
+          for (int k = 0; k < MMF_BT_MAX_ORIGINS - 1; ++k) {
+            pre |= (bt.t_orig[k] >= s0 - KC && bt.t_orig[k] <= s0 ? 1u : 0u) << k;
+            bt_in |= (bt.t_orig[k] > s0 && bt.t_orig[k] < s0 + KC ? 1u : 0u) << k;
+          }
+          while (pre) {
+            const int k = __ffs(pre) - 1;
+            pre &= pre - 1u;
+            bt_write_moments(bt, k, grp, a.n, tr, frow0, t4, acc, folded, sacc);
+          }
+        }
+        // (if constexpr, and the plain chunk below written out twice: the other instantiations must compile to exactly
+        // the code they had before the backtest existed)
+        if constexpr (BT) {
+        if (bt_in != 0u) {
+          // the chunk in column ranges [lo, hi) split at its origins: the A fragments of the other columns are zero,
+          // the B tiles are the stage's as always; after each range that ends at an origin the moments are written
+          int lo = 0;
+          uint32_t m = bt_in;
+          for (;;) {
+            const int k = m ? __ffs(m) - 1 : -1;
+            const int hi = k >= 0 ? __ldg(&bt.cals[k].t_fit) - ch * KC : KC;
+            wgmma_fence();
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int kk = 0; kk < KC / 8; ++kk) {
+                const uint64_t bdesc = bdesc0 + static_cast<uint64_t>(kk * 2);
+                uint32_t fh[4], fl[4];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {                 // element e: column 8 kk + 4 (e >> 1) + t4
+                  const int col = 8 * kk + 4 * (e >> 1) + t4;
+                  const bool in = col >= lo && col < hi;
+                  fh[e] = in ? ahi[h][kk][e] : 0u;
+                  fl[e] = in ? alo[h][kk][e] : 0u;
+                }
+                wgmma_m64n32k8_tf32_rs(acc[h], fh, bdesc);
+#ifndef MMF_TC_NO_LO_TERM
+                wgmma_m64n32k8_tf32_rs(acc[h], fl, bdesc);
+#endif
+              }
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(acc[0]);
+            wgmma_fence_regs(acc[1]);
+            if (k < 0) break;
+            bt_write_moments(bt, k, grp, a.n, tr, frow0, t4, acc, folded, sacc);
+            m &= m - 1u;
+            lo = hi;
+          }
+        } else {
         wgmma_fence();
 #pragma unroll
         for (int h = 0; h < 2; ++h)
@@ -377,6 +467,24 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
         wgmma_wait<0>();
         wgmma_fence_regs(acc[0]);
         wgmma_fence_regs(acc[1]);
+        }
+        } else {
+        wgmma_fence();
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int kk = 0; kk < KC / 8; ++kk) {
+            const uint64_t bdesc = bdesc0 + static_cast<uint64_t>(kk * 2);       // +32 B (16-B units)
+            wgmma_m64n32k8_tf32_rs(acc[h], ahi[h][kk], bdesc);
+#ifndef MMF_TC_NO_LO_TERM      // negative-control build (tests): without the lo term the path is tf32-grade and must FAIL parity
+            wgmma_m64n32k8_tf32_rs(acc[h], alo[h][kk], bdesc);
+#endif
+          }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc[0]);
+        wgmma_fence_regs(acc[1]);
+        }
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_empty(stage));   // this warp's MMAs and smem reads of the stage are done
         if (++since_fold == FOLD_CHUNKS && ch + NGROUPS < tr.n_chunks) {   // more chunks follow: fold and restart
@@ -403,6 +511,17 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
       if (scan && (nm & 3) != 0 && nm < SOLVE_SEG) {    // flush the partial group (right-aligned: oldest first)
         uint16_t* __restrict__ mt = a.recs[(int64_t)tr.row0 + r].miss_t + seg * SOLVE_SEG;
         *reinterpret_cast<unsigned long long*>(mt + (nm & ~3)) = packq >> (16 * (4 - (nm & 3)));
+      }
+      if constexpr (BT) {                                         // earlier origins at or beyond the end of this group's last chunk
+        const int s_end = ((tr.n_chunks - 1 - seg) / NGROUPS * NGROUPS + seg + 1) * KC;
+        uint32_t rest = 0;
+#pragma unroll
+        for (int k = 0; k < MMF_BT_MAX_ORIGINS - 1; ++k) rest |= (bt.t_orig[k] != INT32_MAX && bt.t_orig[k] >= s_end ? 1u : 0u) << k;
+        while (rest) {
+          const int k = __ffs(rest) - 1;
+          rest &= rest - 1u;
+          bt_write_moments(bt, k, grp, a.n, tr, frow0, t4, acc, folded, sacc);
+        }
       }
       // hand the tile's partial moments (hi and lo columns folded: b = D[:, p] + D[:, P + p]) to the epilogue
       if (!folded) mbar_wait(bar_accempty(ab), ((lt >> 1) & 1) ^ 1u);  // epilogue of tile lt-2 has drained this slot
@@ -492,6 +611,115 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
       // gaps the consumer warpgroups saw in this tile, by chunk parity
       const unsigned f0 = s_nm[(ab * NGROUPS + 0) * TILE_M + r], f1 = s_nm[(ab * NGROUPS + 1) * TILE_M + r];
       const double ss = SE ? s_ss[(ab * NGROUPS + 0) * TILE_M + r] + s_ss[(ab * NGROUPS + 1) * TILE_M + r] : 0.0;
+      if constexpr (BT) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_accempty(ab));   // g, f0 and f1 are in registers
+        // every origin of the row by the plain epilogue's rules, with origin k's own gap counts and t_k; the last
+        // origin (t_K) is the tile's hand-off itself, the earlier ones the two groups' moments in bt.mom
+        for (int k = 0; k < bt.n_origin; ++k) {
+          const bool last = k == bt.n_origin - 1;
+          const int4 m0 = __ldg(reinterpret_cast<const int4*>(bt.cals + k));   // {t_k, n_chunks, n_rows, kept_mask}
+          const int tk = m0.x;
+          float gk[P];
+          if (last || !live) {
+#pragma unroll
+            for (int p = 0; p < P; ++p) gk[p] = g[p];
+          } else {
+            const float4* p0 = reinterpret_cast<const float4*>(bt.mom + (((int64_t)k * NGROUPS + 0) * a.n + row) * P);
+            const float4* p1 = reinterpret_cast<const float4*>(bt.mom + (((int64_t)k * NGROUPS + 1) * a.n + row) * P);
+#pragma unroll
+            for (int q = 0; q < P / 4; ++q) {
+              const float4 u = p0[q], w = p1[q];
+              gk[4 * q] = u.x + w.x; gk[4 * q + 1] = u.y + w.y; gk[4 * q + 2] = u.z + w.z; gk[4 * q + 3] = u.w + w.w;
+            }
+          }
+          // gaps below t_k per segment: a prefix of the positions recorded in the last origin's record (ascending per
+          // segment); a segment that overflowed holds its first SOLVE_SEG positions and, in `ss`, the next one
+          const SolveRec* __restrict__ src = collect ? a.recs + row : nullptr;
+          int n0 = f0 & 0x7fff, n1 = f1 & 0x7fff;
+          bool over = false;
+          if (collect && !last && live && (n0 | n1) != 0) {
+#pragma unroll
+            for (int sg = 0; sg < 2; ++sg) {
+              const int tot = sg ? n1 : n0;
+              const uint16_t* mt = src->miss_t + sg * SOLVE_SEG;
+              const int have = tot < SOLVE_SEG ? tot : SOLVE_SEG;
+              int cnt = 0;
+              while (cnt < have && mt[cnt] < tk) ++cnt;
+              if (cnt == SOLVE_SEG && tot > SOLVE_SEG && reinterpret_cast<const uint16_t*>(&src->ss)[sg] < tk) over = true;
+              if (sg) n1 = cnt; else n0 = cnt;
+            }
+          }
+          bool general = false;
+          if (collect)
+            general = ((f0 | f1) & 0x8000u) != 0u || over || n0 > SOLVE_SEG || n1 > SOLVE_SEG || 2 * (n0 + n1) > tk;
+          bool finite = true;
+#pragma unroll
+          for (int p = 0; p < P; ++p) {
+            finite = finite && is_finite_bits(gk[p]);
+            if (!((kept_mask >> p) & 1u)) gk[p] = 0.f;
+          }
+          const bool pend = live && (!finite || general);
+          const bool defer = live && !pend && (n0 + n1) > 0;
+          const unsigned pm = __ballot_sync(0xffffffffu, pend);
+          if (lane == 0 && pm != 0u) {
+            atomicAdd(pending_count, __popc(pm));
+            atomicAdd(bt.pending + k, __popc(pm));
+          }
+          const unsigned dm = __ballot_sync(0xffffffffu, defer);
+          if (dm != 0u) {
+            unsigned base = 0;
+            if (lane == 0) base = atomicAdd(bt.rec_count + k, __popc(dm));
+            base = __shfl_sync(0xffffffffu, base, 0);
+            if (defer) {
+              SolveRec& rec = bt.recs[(int64_t)k * a.n + row];
+              float bk[P];
+              if (last) {
+#pragma unroll
+                for (int p = 0; p < P; ++p) bk[p] = gk[p];
+              } else {                                  // into origin k's own basis: b^(k) = T_k^T b_k
+                const float* __restrict__ tm = bt.tmat + (size_t)k * P * P;
+#pragma unroll
+                for (int p = 0; p < P; ++p) {
+                  float s = 0.f;
+#pragma unroll
+                  for (int q = 0; q < P; ++q) s = fmaf(__ldg(tm + q * P + p), gk[q], s);
+                  bk[p] = s;
+                }
+                for (int sg = 0; sg < 2; ++sg) {
+                  const int cnt = sg ? n1 : n0;
+                  for (int e = 0; e < cnt; ++e) rec.miss_t[sg * SOLVE_SEG + e] = src->miss_t[sg * SOLVE_SEG + e];
+                }
+              }
+              float4* bp = reinterpret_cast<float4*>(rec.b);
+              bp[0] = make_float4(bk[0], bk[1], bk[2], bk[3]);    bp[1] = make_float4(bk[4], bk[5], bk[6], bk[7]);
+              bp[2] = make_float4(bk[8], bk[9], bk[10], bk[11]);  bp[3] = make_float4(bk[12], bk[13], bk[14], bk[15]);
+              rec.c = c;
+              rec.nm[0] = static_cast<uint16_t>(n0);
+              rec.nm[1] = static_cast<uint16_t>(n1);
+              rec.cal = k;
+              const unsigned slot = base + __popc(dm & ((1u << lane) - 1u));
+              if (slot < a.rec_cap) bt.rec_rows[(int64_t)k * a.n + slot] = row;
+            }
+          }
+          if (live && !pend && !defer) {
+            const float* __restrict__ pk = bt.pred + (size_t)k * a.n_pred * P;
+            const int64_t off = ((int64_t)k * bt.out_kstride + row) * a.ld_out;
+            if (vec_out) {
+              for (int j = 0; j < a.n_pred; j += 4) {
+                float o[4];
+#pragma unroll
+                for (int w = 0; w < 4; ++w) o[w] = dot16(pk + (j + w) * P, gk, c);
+                store_out4(a, off + j, make_float4(o[0], o[1], o[2], o[3]));
+              }
+            } else {
+              for (int j = 0; j < a.n_pred; ++j) store_out1(a, off + j, dot16(pk + j * P, gk, c));
+            }
+          }
+          if (live) a.status[(int64_t)k * bt.st_kstride + row] = pend ? MMF_STATUS_PENDING : (defer ? MMF_STATUS_DEFERRED : MMF_STATUS_OK);
+        }
+        continue;
+      }
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_accempty(ab));     // the consumers may overwrite this slot now
       int nm0 = 0, nm1 = 0;
@@ -657,15 +885,15 @@ bool fit_tc_supported(const DesignView& d, const FitArgs& a, const char** why) {
   return w == nullptr;
 }
 
-template <int STAGES, int OBUF, bool MULTI, bool BAL = false, bool SE = false>
+template <int STAGES, int OBUF, bool MULTI, bool BAL = false, bool SE = false, bool BT = false>
 static cudaError_t launch_variant(const DesignView& d, const FitArgs& a, const TcLaunch& tl, uint32_t* pending_count,
                                   int sm_count, cudaStream_t s, int n_tiles, int n_chunks, const MultiView& mv,
-                                  const SeArgs& se = SeArgs{}) {
+                                  const SeArgs& se = SeArgs{}, const BtArgs& bt = BtArgs{}) {
   const size_t smem = SmemLayoutT<STAGES, OBUF, SE>::total + 1024;
-  cudaError_t e = cudaFuncSetAttribute(fit_tc_kernel<STAGES, OBUF, MULTI, BAL, SE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaError_t e = cudaFuncSetAttribute(fit_tc_kernel<STAGES, OBUF, MULTI, BAL, SE, BT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   const int grid = BAL ? (int)((a.n + mv.bal_rows - 1) / mv.bal_rows) : (n_tiles < sm_count ? n_tiles : sm_count);
-  fit_tc_kernel<STAGES, OBUF, MULTI, BAL, SE><<<grid, THREADS, smem, s>>>(tl, d, a, pending_count, n_tiles, n_chunks, mv, se);
+  fit_tc_kernel<STAGES, OBUF, MULTI, BAL, SE, BT><<<grid, THREADS, smem, s>>>(tl, d, a, pending_count, n_tiles, n_chunks, mv, se, bt);
   return cudaGetLastError();
 }
 
@@ -705,6 +933,14 @@ cudaError_t launch_fit_tc_se(const DesignView& d, const FitArgs& a, const TcLaun
   const int n_tiles = (int)((a.n + TILE_M - 1) / TILE_M);
   return launch_variant<8, 1, false, false, true>(d, a, tl, pending_count, sm_count, s, n_tiles, d.t_pad / KC,
                                                   MultiView{}, se);
+}
+
+cudaError_t launch_fit_tc_bt(const DesignView& d, const FitArgs& a, const TcLaunch& tl, uint32_t* pending_count,
+                             int sm_count, cudaStream_t s, const BtArgs& bt) {
+  if (a.n <= 0) return cudaSuccess;
+  const int n_tiles = (int)((a.n + TILE_M - 1) / TILE_M);
+  return launch_variant<8, 1, false, false, false, true>(d, a, tl, pending_count, sm_count, s, n_tiles, d.t_pad / KC,
+                                                         MultiView{}, SeArgs{}, bt);
 }
 
 }  // namespace mmf

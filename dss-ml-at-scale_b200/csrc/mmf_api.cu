@@ -131,6 +131,18 @@ struct MultiPlan {
   const void* key_y = nullptr;  int64_t key_n = -1, key_ld = -1;  std::vector<int64_t> key_rows;
 };
 
+// Backtest plan (DESIGN.md section 4.12): the longest window [0, t_K) is the basis the tensor-core kernel accumulates in;
+// origin k is calendar k of a stacked plan (its own whitening, t_fit = t_k), which the general passes use as they are.
+struct BtPlan {
+  bool valid = false;
+  int32_t n_origin = 0, horizon = 0;
+  int32_t origin[MMF_BT_MAX_ORIGINS] = {};
+  Plan common;
+  MultiPlan cals;
+  float* d_pred = nullptr;             // [K][horizon][P] origin k's prediction rows in the common basis, T_k a^(k)_t
+  float* d_tmat = nullptr;             // [K][P][P] T_k = W^-1 W_k
+};
+
 constexpr int NBUF = 3;
 
 struct Staging {
@@ -188,6 +200,12 @@ struct mmf_ctx {
   size_t pack_scratch_cap = 0;
   Plan plan;
   MultiPlan multi;
+  BtPlan bt;
+  float* d_bt_mom = nullptr;  size_t bt_mom_cap = 0;   // backtest scratch, per slab: moments at the earlier origins,
+  SolveRec* d_bt_recs = nullptr;  size_t bt_recs_cap = 0;   // [K][slab] records, [K][slab] work lists,
+  int64_t* d_bt_rows = nullptr;  size_t bt_rows_cap = 0;
+  uint32_t* d_bt_ctr = nullptr;  size_t bt_ctr_cap = 0;     // {records queued[K], rows left to the general pass[K]},
+  float* d_bt_pred = nullptr;  size_t bt_pred_cap = 0;      // forecasts when the caller did not ask for them
   Staging st[NBUF];
   NarrowPool* narrow_pool = nullptr;   // created on the first host-buffer call that narrows
   HostSlot hslot[NHOST];
@@ -207,6 +225,13 @@ void free_plan(Plan& p) {
   cudaFree(p.d_a4); cudaFree(p.d_at); cudaFree(p.d_apred); cudaFree(p.d_w); cudaFree(p.d_ap_hi); cudaFree(p.d_ap_lo);
   cudaFree(p.d_sfac);
   p = Plan{};
+}
+
+void free_bt(BtPlan& b) {
+  free_plan(b.common);
+  free_multi(b.cals);
+  cudaFree(b.d_pred); cudaFree(b.d_tmat);
+  b = BtPlan{};
 }
 
 // Scratch that a captured CUDA graph points into must not move: while ctx->pinned > 0 a reallocation is refused.
@@ -296,6 +321,159 @@ inline void split_tf32(float v, float* hi, float* lo) {
   memcpy(hi, &hb, 4);
   float l = v - *hi;
   uint32_t lb; memcpy(&lb, &l, 4); lb &= 0xFFFFE000u; memcpy(lo, &lb, 4);
+}
+
+// The device tables of one calendar (mmf_plan_design; the common basis of a backtest plan).  X is validated.
+int build_plan(Plan& pl, const double* X, int32_t n_rows, int32_t p, int32_t t_fit, int32_t has_constant) {
+
+  // ---- float64 calendar Gram, in-order Cholesky with aliasing, A = X W (whiten_calendar above)
+  pl.n_rows = n_rows;
+  pl.n_rows_pad = (n_rows + 31) & ~31;
+  pl.t_fit = t_fit;
+  pl.t_pad = (t_fit + 31) & ~31;
+  pl.has_constant = has_constant ? 1 : 0;
+  std::vector<float> A;
+  whiten_calendar(X, n_rows, p, t_fit, pl.W, &pl.kept_mask, A);
+  std::vector<float> a4((size_t)4 * pl.n_rows_pad * 4, 0.f);
+  for (int32_t t = 0; t < n_rows; ++t)
+    for (int q = 0; q < P; ++q) a4[(((size_t)(q >> 2) * pl.n_rows_pad) + t) * 4 + (q & 3)] = A[(size_t)t * P + q];
+  std::vector<float> at((size_t)2 * P * pl.t_pad, 0.f);
+  for (int32_t t = 0; t < t_fit; ++t)
+    for (int q = 0; q < P; ++q) {
+      const float v = A[(size_t)t * P + q];
+      uint32_t hb; memcpy(&hb, &v, 4); hb &= 0xFFFFE000u;
+      float hi; memcpy(&hi, &hb, 4);
+      float lo = v - hi;
+      uint32_t lb; memcpy(&lb, &lo, 4); lb &= 0xFFFFE000u; memcpy(&lo, &lb, 4);
+      at[(size_t)q * pl.t_pad + t] = hi;
+      at[(size_t)(P + q) * pl.t_pad + t] = lo;
+    }
+  float w32[P * P];
+  for (int i = 0; i < P * P; ++i) w32[i] = (float)pl.W[i];
+  std::vector<float> ap_hi(A.size()), ap_lo(A.size());
+  for (size_t i = 0; i < A.size(); ++i) {
+    const float v = A[i];
+    uint32_t hb; memcpy(&hb, &v, 4); hb &= 0xFFFFE000u;
+    float hi; memcpy(&hi, &hb, 4);
+    float lo = v - hi;
+    uint32_t lb; memcpy(&lb, &lo, 4); lb &= 0xFFFFE000u; memcpy(&lo, &lb, 4);
+    ap_hi[i] = hi; ap_lo[i] = lo;
+  }
+
+  CU_TRY(cudaMalloc(&pl.d_a4, a4.size() * sizeof(float)));
+  CU_TRY(cudaMalloc(&pl.d_at, at.size() * sizeof(float)));
+  CU_TRY(cudaMalloc(&pl.d_apred, A.size() * sizeof(float)));
+  CU_TRY(cudaMalloc(&pl.d_w, sizeof(w32)));
+  CU_TRY(cudaMemcpy(pl.d_a4, a4.data(), a4.size() * sizeof(float), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy(pl.d_at, at.data(), at.size() * sizeof(float), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy(pl.d_apred, A.data(), A.size() * sizeof(float), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy(pl.d_w, w32, sizeof(w32), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMalloc(&pl.d_ap_hi, A.size() * sizeof(float)));
+  CU_TRY(cudaMalloc(&pl.d_ap_lo, A.size() * sizeof(float)));
+  CU_TRY(cudaMemcpy(pl.d_ap_hi, ap_hi.data(), A.size() * sizeof(float), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy(pl.d_ap_lo, ap_lo.data(), A.size() * sizeof(float), cudaMemcpyHostToDevice));
+  // leverage of a gap-free series (G_i = I): h_t = |a_t|^2 over the kept columns (the others are zero in A)
+  std::vector<float> sfac(n_rows);
+  for (int32_t t = 0; t < n_rows; ++t) {
+    double h = 0.0;
+    for (int q = 0; q < P; ++q) h += (double)A[(size_t)t * P + q] * (double)A[(size_t)t * P + q];
+    sfac[t] = (float)std::sqrt(1.0 + h);
+  }
+  CU_TRY(cudaMalloc(&pl.d_sfac, sfac.size() * sizeof(float)));
+  CU_TRY(cudaMemcpy(pl.d_sfac, sfac.data(), sfac.size() * sizeof(float), cudaMemcpyHostToDevice));
+  int rc = encode_2d(pl.tmap_at, pl.d_at, (uint64_t)pl.t_pad, (uint64_t)(2 * P), (uint64_t)pl.t_pad * 4, 32, 2 * P);
+  if (rc != MMF_OK) return rc;
+  rc = encode_2d(pl.tmap_bhi, pl.d_ap_hi, (uint64_t)P, (uint64_t)n_rows, (uint64_t)P * 4, P, 128, CU_TENSOR_MAP_SWIZZLE_64B);
+  if (rc != MMF_OK) return rc;
+  rc = encode_2d(pl.tmap_blo, pl.d_ap_lo, (uint64_t)P, (uint64_t)n_rows, (uint64_t)P * 4, P, 128, CU_TENSOR_MAP_SWIZZLE_64B);
+  if (rc != MMF_OK) return rc;
+  pl.valid = true;
+  return MMF_OK;
+}
+
+// Stack the whitened designs of n_cal calendars (mmf_plan_calendars; the origins of a backtest plan).  Validates the
+// calendars, then waits for the stream `sync` before it frees the previous tables of `m`.
+int build_multi(MultiPlan& m, const double* X_all, int32_t n_cal, const int32_t* n_rows, const int32_t* t_fit,
+                const int32_t* pred_start, const int32_t* n_pred_cal, int32_t p, int32_t has_constant, bool many,
+                int32_t n_pred, int32_t n_pred_max, cudaStream_t sync) {
+  size_t total_rows = 0;
+  int32_t tmax = 0, tmin = INT32_MAX;
+  for (int c = 0; c < n_cal; ++c) {
+    if (t_fit[c] < 33 || t_fit[c] > 65535 || n_rows[c] < t_fit[c])
+      return fail(MMF_E_UNSUPPORTED, "calendar %d: need 33 <= t_fit <= 65535 and n_rows >= t_fit (t_fit=%d n_rows=%d)", c, t_fit[c], n_rows[c]);
+    if (pred_start[c] < 0 || pred_start[c] + n_pred_cal[c] > n_rows[c])
+      return fail(MMF_E_INVALID, "calendar %d: prediction rows [%d,%d) outside its %d design rows", c, pred_start[c],
+                  pred_start[c] + n_pred_cal[c], n_rows[c]);
+    total_rows += (size_t)n_rows[c];
+    tmax = std::max(tmax, t_fit[c]);
+    tmin = std::min(tmin, t_fit[c]);
+  }
+  for (size_t i = 0; i < total_rows * (size_t)p; ++i)
+    if (!std::isfinite(X_all[i])) return fail(MMF_E_INVALID, "design matrix has a non-finite entry at %zu", i);
+  CU_TRY(cudaStreamSynchronize(sync));
+  free_multi(m);
+  m.n_cal = n_cal; m.n_pred = many ? 1 : n_pred; m.has_constant = has_constant ? 1 : 0;
+  m.many_pred = many; m.n_pred_max = n_pred_max;
+  m.t_fit_max = tmax; m.t_pad_max = (tmax + 31) & ~31; m.min_chunks = (tmin + 31) / 32;
+  m.cals.resize(n_cal);
+  m.a4_off.resize(n_cal);
+  std::vector<float> at((size_t)n_cal * 2 * P * m.t_pad_max, 0.f), apred(total_rows * P);
+  size_t a4_total = 0;
+  for (int c = 0; c < n_cal; ++c) { m.a4_off[c] = a4_total; a4_total += (size_t)4 * ((n_rows[c] + 31) & ~31); }
+  std::vector<float> a4(a4_total * 4, 0.f);
+  size_t row_off = 0;
+  std::vector<float> A;
+  double W[P * P];
+  for (int c = 0; c < n_cal; ++c) {
+    const double* X = X_all + row_off * (size_t)p;
+    if (has_constant)
+      for (int32_t t = 0; t < n_rows[c]; ++t)
+        if (X[(size_t)t * p] != 1.0) return fail(MMF_E_INVALID, "has_constant=1 but calendar %d has X[%d,0] != 1", c, t);
+    CalMeta& cm = m.cals[c];
+    whiten_calendar(X, n_rows[c], p, t_fit[c], W, &cm.kept_mask, A);
+    cm.t_fit = t_fit[c]; cm.n_chunks = (t_fit[c] + 31) / 32; cm.n_rows = n_rows[c];
+    cm.row_off = (int32_t)row_off; cm.pred_start = pred_start[c]; cm.n_pred = n_pred_cal[c]; cm.n_rows_pad = (n_rows[c] + 31) & ~31;
+    memcpy(apred.data() + row_off * P, A.data(), A.size() * sizeof(float));
+    float* atc = at.data() + (size_t)c * 2 * P * m.t_pad_max;
+    for (int32_t t = 0; t < t_fit[c]; ++t)
+      for (int q = 0; q < P; ++q) split_tf32(A[(size_t)t * P + q], atc + (size_t)q * m.t_pad_max + t, atc + (size_t)(P + q) * m.t_pad_max + t);
+    float* a4c = a4.data() + m.a4_off[c] * 4;
+    for (int32_t t = 0; t < n_rows[c]; ++t)
+      for (int q = 0; q < P; ++q) a4c[(((size_t)(q >> 2) * cm.n_rows_pad) + t) * 4 + (q & 3)] = A[(size_t)t * P + q];
+    row_off += (size_t)n_rows[c];
+  }
+  if (row_off > (size_t)INT32_MAX) return fail(MMF_E_UNSUPPORTED, "too many design rows in one ragged plan");
+  CU_TRY(cudaMalloc(&m.d_cals, (size_t)n_cal * sizeof(CalMeta)));
+  CU_TRY(cudaMalloc(&m.d_at, at.size() * sizeof(float)));
+  CU_TRY(cudaMalloc(&m.d_apred, apred.size() * sizeof(float)));
+  CU_TRY(cudaMalloc(&m.d_a4, a4.size() * sizeof(float)));
+  CU_TRY(cudaMalloc(&m.d_w, P * P * sizeof(float)));
+  CU_TRY(cudaMalloc(&m.d_pending_by_cal, (size_t)n_cal * sizeof(uint32_t)));
+  CU_TRY(cudaMalloc(&m.d_tmaps_y, (size_t)n_cal * 128));
+  CU_TRY(cudaMemcpy(m.d_cals, m.cals.data(), (size_t)n_cal * sizeof(CalMeta), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy(m.d_at, at.data(), at.size() * sizeof(float), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy(m.d_apred, apred.data(), apred.size() * sizeof(float), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy(m.d_a4, a4.data(), a4.size() * sizeof(float), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemset(m.d_w, 0, P * P * sizeof(float)));
+  int rc = encode_2d(m.tmap_at, m.d_at, (uint64_t)m.t_pad_max, (uint64_t)n_cal * 2 * P, (uint64_t)m.t_pad_max * 4, 32, 2 * P);
+  if (rc != MMF_OK) return rc;
+  if (many) {
+    // B operand of predict_tc_kernel: tf32-hi / lo of every calendar's whitened rows, stacked (+128 zero rows: the last
+    // chunk of the last calendar reads a full box)
+    std::vector<float> hi((total_rows + 128) * P, 0.f), lo((total_rows + 128) * P, 0.f);
+    for (size_t i = 0; i < total_rows * P; ++i) split_tf32(apred[i], &hi[i], &lo[i]);
+    CU_TRY(cudaMalloc(&m.d_ap_hi, hi.size() * sizeof(float)));
+    CU_TRY(cudaMalloc(&m.d_ap_lo, lo.size() * sizeof(float)));
+    CU_TRY(cudaMemcpy(m.d_ap_hi, hi.data(), hi.size() * sizeof(float), cudaMemcpyHostToDevice));
+    CU_TRY(cudaMemcpy(m.d_ap_lo, lo.data(), lo.size() * sizeof(float), cudaMemcpyHostToDevice));
+    rc = encode_2d(m.tmap_bhi, m.d_ap_hi, (uint64_t)P, (uint64_t)(total_rows + 128), (uint64_t)P * 4, P, 128, CU_TENSOR_MAP_SWIZZLE_64B);
+    if (rc != MMF_OK) return rc;
+    rc = encode_2d(m.tmap_blo, m.d_ap_lo, (uint64_t)P, (uint64_t)(total_rows + 128), (uint64_t)P * 4, P, 128, CU_TENSOR_MAP_SWIZZLE_64B);
+    if (rc != MMF_OK) return rc;
+    CU_TRY(cudaMalloc(&m.d_tmaps_out, (size_t)n_cal * 128));
+  }
+  m.valid = true;
+  return MMF_OK;
 }
 
 // Enqueue the fit of ONE slab of device-resident rows on `s`.  status must be non-null.
@@ -584,6 +762,8 @@ int mmf_destroy(mmf_ctx* ctx) {
   cudaDeviceSynchronize();
   free_plan(ctx->plan);
   free_multi(ctx->multi);
+  free_bt(ctx->bt);
+  cudaFree(ctx->d_bt_mom); cudaFree(ctx->d_bt_recs); cudaFree(ctx->d_bt_rows); cudaFree(ctx->d_bt_ctr); cudaFree(ctx->d_bt_pred);
   for (int i = 0; i < NBUF; ++i) {
     Staging& s = ctx->st[i];
     cudaFree(s.d_y); cudaFree(s.d_yraw); cudaFree(s.d_out); cudaFree(s.d_beta); cudaFree(s.d_status);
@@ -649,71 +829,7 @@ int mmf_plan_design(mmf_ctx* ctx, const double* X, int32_t n_rows, int32_t p, in
   CU_TRY(cudaSetDevice(ctx->device));
   CU_TRY(cudaStreamSynchronize(ctx->stream));
   free_plan(ctx->plan);
-  Plan& pl = ctx->plan;
-
-  // ---- float64 calendar Gram, in-order Cholesky with aliasing, A = X W (whiten_calendar above)
-  pl.n_rows = n_rows;
-  pl.n_rows_pad = (n_rows + 31) & ~31;
-  pl.t_fit = t_fit;
-  pl.t_pad = (t_fit + 31) & ~31;
-  pl.has_constant = has_constant ? 1 : 0;
-  std::vector<float> A;
-  whiten_calendar(X, n_rows, p, t_fit, pl.W, &pl.kept_mask, A);
-  std::vector<float> a4((size_t)4 * pl.n_rows_pad * 4, 0.f);
-  for (int32_t t = 0; t < n_rows; ++t)
-    for (int q = 0; q < P; ++q) a4[(((size_t)(q >> 2) * pl.n_rows_pad) + t) * 4 + (q & 3)] = A[(size_t)t * P + q];
-  std::vector<float> at((size_t)2 * P * pl.t_pad, 0.f);
-  for (int32_t t = 0; t < t_fit; ++t)
-    for (int q = 0; q < P; ++q) {
-      const float v = A[(size_t)t * P + q];
-      uint32_t hb; memcpy(&hb, &v, 4); hb &= 0xFFFFE000u;
-      float hi; memcpy(&hi, &hb, 4);
-      float lo = v - hi;
-      uint32_t lb; memcpy(&lb, &lo, 4); lb &= 0xFFFFE000u; memcpy(&lo, &lb, 4);
-      at[(size_t)q * pl.t_pad + t] = hi;
-      at[(size_t)(P + q) * pl.t_pad + t] = lo;
-    }
-  float w32[P * P];
-  for (int i = 0; i < P * P; ++i) w32[i] = (float)pl.W[i];
-  std::vector<float> ap_hi(A.size()), ap_lo(A.size());
-  for (size_t i = 0; i < A.size(); ++i) {
-    const float v = A[i];
-    uint32_t hb; memcpy(&hb, &v, 4); hb &= 0xFFFFE000u;
-    float hi; memcpy(&hi, &hb, 4);
-    float lo = v - hi;
-    uint32_t lb; memcpy(&lb, &lo, 4); lb &= 0xFFFFE000u; memcpy(&lo, &lb, 4);
-    ap_hi[i] = hi; ap_lo[i] = lo;
-  }
-
-  CU_TRY(cudaMalloc(&pl.d_a4, a4.size() * sizeof(float)));
-  CU_TRY(cudaMalloc(&pl.d_at, at.size() * sizeof(float)));
-  CU_TRY(cudaMalloc(&pl.d_apred, A.size() * sizeof(float)));
-  CU_TRY(cudaMalloc(&pl.d_w, sizeof(w32)));
-  CU_TRY(cudaMemcpy(pl.d_a4, a4.data(), a4.size() * sizeof(float), cudaMemcpyHostToDevice));
-  CU_TRY(cudaMemcpy(pl.d_at, at.data(), at.size() * sizeof(float), cudaMemcpyHostToDevice));
-  CU_TRY(cudaMemcpy(pl.d_apred, A.data(), A.size() * sizeof(float), cudaMemcpyHostToDevice));
-  CU_TRY(cudaMemcpy(pl.d_w, w32, sizeof(w32), cudaMemcpyHostToDevice));
-  CU_TRY(cudaMalloc(&pl.d_ap_hi, A.size() * sizeof(float)));
-  CU_TRY(cudaMalloc(&pl.d_ap_lo, A.size() * sizeof(float)));
-  CU_TRY(cudaMemcpy(pl.d_ap_hi, ap_hi.data(), A.size() * sizeof(float), cudaMemcpyHostToDevice));
-  CU_TRY(cudaMemcpy(pl.d_ap_lo, ap_lo.data(), A.size() * sizeof(float), cudaMemcpyHostToDevice));
-  // leverage of a gap-free series (G_i = I): h_t = |a_t|^2 over the kept columns (the others are zero in A)
-  std::vector<float> sfac(n_rows);
-  for (int32_t t = 0; t < n_rows; ++t) {
-    double h = 0.0;
-    for (int q = 0; q < P; ++q) h += (double)A[(size_t)t * P + q] * (double)A[(size_t)t * P + q];
-    sfac[t] = (float)std::sqrt(1.0 + h);
-  }
-  CU_TRY(cudaMalloc(&pl.d_sfac, sfac.size() * sizeof(float)));
-  CU_TRY(cudaMemcpy(pl.d_sfac, sfac.data(), sfac.size() * sizeof(float), cudaMemcpyHostToDevice));
-  int rc = encode_2d(pl.tmap_at, pl.d_at, (uint64_t)pl.t_pad, (uint64_t)(2 * P), (uint64_t)pl.t_pad * 4, 32, 2 * P);
-  if (rc != MMF_OK) return rc;
-  rc = encode_2d(pl.tmap_bhi, pl.d_ap_hi, (uint64_t)P, (uint64_t)n_rows, (uint64_t)P * 4, P, 128, CU_TENSOR_MAP_SWIZZLE_64B);
-  if (rc != MMF_OK) return rc;
-  rc = encode_2d(pl.tmap_blo, pl.d_ap_lo, (uint64_t)P, (uint64_t)n_rows, (uint64_t)P * 4, P, 128, CU_TENSOR_MAP_SWIZZLE_64B);
-  if (rc != MMF_OK) return rc;
-  pl.valid = true;
-  return MMF_OK;
+  return build_plan(ctx->plan, X, n_rows, p, t_fit, has_constant);
 }
 
 int mmf_pin_scratch(mmf_ctx* ctx, int32_t delta) {
@@ -1104,86 +1220,9 @@ int mmf_plan_calendars(mmf_ctx* ctx, const double* X_all, int32_t n_cal, const i
     n_pred_max = std::max(n_pred_max, n_pred_cal[c]);
   }
   if (ctx->pinned > 0) return fail(MMF_E_UNSUPPORTED, "a captured CUDA graph pins this context");
-  size_t total_rows = 0;
-  int32_t tmax = 0, tmin = INT32_MAX;
-  for (int c = 0; c < n_cal; ++c) {
-    if (t_fit[c] < 33 || t_fit[c] > 65535 || n_rows[c] < t_fit[c])
-      return fail(MMF_E_UNSUPPORTED, "calendar %d: need 33 <= t_fit <= 65535 and n_rows >= t_fit (t_fit=%d n_rows=%d)", c, t_fit[c], n_rows[c]);
-    if (pred_start[c] < 0 || pred_start[c] + n_pred_cal[c] > n_rows[c])
-      return fail(MMF_E_INVALID, "calendar %d: prediction rows [%d,%d) outside its %d design rows", c, pred_start[c],
-                  pred_start[c] + n_pred_cal[c], n_rows[c]);
-    total_rows += (size_t)n_rows[c];
-    tmax = std::max(tmax, t_fit[c]);
-    tmin = std::min(tmin, t_fit[c]);
-  }
-  for (size_t i = 0; i < total_rows * (size_t)p; ++i)
-    if (!std::isfinite(X_all[i])) return fail(MMF_E_INVALID, "design matrix has a non-finite entry at %zu", i);
   CU_TRY(cudaSetDevice(ctx->device));
-  CU_TRY(cudaStreamSynchronize(ctx->stream));
-  free_multi(ctx->multi);
-  MultiPlan& m = ctx->multi;
-  m.n_cal = n_cal; m.n_pred = many ? 1 : n_pred; m.has_constant = has_constant ? 1 : 0;
-  m.many_pred = many; m.n_pred_max = n_pred_max;
-  m.t_fit_max = tmax; m.t_pad_max = (tmax + 31) & ~31; m.min_chunks = (tmin + 31) / 32;
-  m.cals.resize(n_cal);
-  m.a4_off.resize(n_cal);
-  std::vector<float> at((size_t)n_cal * 2 * P * m.t_pad_max, 0.f), apred(total_rows * P);
-  size_t a4_total = 0;
-  for (int c = 0; c < n_cal; ++c) { m.a4_off[c] = a4_total; a4_total += (size_t)4 * ((n_rows[c] + 31) & ~31); }
-  std::vector<float> a4(a4_total * 4, 0.f);
-  size_t row_off = 0;
-  std::vector<float> A;
-  double W[P * P];
-  for (int c = 0; c < n_cal; ++c) {
-    const double* X = X_all + row_off * (size_t)p;
-    if (has_constant)
-      for (int32_t t = 0; t < n_rows[c]; ++t)
-        if (X[(size_t)t * p] != 1.0) return fail(MMF_E_INVALID, "has_constant=1 but calendar %d has X[%d,0] != 1", c, t);
-    CalMeta& cm = m.cals[c];
-    whiten_calendar(X, n_rows[c], p, t_fit[c], W, &cm.kept_mask, A);
-    cm.t_fit = t_fit[c]; cm.n_chunks = (t_fit[c] + 31) / 32; cm.n_rows = n_rows[c];
-    cm.row_off = (int32_t)row_off; cm.pred_start = pred_start[c]; cm.n_pred = n_pred_cal[c]; cm.n_rows_pad = (n_rows[c] + 31) & ~31;
-    memcpy(apred.data() + row_off * P, A.data(), A.size() * sizeof(float));
-    float* atc = at.data() + (size_t)c * 2 * P * m.t_pad_max;
-    for (int32_t t = 0; t < t_fit[c]; ++t)
-      for (int q = 0; q < P; ++q) split_tf32(A[(size_t)t * P + q], atc + (size_t)q * m.t_pad_max + t, atc + (size_t)(P + q) * m.t_pad_max + t);
-    float* a4c = a4.data() + m.a4_off[c] * 4;
-    for (int32_t t = 0; t < n_rows[c]; ++t)
-      for (int q = 0; q < P; ++q) a4c[(((size_t)(q >> 2) * cm.n_rows_pad) + t) * 4 + (q & 3)] = A[(size_t)t * P + q];
-    row_off += (size_t)n_rows[c];
-  }
-  if (row_off > (size_t)INT32_MAX) return fail(MMF_E_UNSUPPORTED, "too many design rows in one ragged plan");
-  CU_TRY(cudaMalloc(&m.d_cals, (size_t)n_cal * sizeof(CalMeta)));
-  CU_TRY(cudaMalloc(&m.d_at, at.size() * sizeof(float)));
-  CU_TRY(cudaMalloc(&m.d_apred, apred.size() * sizeof(float)));
-  CU_TRY(cudaMalloc(&m.d_a4, a4.size() * sizeof(float)));
-  CU_TRY(cudaMalloc(&m.d_w, P * P * sizeof(float)));
-  CU_TRY(cudaMalloc(&m.d_pending_by_cal, (size_t)n_cal * sizeof(uint32_t)));
-  CU_TRY(cudaMalloc(&m.d_tmaps_y, (size_t)n_cal * 128));
-  CU_TRY(cudaMemcpy(m.d_cals, m.cals.data(), (size_t)n_cal * sizeof(CalMeta), cudaMemcpyHostToDevice));
-  CU_TRY(cudaMemcpy(m.d_at, at.data(), at.size() * sizeof(float), cudaMemcpyHostToDevice));
-  CU_TRY(cudaMemcpy(m.d_apred, apred.data(), apred.size() * sizeof(float), cudaMemcpyHostToDevice));
-  CU_TRY(cudaMemcpy(m.d_a4, a4.data(), a4.size() * sizeof(float), cudaMemcpyHostToDevice));
-  CU_TRY(cudaMemset(m.d_w, 0, P * P * sizeof(float)));
-  int rc = encode_2d(m.tmap_at, m.d_at, (uint64_t)m.t_pad_max, (uint64_t)n_cal * 2 * P, (uint64_t)m.t_pad_max * 4, 32, 2 * P);
-  if (rc != MMF_OK) return rc;
-  if (many) {
-    // B operand of predict_tc_kernel: tf32-hi / lo of every calendar's whitened rows, stacked (+128 zero rows: the last
-    // chunk of the last calendar reads a full box)
-    std::vector<float> hi((total_rows + 128) * P, 0.f), lo((total_rows + 128) * P, 0.f);
-    for (size_t i = 0; i < total_rows * P; ++i) split_tf32(apred[i], &hi[i], &lo[i]);
-    CU_TRY(cudaMalloc(&m.d_ap_hi, hi.size() * sizeof(float)));
-    CU_TRY(cudaMalloc(&m.d_ap_lo, lo.size() * sizeof(float)));
-    CU_TRY(cudaMemcpy(m.d_ap_hi, hi.data(), hi.size() * sizeof(float), cudaMemcpyHostToDevice));
-    CU_TRY(cudaMemcpy(m.d_ap_lo, lo.data(), lo.size() * sizeof(float), cudaMemcpyHostToDevice));
-    rc = encode_2d(m.tmap_bhi, m.d_ap_hi, (uint64_t)P, (uint64_t)(total_rows + 128), (uint64_t)P * 4, P, 128, CU_TENSOR_MAP_SWIZZLE_64B);
-    if (rc != MMF_OK) return rc;
-    rc = encode_2d(m.tmap_blo, m.d_ap_lo, (uint64_t)P, (uint64_t)(total_rows + 128), (uint64_t)P * 4, P, 128, CU_TENSOR_MAP_SWIZZLE_64B);
-    if (rc != MMF_OK) return rc;
-    CU_TRY(cudaMalloc(&m.d_tmaps_out, (size_t)n_cal * 128));
-  }
-  m.valid = true;
-  return MMF_OK;
+  return build_multi(ctx->multi, X_all, n_cal, n_rows, t_fit, pred_start, n_pred_cal, p, has_constant, many, n_pred,
+                     n_pred_max, ctx->stream);
 }
 
 int mmf_fit_forecast_ragged_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, const int64_t* cal_row_start,
@@ -1352,6 +1391,240 @@ int mmf_fit_forecast_ragged_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t
     CU_TRY(cudaEventElapsedTime(&stats->kernel_ms, ctx->ev_k0, ctx->ev_k1));
     stats->total_ms = stats->kernel_ms;
     stats->n_series = n; stats->n_pending = pend; stats->kernel_launches = launches; stats->kernel_used = MMF_KERNEL_TC;
+  }
+  return MMF_OK;
+}
+
+// ---- rolling-origin backtest: K origins in one pass (DESIGN.md sections 2 item 8, 4.12) -------------------------
+int mmf_plan_backtest(mmf_ctx* ctx, const double* X, int32_t n_rows, int32_t p, int32_t has_constant, int32_t n_origin,
+                      const int32_t* origin, int32_t horizon) {
+  if (!ctx || !X || !origin) return fail(MMF_E_INVALID, "ctx, X or origin is NULL");
+  if (p < 1 || p > P) return fail(MMF_E_INVALID, "p=%d outside [1,%d]", p, P);
+  if (n_origin < 1 || n_origin > MMF_BT_MAX_ORIGINS)
+    return fail(MMF_E_INVALID, "n_origin=%d outside [1,%d]", n_origin, MMF_BT_MAX_ORIGINS);
+  if (horizon < 1 || horizon > 64) return fail(MMF_E_INVALID, "horizon=%d outside [1,64]", horizon);
+  for (int k = 0; k < n_origin; ++k)
+    if (origin[k] < 33 || (k > 0 && origin[k] <= origin[k - 1]))
+      return fail(MMF_E_INVALID, "origins must be increasing and at least 33 (origin[%d]=%d)", k, origin[k]);
+  const int32_t t_k = origin[n_origin - 1];
+  if (t_k > 65535) return fail(MMF_E_UNSUPPORTED, "the last origin %d exceeds 65535", t_k);
+  if ((int64_t)t_k + horizon > n_rows)
+    return fail(MMF_E_INVALID, "the last origin + horizon = %d exceeds the %d design rows", t_k + horizon, n_rows);
+  for (int64_t i = 0; i < (int64_t)n_rows * p; ++i)
+    if (!std::isfinite(X[i])) return fail(MMF_E_INVALID, "design matrix has a non-finite entry at %lld", (long long)i);
+  if (has_constant)
+    for (int32_t t = 0; t < n_rows; ++t)
+      if (X[(int64_t)t * p] != 1.0) return fail(MMF_E_INVALID, "has_constant=1 but X[%d,0] != 1", t);
+  if (ctx->pinned > 0) return fail(MMF_E_UNSUPPORTED, "a captured CUDA graph pins this context");
+  // origin k as calendar k: the first t_k + horizon rows of X, fit on [0, t_k), evaluated on [t_k, t_k + horizon)
+  std::vector<int32_t> rows(n_origin), tfit(n_origin), pstart(n_origin), npred(n_origin, horizon);
+  std::vector<double> X_all;
+  for (int k = 0; k < n_origin; ++k) {
+    rows[k] = origin[k] + horizon; tfit[k] = origin[k]; pstart[k] = origin[k];
+    X_all.insert(X_all.end(), X, X + (size_t)rows[k] * p);
+  }
+  // the change of basis, float64: x_t = a_t W^-1 on the columns the longest window keeps, so a^(k)_t = a_t T_k with
+  // T_k = W^-1 W_k.  W is upper triangular on its kept columns (W = L^-T): T_k by back substitution.
+  double W[P * P];
+  uint32_t kept = 0;
+  std::vector<float> A;
+  whiten_calendar(X, t_k + horizon, p, t_k, W, &kept, A);
+  std::vector<float> tmat((size_t)n_origin * P * P, 0.f), pred((size_t)n_origin * horizon * P, 0.f);
+  for (int k = 0; k < n_origin; ++k) {
+    float* tk = tmat.data() + (size_t)k * P * P;
+    float* pk = pred.data() + (size_t)k * horizon * P;
+    if (k == n_origin - 1) {                               // the longest window itself: T = I, its own rows exactly
+      for (int j = 0; j < P; ++j) tk[j * P + j] = ((kept >> j) & 1u) ? 1.f : 0.f;
+      memcpy(pk, A.data() + (size_t)t_k * P, (size_t)horizon * P * sizeof(float));
+      continue;
+    }
+    double Wk[P * P];
+    uint32_t kept_k = 0;
+    std::vector<float> Ak;
+    whiten_calendar(X, rows[k], p, tfit[k], Wk, &kept_k, Ak);
+    if ((kept_k & ~kept) != 0u)
+      return fail(MMF_E_UNSUPPORTED, "origin %d keeps a column the longest window drops (kept 0x%x, longest 0x%x)",
+                  origin[k], kept_k, kept);
+    double T[P][P] = {};
+    for (int c = 0; c < P; ++c)
+      for (int r = P - 1; r >= 0; --r) {
+        if (!((kept >> r) & 1u)) continue;
+        double s = Wk[r * P + c];
+        for (int q = r + 1; q < P; ++q) s -= W[r * P + q] * T[q][c];
+        T[r][c] = s / W[r * P + r];
+      }
+    for (int r = 0; r < P; ++r)
+      for (int c = 0; c < P; ++c) tk[r * P + c] = (float)T[r][c];
+    // prediction rows in the common basis: T_k a^(k)_t, a^(k)_t = x_t W_k, all in float64
+    for (int h = 0; h < horizon; ++h) {
+      const double* x = X + (size_t)(origin[k] + h) * p;
+      double ak[P];
+      for (int c = 0; c < P; ++c) {
+        double s = 0.0;
+        for (int i = 0; i < p; ++i) s += x[i] * Wk[i * P + c];
+        ak[c] = s;
+      }
+      for (int r = 0; r < P; ++r) {
+        double s = 0.0;
+        for (int c = 0; c < P; ++c) s += T[r][c] * ak[c];
+        pk[(size_t)h * P + r] = (float)s;
+      }
+    }
+  }
+  CU_TRY(cudaSetDevice(ctx->device));
+  CU_TRY(cudaStreamSynchronize(ctx->stream));
+  free_bt(ctx->bt);
+  BtPlan& b = ctx->bt;
+  int rc = build_plan(b.common, X, t_k + horizon, p, t_k, has_constant);
+  if (rc == MMF_OK)
+    rc = build_multi(b.cals, X_all.data(), n_origin, rows.data(), tfit.data(), pstart.data(), npred.data(), p, has_constant,
+                     false, horizon, horizon, ctx->stream);
+  if (rc != MMF_OK) { free_bt(ctx->bt); return rc; }
+  CU_TRY(cudaMalloc(&b.d_pred, pred.size() * sizeof(float)));
+  CU_TRY(cudaMalloc(&b.d_tmat, tmat.size() * sizeof(float)));
+  CU_TRY(cudaMemcpy(b.d_pred, pred.data(), pred.size() * sizeof(float), cudaMemcpyHostToDevice));
+  CU_TRY(cudaMemcpy(b.d_tmat, tmat.data(), tmat.size() * sizeof(float), cudaMemcpyHostToDevice));
+  b.n_origin = n_origin; b.horizon = horizon;
+  for (int k = 0; k < n_origin; ++k) b.origin[k] = origin[k];
+  b.valid = true;
+  return MMF_OK;
+}
+
+int mmf_backtest_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, float* out_pred, int64_t ld_out,
+                     float* out_metrics, int32_t* out_count, int32_t* out_status, mmf_stats* stats) {
+  if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
+  GrowScope grow_scope(ctx);
+  const BtPlan& b = ctx->bt;
+  if (!b.valid) return fail(MMF_E_NOPLAN, "mmf_plan_backtest has not been called");
+  const int K = b.n_origin, H = b.horizon, t_K = b.origin[K - 1];
+  if (n < 0 || (n > 0 && !y)) return fail(MMF_E_INVALID, "bad y / n");
+  if (!out_pred && !out_metrics) return fail(MMF_E_INVALID, "out_pred and out_metrics are both NULL");
+  if (ld_y < (int64_t)t_K + H)
+    return fail(MMF_E_INVALID, "ld_y=%lld < last origin + horizon = %d (the actual values are read)", (long long)ld_y, t_K + H);
+  if (out_pred && ld_out < H) return fail(MMF_E_INVALID, "ld_out=%lld < horizon=%d", (long long)ld_out, H);
+  if (stats) memset(stats, 0, sizeof(*stats));
+  if (n == 0) return MMF_OK;
+  if (n > (int64_t)0x7fffffff - 128) return fail(MMF_E_UNSUPPORTED, "n too large for 32-bit TMA coordinates");
+  if (ld_y % 4 != 0 || (reinterpret_cast<uintptr_t>(y) & 15u) != 0)
+    return fail(MMF_E_UNSUPPORTED, "backtests need a 16-B aligned y with ld_y %% 4 == 0 (TMA)");
+  CU_TRY(cudaSetDevice(ctx->device));
+  if (!is_device_ptr(y) || (out_pred && !is_device_ptr(out_pred)) || (out_metrics && !is_device_ptr(out_metrics)) ||
+      (out_count && !is_device_ptr(out_count)) || (out_status && !is_device_ptr(out_status)))
+    return fail(MMF_E_UNSUPPORTED, "mmf_backtest_f32 takes device buffers only");
+  cudaStream_t s = ctx->stream;
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  CU_TRY(cudaStreamIsCapturing(s, &cap));
+  if (cap != cudaStreamCaptureStatusNone) return fail(MMF_E_UNSUPPORTED, "backtests cannot be captured into a CUDA graph");
+  // slabs (section 4.10) over the K * n output rows: at most 2^20 of them per slab, whole 128-row tiles, equal slabs
+  int64_t slab = n;
+  if ((int64_t)K * n > ((int64_t)1 << 20)) {
+    slab = std::max<int64_t>(128, (((int64_t)1 << 20) / K) & ~(int64_t)127);
+    const int64_t n_slabs = (n + slab - 1) / slab;
+    slab = (((n + n_slabs - 1) / n_slabs) + 127) & ~(int64_t)127;
+  }
+  const int64_t n_slabs = (n + slab - 1) / slab;
+  const bool may_mask = !ctx->cfg.assume_finite;
+  int32_t* status = out_status;
+  if (!status) {
+    int rc = grow_status_scratch(ctx, (int64_t)K * n, s);
+    if (rc != MMF_OK) return rc;
+    status = ctx->d_status_scratch;
+  }
+  int rc = grow((void**)&ctx->d_bt_ctr, &ctx->bt_ctr_cap, 2 * MMF_BT_MAX_ORIGINS * sizeof(uint32_t));
+  if (rc == MMF_OK && K > 1) rc = grow((void**)&ctx->d_bt_mom, &ctx->bt_mom_cap, (size_t)(K - 1) * 2 * slab * P * sizeof(float));
+  if (rc == MMF_OK && may_mask) rc = grow((void**)&ctx->d_bt_recs, &ctx->bt_recs_cap, (size_t)K * slab * sizeof(SolveRec));
+  if (rc == MMF_OK && may_mask) rc = grow((void**)&ctx->d_bt_rows, &ctx->bt_rows_cap, (size_t)K * slab * sizeof(int64_t));
+  const int64_t ld_scr = (H + 3) & ~3;
+  if (rc == MMF_OK && !out_pred) rc = grow((void**)&ctx->d_bt_pred, &ctx->bt_pred_cap, (size_t)K * slab * ld_scr * sizeof(float));
+  uint32_t* slab_pending = nullptr;
+  if (rc == MMF_OK && stats) {
+    const mmf_ctx* saved = g_grow_ctx;
+    g_grow_ctx = nullptr;
+    rc = grow((void**)&ctx->d_slab_pending, &ctx->slab_pending_cap, (size_t)n_slabs * sizeof(uint32_t));
+    g_grow_ctx = saved;
+    slab_pending = ctx->d_slab_pending;
+  }
+  if (rc != MMF_OK) return rc;
+  const int cs = ctx->counter_set;
+  uint32_t* counters = ctx->d_pending + CTR_WORDS * cs;
+  ctx->set_clean[cs] = false;
+  const DesignView d = view_of(b.common);
+  DesignView dm{};                                         // the origins' stacked designs, as a ragged plan's
+  dm.a4 = b.cals.d_a4; dm.at = b.cals.d_at; dm.apred = b.cals.d_apred; dm.w = b.cals.d_w;
+  dm.n_rows = b.cals.cals[0].n_rows; dm.n_rows_pad = b.cals.cals[0].n_rows_pad;
+  dm.t_fit = b.cals.t_fit_max; dm.t_pad = b.cals.t_pad_max; dm.kept_mask = 0xFFFFu; dm.has_constant = b.cals.has_constant;
+  uint32_t* rec_count = ctx->d_bt_ctr;
+  uint32_t* pend_by_origin = ctx->d_bt_ctr + MMF_BT_MAX_ORIGINS;
+  if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, s));
+  int launches = 0;
+  for (int64_t off = 0, si = 0; off < n; off += slab, ++si) {
+    const int64_t m = std::min(slab, n - off);
+    float* obase = out_pred ? out_pred + off * ld_out : ctx->d_bt_pred;
+    const int64_t ldo = out_pred ? ld_out : ld_scr;
+    const int64_t okstride = out_pred ? n : m;
+    CU_TRY(cudaMemsetAsync(counters, 0, CTR_WORDS * sizeof(uint32_t), s));
+    CU_TRY(cudaMemsetAsync(ctx->d_bt_ctr, 0, 2 * MMF_BT_MAX_ORIGINS * sizeof(uint32_t), s));
+    FitArgs a{};
+    a.y = y + off * ld_y; a.n = m; a.ld_y = ld_y; a.pred_start = t_K; a.n_pred = H;
+    a.out = obase; a.ld_out = ldo; a.status = status + off; a.n_out = 1;
+    if (may_mask) {
+      a.recs = ctx->d_bt_recs + (int64_t)(K - 1) * m;       // the consumers record gap positions in the last origin's block
+      a.rec_rows = ctx->d_bt_rows + (int64_t)(K - 1) * m;
+      a.rec_count = rec_count + (K - 1);
+      a.rec_cap = (uint32_t)m;
+    }
+    BtArgs bt{};
+    bt.cals = b.cals.d_cals; bt.pred = b.d_pred; bt.tmat = b.d_tmat; bt.mom = ctx->d_bt_mom;
+    bt.recs = ctx->d_bt_recs; bt.rec_rows = ctx->d_bt_rows; bt.rec_count = rec_count; bt.pending = pend_by_origin;
+    bt.out_kstride = okstride; bt.st_kstride = n; bt.n_origin = K;
+    for (int k = 0; k < MMF_BT_MAX_ORIGINS - 1; ++k) bt.t_orig[k] = k < K - 1 ? b.origin[k] : INT32_MAX;
+    TcLaunch tl;
+    rc = encode_2d(tl.tmap_y, a.y, (uint64_t)t_K, (uint64_t)m, (uint64_t)ld_y * 4, 32, 128);
+    if (rc != MMF_OK) return rc;
+    memcpy(tl.tmap_at, b.common.tmap_at, 128);
+    CU_TRY(launch_fit_tc_bt(d, a, tl, counters, ctx->sm_count, s, bt));
+    ++launches;
+    if (may_mask) {
+      // per origin: the general pass for the rows the fast path left to it (exits at once when there are none), then
+      // the solve of the queued records, calendar = origin
+      for (int k = 0; k < K; ++k) {
+        const CalMeta& cm = b.cals.cals[k];
+        DesignView dk = dm;
+        dk.a4 = b.cals.d_a4 + b.cals.a4_off[k]; dk.apred = b.cals.d_apred + (size_t)cm.row_off * P;
+        dk.n_rows = cm.n_rows; dk.n_rows_pad = cm.n_rows_pad; dk.t_fit = cm.t_fit; dk.t_pad = (cm.t_fit + 31) & ~31;
+        dk.kept_mask = cm.kept_mask;
+        FitArgs ak = a;
+        ak.out = obase + (int64_t)k * okstride * ldo; ak.status = status + (int64_t)k * n + off;
+        ak.pred_start = cm.pred_start; ak.recs = ctx->d_bt_recs + (int64_t)k * m; ak.rec_rows = ctx->d_bt_rows + (int64_t)k * m;
+        ak.rec_count = rec_count + k; ak.row_base = 0; ak.cal_id = k;
+        ak.only_pending = 1; ak.pending_count = pend_by_origin + k;
+        CU_TRY(launch_fit_warp(dk, ak, ctx->sm_count, s));
+        ak.pending_count = nullptr;
+        CU_TRY(launch_solve_rows(dm, ak, ctx->sm_count, s, b.cals.d_cals));
+        launches += 2;
+      }
+    }
+    ScoreArgs sa{};
+    sa.pred = obase; sa.ld_pred = ldo; sa.pred_kstride = okstride; sa.y = a.y; sa.ld_y = ld_y; sa.cals = b.cals.d_cals;
+    sa.metrics = out_metrics ? out_metrics + off * MMF_BT_NMETRIC : nullptr; sa.count = out_count ? out_count + off : nullptr;
+    sa.out_kstride = n; sa.n = m; sa.n_origin = K; sa.horizon = H;
+    if (sa.metrics || sa.count) {
+      CU_TRY(launch_bt_score(sa, ctx->sm_count, s));
+      ++launches;
+    }
+    if (slab_pending != nullptr)
+      CU_TRY(cudaMemcpyAsync(slab_pending + si, counters, sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+  }
+  ctx->last_set = cs;
+  if (stats) {
+    CU_TRY(cudaEventRecord(ctx->ev_k1, s));
+    CU_TRY(cudaEventSynchronize(ctx->ev_k1));
+    CU_TRY(cudaEventElapsedTime(&stats->kernel_ms, ctx->ev_k0, ctx->ev_k1));
+    stats->total_ms = stats->kernel_ms;
+    std::vector<uint32_t> pend((size_t)n_slabs);
+    CU_TRY(cudaMemcpy(pend.data(), slab_pending, pend.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    for (uint32_t v : pend) stats->n_pending += v;
+    stats->n_series = n; stats->kernel_launches = launches; stats->kernel_used = MMF_KERNEL_TC;
   }
   return MMF_OK;
 }

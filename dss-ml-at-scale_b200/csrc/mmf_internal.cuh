@@ -119,6 +119,24 @@ struct SeArgs {
   const float* sfac;        // [n_rows] sqrt(1 + |a_t|^2) of the planned design (gap-free rows: G_i = I)
 };
 
+// Backtest calls (mmf_backtest_f32, DESIGN.md section 2 item 8): one pass of fit_tc_kernel over [0, t_K) captures the
+// moments at every origin t_0 < ... < t_{K-1} = t_K in the basis of the longest window.  Origin k is calendar k of the
+// backtest plan's stacked designs (its own whitening, t_fit = t_k, prediction rows [t_k, t_k + n_pred)).
+struct BtArgs {
+  const CalMeta* cals;      // [K] the origins as calendars of the stacked plan
+  const float* pred;        // [K][n_pred][P] origin k's prediction rows in the common basis, T_k a^(k)_t (float64 -> fp32)
+  const float* tmat;        // [K][P][P] T_k = W^-1 W_k, row-major: b^(k) = T_k^T b_k
+  float* mom;               // [K-1][2 consumer groups][n][P] partial moments at the earlier origins
+  SolveRec* recs;           // [K][n] records by origin, then row (FitArgs::recs is block K-1)
+  int64_t* rec_rows;        // [K][n] work lists
+  uint32_t* rec_count;      // [K]
+  uint32_t* pending;        // [K] rows of each origin left to the general pass
+  int64_t out_kstride;      // rows between the origin blocks of FitArgs::out
+  int64_t st_kstride;       // ... and of FitArgs::status
+  int32_t n_origin;
+  int32_t t_orig[MMF_BT_MAX_ORIGINS - 1];   // t_k of the earlier origins; INT32_MAX from n_origin - 1 on
+};
+
 // warp-per-series CUDA-core kernel (general path)
 cudaError_t launch_fit_warp(const DesignView& d, const FitArgs& a, int sm_count, cudaStream_t s,
                             const SeArgs* se = nullptr);
@@ -174,7 +192,26 @@ cudaError_t launch_fit_tc(const DesignView& d, const FitArgs& a, const TcLaunch&
 // the product configuration <8, 1> with the standard-error outputs (SE instantiation)
 cudaError_t launch_fit_tc_se(const DesignView& d, const FitArgs& a, const TcLaunch& tl, uint32_t* pending_count,
                              int sm_count, cudaStream_t s, const SeArgs& se);
+// the product configuration <8, 1> capturing the moments at every backtest origin (BT instantiation)
+cudaError_t launch_fit_tc_bt(const DesignView& d, const FitArgs& a, const TcLaunch& tl, uint32_t* pending_count,
+                             int sm_count, cudaStream_t s, const BtArgs& bt);
 bool fit_tc_supported(const DesignView& d, const FitArgs& a, const char** why);
+
+// Forecast errors of a backtest (backtest.cu): one warp per (series, origin) scores pred[k][i][0, H) against
+// y[i][t_k, t_k + H) and writes {MSE, MAE, bias, MAPE} and the number of scored points.
+struct ScoreArgs {
+  const float* pred;        // origin k, row i: pred + (k * pred_kstride + i) * ld_pred
+  int64_t ld_pred, pred_kstride;
+  const float* y;           // row i: y + i * ld_y
+  int64_t ld_y;
+  const CalMeta* cals;      // t_fit of calendar k = origin t_k
+  float* metrics;           // nullable: (k * out_kstride + i) * MMF_BT_NMETRIC
+  int32_t* count;           // nullable: k * out_kstride + i
+  int64_t out_kstride;
+  int64_t n;                // rows
+  int32_t n_origin, horizon;
+};
+cudaError_t launch_bt_score(const ScoreArgs& sa, int sm_count, cudaStream_t s);
 
 // per-series model selection by hold-out MSE over nested whitened designs (select.cu)
 constexpr int MMF_MAX_CAND = 8;

@@ -319,6 +319,61 @@ class ForecastEngine:
                                  st.kernel_launches, "tc")
         return res
 
+    # ---- rolling-origin backtest: K origins, one pass over the data -----------------------------------------------
+    def plan_backtest(self, start, t_len: int, freq: str = "D", horizon: int = 28, n_origins: int = 3,
+                      step: int | None = None, design: str = "trend_season_exog"):
+        """Plan a backtest of series that start at ``start`` and have ``t_len`` grid rows: origin ``k`` of ``n_origins``
+        fits rows ``[0, t_k)`` and forecasts ``[t_k, t_k + horizon)``, ``t_k = t_len - horizon - (n_origins-1-k) * step``
+        (``step`` defaults to ``horizon``), so the last origin is the reference's train / score split (02:372-380).
+        Every origin's model is the plain model planned with ``t_fit = t_k`` on the design of the whole window
+        (``mmf_plan_backtest``).  Returns the origins (int32 array); the first forecast date of origin k is
+        ``calendar_grid(start, t_len)[t_k]``."""
+        step = int(horizon if step is None else step)
+        n_origins, horizon, t_len = int(n_origins), int(horizon), int(t_len)
+        if step < 1:
+            raise ValueError("step must be >= 1")
+        origins = np.array([t_len - horizon - (n_origins - 1 - k) * step for k in range(n_origins)], dtype=np.int32)
+        days = D.calendar_grid(start, t_len, freq)
+        X = np.ascontiguousarray(D.design_matrix(days, t_len - horizon, design), dtype=np.float64)
+        N.check(self._lib.mmf_plan_backtest(self._h, X.ctypes.data, X.shape[0], X.shape[1],
+                                            1 if D.design_has_constant(design) else 0, len(origins),
+                                            origins.ctypes.data, horizon))
+        self._backtest = (origins, horizon, t_len)
+        return origins
+
+    def backtest(self, y, want_pred: bool = True, want_stats: bool = False):
+        """Run the planned backtest on ``y`` [n, >= t_len] (float32 CUDA tensor, NaN = missing).  Returns
+        ``{"pred": [K, n, horizon] or None, "metrics": [K, n, 4] (MSE, MAE, bias, MAPE), "count": [K, n],
+        "status": [K, n]}`` as CUDA tensors; forecasts are scored on the device (``mmf_backtest_f32``).  The kernel reads
+        ``y`` with TMA: a tensor whose row pitch is not a multiple of 4 floats or that is not 16-B aligned is first copied
+        into a pitched buffer (``device_packed``)."""
+        import torch
+        if getattr(self, "_backtest", None) is None:
+            raise RuntimeError("plan_backtest() must be called first")
+        origins, h, t_len = self._backtest
+        yp, n, t_have, ld_y = _describe(y, "y")
+        if not (_is_torch(y) and y.is_cuda and y.dtype == torch.float32) or t_have < t_len:
+            raise ValueError(f"y must be a float32 CUDA tensor with at least {t_len} columns")
+        if ld_y % 4 or yp % 16:
+            y = device_packed(y, device=y.device)
+            yp, n, t_have, ld_y = _describe(y, "y")
+        self.set_stream(torch.cuda.current_stream(y.device).cuda_stream)
+        k = len(origins)
+        pred = torch.empty((k, n, (h + 3) & ~3), device=y.device, dtype=torch.float32)[:, :, :h] if want_pred else None
+        metrics = torch.empty((k, n, N.BT_NMETRIC), device=y.device, dtype=torch.float32)
+        count = torch.empty((k, n), device=y.device, dtype=torch.int32)
+        status = torch.empty((k, n), device=y.device, dtype=torch.int32)
+        st = N.MmfStats() if want_stats else None
+        N.check(self._lib.mmf_backtest_f32(self._h, yp, n, ld_y, pred.data_ptr() if pred is not None else None,
+                                           pred.stride(1) if pred is not None else 0, metrics.data_ptr(),
+                                           count.data_ptr(), status.data_ptr(), C.byref(st) if st is not None else None))
+        res = {"pred": pred, "metrics": metrics, "count": count, "status": status}
+        if st is not None:
+            self.launches += st.kernel_launches
+            res["stats"] = Stats(st.kernel_ms, st.total_ms, st.n_series, st.n_pending, st.h2d_bytes, st.d2h_bytes,
+                                 st.kernel_launches, "tc")
+        return res
+
     def whitening(self):
         W = np.zeros((N.MMF_P, N.MMF_P), dtype=np.float64)
         kept = np.zeros(N.MMF_P, dtype=np.int32)

@@ -41,6 +41,18 @@ def tuning_schema(keys=DEFAULT_KEYS, date_col="Date", value_col="Demand", interv
                      + extra)
 
 
+BACKTEST_METRICS = ("MSE", "MAE", "Bias", "MAPE")
+
+
+def backtest_schema(keys=DEFAULT_KEYS):
+    """The rows of ``backtest_groups``: keys..., ``Cutoff`` (the first forecast date of the origin), ``N`` (scored
+    points) and the four metrics."""
+    import pyarrow as pa
+
+    return pa.schema([(k, pa.string()) for k in keys] + [("Cutoff", pa.date32()), ("N", pa.int32())]
+                     + [(m, pa.float32()) for m in BACKTEST_METRICS])
+
+
 def enriched_schema(keys=DEFAULT_KEYS, date_col="Date", value_col="Demand"):
     import pyarrow as pa
 
@@ -538,6 +550,62 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
         return parts[0]
     out = pd.concat(parts, ignore_index=True)
     return out.take(_global_order(buckets, keys, lengths)).reset_index(drop=True)
+
+
+def backtest_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Demand", freq="W-MON",
+                    horizon=FORECAST_HORIZON, n_origins=3, step=None, design="trend_season_exog",
+                    pack: str = "host", engine: ForecastEngine | None = None) -> pd.DataFrame:
+    """Rolling-origin backtest of every group in ``pdf`` (pandas, or Arrow with ``pack="device"`` / an Arrow table):
+    each group is cut at ``n_origins`` origins placed relative to its OWN last date, ``t_k = t_len - horizon -
+    (n_origins-1-k) * step`` grid rows (``step`` defaults to ``horizon``), so the last origin is the reference's train /
+    score split (02:372-380).  Origin k fits the group's rows before t_k and its ``horizon`` forecasts are scored
+    against the actual values (``ForecastEngine.backtest``: one pass over the data and one call per calendar bucket).
+
+    Returns ``backtest_schema(keys)`` rows in (key, Cutoff) order: keys..., ``Cutoff`` (first forecast date of the
+    origin), ``N`` (scored points: forecast and actual value both present), ``MSE``, ``MAE``, ``Bias`` (mean of
+    forecast - actual) and ``MAPE`` (over the scored points with a non-zero actual value), float32, NaN where nothing is
+    averaged.  A (group, origin) with fewer than 33 fit rows is left out (the engine's minimum fit window), so a short
+    group contributes fewer origins or no row at all."""
+    eng = engine or default_engine()
+    keys = list(keys)
+    K, horizon = int(n_origins), int(horizon)
+    step = horizon if step is None else int(step)
+    if K < 1 or step < 1:
+        raise ValueError("need n_origins >= 1 and step >= 1")
+    buckets = _buckets_for(pdf, keys, date_col, value_col, freq, pack, eng)
+    parts, used, lengths = [], [], []
+    for b in buckets:
+        first = b.t_len - horizon - (K - 1) * step
+        k0 = 0 if first >= 33 else -(-(33 - first) // step)      # origins below 33 fit rows are left out
+        if k0 >= K:
+            continue
+        origins = np.asarray(eng.plan_backtest(b.start, b.t_len, freq, horizon, K - k0, step, design))
+        yd = b.y
+        if pack != "device" and isinstance(eng, ForecastEngine):
+            from .engine import device_packed
+            yd = device_packed(b.y)
+        res = eng.backtest(yd, want_pred=False)
+        met = np.asarray(_host(res["metrics"]), dtype=np.float32)          # [k, n, 4]
+        cnt = np.asarray(_host(res["count"]), dtype=np.int32)              # [k, n]
+        k, n = cnt.shape
+        row_of = np.repeat(np.arange(n), k)
+        cut = D.calendar_grid(b.start, b.t_len, freq)[origins].astype("datetime64[ns]")
+        frame = {c: pd.Series(b.key_frame[c].array.take(row_of), dtype=b.key_frame[c].dtype, copy=False) for c in keys}
+        frame["Cutoff"] = np.tile(cut, n)
+        frame["N"] = np.ascontiguousarray(cnt.T).reshape(-1)
+        mt = np.ascontiguousarray(met.transpose(1, 0, 2)).reshape(-1, len(BACKTEST_METRICS))
+        for j, m in enumerate(BACKTEST_METRICS):
+            frame[m] = mt[:, j]
+        parts.append(pd.DataFrame(frame))
+        used.append(b)
+        lengths.append(k)
+    if not parts:
+        return pd.DataFrame({**{c: pd.Series(dtype=object) for c in keys}, "Cutoff": pd.Series(dtype="datetime64[ns]"),
+                             "N": pd.Series(dtype=np.int32), **{m: pd.Series(dtype=np.float32) for m in BACKTEST_METRICS}})
+    if len(parts) == 1:
+        return parts[0]
+    out = pd.concat(parts, ignore_index=True)
+    return out.take(_global_order(used, keys, lengths)).reset_index(drop=True)
 
 
 def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Demand",

@@ -31,11 +31,13 @@
 extern "C" {
 #endif
 
-#define MMF_VERSION 103          /* 0.1.3 */
+#define MMF_VERSION 104          /* 0.1.4 */
 #define MMF_P 16                 /* design columns (zero-pad narrower designs) */
 #define MMF_PIVOT_TOL 1e-3f      /* per-series relative Cholesky pivot threshold */
 #define MMF_CAL_TOL 1e-10        /* aliasing threshold on the float64 calendar Gram */
 #define MMF_SELECT_MAX_HOLD 3500 /* held-out rows mmf_fit_select_forecast_f32 accepts (64 B of shared memory each) */
+#define MMF_BT_MAX_ORIGINS 8     /* backtest origins per call (mmf_plan_backtest) */
+#define MMF_BT_NMETRIC 4         /* backtest metrics per (origin, series): MSE, MAE, bias, MAPE */
 
 /* return codes */
 #define MMF_OK 0
@@ -197,6 +199,31 @@ int mmf_plan_calendars(mmf_ctx* ctx, const double* X_all, int32_t n_cal, const i
                        const int32_t* pred_start, const int32_t* n_pred, int32_t p, int32_t has_constant);
 int mmf_fit_forecast_ragged_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, const int64_t* cal_row_start,
                                 float* out_pred, int64_t ld_out, int32_t* out_status, mmf_stats* stats);
+
+/* ---- rolling-origin backtest: K forecast origins in one pass over the data -------------------------------------
+ * Origin k (0 <= k < n_origin <= MMF_BT_MAX_ORIGINS, 33 <= origin[0] < ... < origin[n_origin-1]) is exactly the plain
+ * model of mmf_plan_design(X, t_fit = origin[k]) evaluated on design rows [origin[k], origin[k] + horizon): the same
+ * whitening, kept columns, centring constant, pivot rule and status codes (DESIGN.md section 2 item 8).
+ * mmf_plan_backtest: X [n_rows, p] float64 as for mmf_plan_design, 1 <= horizon <= 64,
+ * origin[n_origin-1] + horizon <= n_rows, origin[n_origin-1] <= 65535.  A plan of its own: the mmf_plan_design and
+ * mmf_plan_calendars plans stay in force.
+ * mmf_backtest_f32: y [n, ld_y] device, ld_y >= origin[n_origin-1] + horizon (the actual values are read), 16-B
+ * aligned with ld_y % 4 == 0.  Outputs, each nullable (but not out_pred and out_metrics both), device:
+ *   out_pred    [n_origin][n][ld_out]  forecasts of origin k for series i (ld_out >= horizon)
+ *   out_metrics [n_origin][n][MMF_BT_NMETRIC]  MSE, MAE, bias = mean(forecast - actual), MAPE = mean |e| / |y| over
+ *               the points with y != 0; only points where the forecast and y are both finite are scored, in float64;
+ *               NaN where nothing is averaged
+ *   out_count   [n_origin][n]  scored points
+ *   out_status  [n_origin][n]  MMF_STATUS_* of origin k's fit
+ * Enqueued on the ctx stream; the call synchronises only when `stats` is non-NULL.  Refused arguments write nothing.
+ * replaces: the reference's single train / score split (split_train_score_data, 02:372-380) and its hold-out MSE
+ * (02:453-459), at several origins. */
+int mmf_plan_backtest(mmf_ctx* ctx, const double* X, int32_t n_rows, int32_t p, int32_t has_constant,
+                      int32_t n_origin, const int32_t* origin, int32_t horizon);
+int mmf_backtest_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y,
+                     float* out_pred, int64_t ld_out,
+                     float* out_metrics, int32_t* out_count,
+                     int32_t* out_status, mmf_stats* stats);
 
 /* ---- multi-GPU: fit + write the forecast rows into every GPU's copy of the table ----------
  * Same fit as above (device buffers only, enqueue-only), but each forecast row is stored to

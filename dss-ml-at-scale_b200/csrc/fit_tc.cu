@@ -131,38 +131,24 @@ __device__ __forceinline__ float lds32(uint32_t addr) {
 
 // MULTI: a ragged launch -- every 128-row tile names its calendar (mv.tiles / mv.cals); `n_chunks` is then only the
 // minimum over the calendars (>= 2).  MULTI == false compiles to the single-calendar kernel.
-// BAL (tc_variant = 3, an experiment): a balanced launch -- instead of dealing 128-row tiles round robin, every CTA owns
-// one contiguous range of mv.bal_rows rows (a multiple of 8) and walks it in 128-row tiles; the range's last tile is
-// short and is loaded as 8-row boxes, so no SM streams rows it does not own.
-// Rows are independent in the GEMM, so the forecasts are bit-identical to the round-robin launch's.
 // SE (standard-error calls, single calendar): the consumers also sum S = sum (y - c)^2 of their fragment rows and the
 // epilogue writes sigma / dof (and the se row in future mode) of the gap-free rows; the MMA inputs are unchanged.
 // BT (backtest calls, single calendar, d = the longest window t_K): a consumer group writes its running moments to
 // bt.mom at every earlier origin t_k -- a chunk that contains t_k is issued twice, first with its values at t >= t_k
 // zeroed, then with the complementary ones -- and the epilogue finishes every origin of a row (DESIGN.md section 4.12).
-template <int STAGES, int OBUF, bool MULTI, bool BAL, bool SE = false, bool BT = false>
+template <int STAGES, int OBUF, bool MULTI, bool SE = false, bool BT = false>
 __global__ void __launch_bounds__(THREADS, 1)
 fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const FitArgs a,
-              uint32_t* __restrict__ pending_count, const int n_tiles_all, const int n_chunks, const MultiView mv,
+              uint32_t* __restrict__ pending_count, const int n_tiles, const int n_chunks, const MultiView mv,
               const SeArgs se, const BtArgs bt) {
-  static_assert(!(MULTI && BAL), "ragged launches carry their own tile table");
-  static_assert(!SE || !(MULTI || BAL), "standard errors are built for the single-calendar round-robin launch");
-  static_assert(!BT || !(MULTI || BAL || SE), "backtests are built for the single-calendar round-robin launch");
+  static_assert(!SE || !MULTI, "standard errors are built for the single-calendar launch");
+  static_assert(!BT || !(MULTI || SE), "backtests are built for the single-calendar launch");
   using SmemLayout = SmemLayoutT<STAGES, OBUF, SE>;
-  // BAL: this CTA's rows; its k-th tile keeps the round-robin loop index blockIdx.x + k * gridDim.x
-  const int64_t cta_row0 = BAL ? (int64_t)blockIdx.x * mv.bal_rows : 0;
-  const int cta_rows = BAL ? (int)(a.n - cta_row0 < mv.bal_rows ? a.n - cta_row0 : mv.bal_rows) : 0;
-  const int n_tiles = BAL ? (int)blockIdx.x + ((cta_rows + TILE_M - 1) / TILE_M) * (int)gridDim.x : n_tiles_all;
   auto tile_rec = [&](int ti) -> TileRec {
     if (MULTI) {
       if (ti >= n_tiles) return TileRec{0, 0, 0, 1};
       const int4 v = __ldg(reinterpret_cast<const int4*>(mv.tiles) + ti);
       return TileRec{v.x, v.y, v.z, v.w};
-    }
-    if (BAL) {
-      const int k = ti / (int)gridDim.x;
-      const int left = cta_rows - k * TILE_M;
-      return TileRec{(int)cta_row0 + k * TILE_M, left >= TILE_M ? TILE_M : (left > 0 ? left : 0), 0, n_chunks};
     }
     const int64_t left = a.n - (int64_t)ti * TILE_M;
     return TileRec{ti * TILE_M, (int)(left >= TILE_M ? TILE_M : (left > 0 ? left : 0)), 0, n_chunks};
@@ -216,7 +202,6 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
       fence_mbar_init();
       prefetch_tensormap(tl.tmap_y);
       prefetch_tensormap(tl.tmap_at);
-      if (BAL) prefetch_tensormap(tl.tmap_y8);
     }
   } else if (warp >= WARP_EPI0) {
     // prediction rows of the whitened design -> shared (broadcast-read in the epilogue); ragged launches reload
@@ -229,8 +214,7 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
   }
   __syncthreads();
   // This CTA is resident: a dependent kernel launched behind this one with programmatic stream serialisation may start
-  // once EVERY CTA has said so -- the streaming solve then finds all producers running (it never has to wait for a
-  // producer that cannot get an SM), the early-exit fix-up kernels hide their launch latency under this kernel's tail.
+  // once EVERY CTA has said so -- the early-exit fix-up kernels hide their launch latency under this kernel's tail.
   if (threadIdx.x == 0) pdl_launch_dependents();
 
   if (warp == WARP_PROD) {
@@ -247,23 +231,6 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
       const void* tmy = MULTI ? static_cast<const void*>(mv.tmaps_y + (size_t)tr.cal * 128) : static_cast<const void*>(tl.tmap_y);
       if (MULTI && tr.cal != last_cal) { fence_tensormap_acquire(tmy); last_cal = tr.cal; }
       const int at_row = MULTI ? tr.cal * 2 * P : 0;
-      if (BAL && tr.nrows < TILE_M) {
-        // short tile: the design box as usual, the series rows as 8-row boxes (same swizzled layout: a box is one
-        // 1,024-B swizzle atom of the stage); rows beyond the tile keep whatever the stage held -- their accumulator
-        // rows hold garbage that nobody reads.  A box that crosses the end of the buffer is zero-filled and still
-        // counts in full.
-        const int nb = (tr.nrows + 7) >> 3;
-        for (int ch = 0; ch < tr.n_chunks; ++ch) {
-          mbar_wait(bar_empty(stage), phase ^ 1u);
-          mbar_expect_tx_elect(bar_full(stage), static_cast<uint32_t>(nb) * 1024u + AT_STAGE_BYTES);
-          tma_issue_2d_elect(bar_full(stage), s_at + stage * AT_STAGE_BYTES, tl.tmap_at, ch * KC, 0, L2_EVICT_LAST);
-          for (int j = 0; j < nb; ++j)
-            tma_issue_2d_elect(bar_full(stage), s_y + stage * Y_STAGE_BYTES + j * 1024, tl.tmap_y8, ch * KC,
-                               tr.row0 + 8 * j, L2_EVICT_FIRST);
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        continue;
-      }
       for (int ch = 0; ch < tr.n_chunks; ++ch) {
         mbar_wait(bar_empty(stage), phase ^ 1u);
         tma_load_2d_x2_elect(bar_full(stage), Y_STAGE_BYTES + AT_STAGE_BYTES,
@@ -308,7 +275,7 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
       for (int h = 0; h < 2; ++h)
 #pragma unroll
         for (int i = 0; i < P; ++i) acc[h][i] = 0.f;
-      const bool scan = collect && (!(MULTI || BAL) || r < tr.nrows);   // short tiles: rows beyond belong to ANOTHER tile
+      const bool scan = collect && (!MULTI || r < tr.nrows);   // short tiles: rows beyond belong to ANOTHER tile
       // segment = parity of the chunk inside the TILE (all of a group's chunks of one tile share it), not the group:
       // with an odd chunk count the groups swap roles from tile to tile, and the order in which the solve applies
       // the gaps -- hence the forecast's last bits -- must not depend on where in a launch the series sits
@@ -760,16 +727,7 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
           rec.nm[1] = static_cast<uint16_t>(nm1);
           rec.cal = tr.cal;
           const unsigned slot = base + __popc(dm & ((1u << lane) - 1u));
-          if (slot < a.rec_cap) {
-            if (a.stream_ctl != nullptr) {
-              // publish: the record (this thread's moments, the consumer warps' positions acquired through bar_accfull) is
-              // ordered before the work-list entry the consumer polls
-              __threadfence();
-              st_release_s64(a.rec_rows + slot, row);
-            } else {
-              a.rec_rows[slot] = row;
-            }
-          }
+          if (slot < a.rec_cap) a.rec_rows[slot] = row;
         }
       }
       if (bulk) {
@@ -860,14 +818,6 @@ fit_tc_kernel(const __grid_constant__ TcLaunch tl, const DesignView d, const Fit
       }
     }
     if (bulk && warp == WARP_EPI0) bulk_wait_all_elect();   // global writes complete before the kernel retires
-    if (a.stream_ctl != nullptr) {
-      // the last CTA to finish tells the streaming solve that the work list is final
-      named_bar_sync(3, 128);
-      if (threadIdx.x == WARP_EPI0 * 32) {
-        __threadfence();
-        if (atomicAdd(a.stream_ctl + 1, 1u) == gridDim.x - 1u) st_release_u32(a.stream_ctl + 2, 1u);
-      }
-    }
   }
 }
 
@@ -885,25 +835,16 @@ bool fit_tc_supported(const DesignView& d, const FitArgs& a, const char** why) {
   return w == nullptr;
 }
 
-template <int STAGES, int OBUF, bool MULTI, bool BAL = false, bool SE = false, bool BT = false>
+template <int STAGES, int OBUF, bool MULTI, bool SE = false, bool BT = false>
 static cudaError_t launch_variant(const DesignView& d, const FitArgs& a, const TcLaunch& tl, uint32_t* pending_count,
                                   int sm_count, cudaStream_t s, int n_tiles, int n_chunks, const MultiView& mv,
                                   const SeArgs& se = SeArgs{}, const BtArgs& bt = BtArgs{}) {
   const size_t smem = SmemLayoutT<STAGES, OBUF, SE>::total + 1024;
-  cudaError_t e = cudaFuncSetAttribute(fit_tc_kernel<STAGES, OBUF, MULTI, BAL, SE, BT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaError_t e = cudaFuncSetAttribute(fit_tc_kernel<STAGES, OBUF, MULTI, SE, BT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  const int grid = BAL ? (int)((a.n + mv.bal_rows - 1) / mv.bal_rows) : (n_tiles < sm_count ? n_tiles : sm_count);
-  fit_tc_kernel<STAGES, OBUF, MULTI, BAL, SE, BT><<<grid, THREADS, smem, s>>>(tl, d, a, pending_count, n_tiles, n_chunks, mv, se, bt);
+  const int grid = n_tiles < sm_count ? n_tiles : sm_count;
+  fit_tc_kernel<STAGES, OBUF, MULTI, SE, BT><<<grid, THREADS, smem, s>>>(tl, d, a, pending_count, n_tiles, n_chunks, mv, se, bt);
   return cudaGetLastError();
-}
-
-// Rows per CTA of a balanced launch (0: deal 128-row tiles round robin), built only for tc_variant = 3, an
-// experiment: with more than one tile per CTA the short tile costs almost a whole tile's pipeline time on EVERY SM, where
-// the round-robin deal leaves the extra tile to a few; a batch of less than one wave spreads over every SM.
-int fit_tc_balanced_rows(int64_t n, int sm_count, int variant) {
-  if (variant != 3) return 0;
-  const int64_t per = (n + sm_count - 1) / sm_count;
-  return (int)((per + 7) / 8 * 8);
 }
 
 cudaError_t launch_fit_tc(const DesignView& d, const FitArgs& a, const TcLaunch& tl, uint32_t* pending_count,
@@ -914,33 +855,25 @@ cudaError_t launch_fit_tc(const DesignView& d, const FitArgs& a, const TcLaunch&
   const int n_tiles = (int)((a.n + TILE_M - 1) / TILE_M);
   const int n_chunks = d.t_pad / KC;
   const MultiView none{};
-  // variant 0 / 1: eight stages, one staging tile.  Variant 2, <6 stages, 2 staging tiles> (tile k+1 staged while the
-  // peer stores of tile k still read theirs; the second tile costs two stages of the 227 KB), is built for experiments.
-  const bool two = variant == 2;
-  const int bal = fit_tc_balanced_rows(a.n, sm_count, variant);
-  if (bal > 0) {
-    MultiView b{};
-    b.bal_rows = bal;
-    return launch_variant<8, 1, false, true>(d, a, tl, pending_count, sm_count, s, n_tiles, n_chunks, b);
-  }
-  return two ? launch_variant<6, 2, false>(d, a, tl, pending_count, sm_count, s, n_tiles, n_chunks, none)
-             : launch_variant<8, 1, false>(d, a, tl, pending_count, sm_count, s, n_tiles, n_chunks, none);
+  // variant 2: <6 stages, 2 staging tiles> (tile k+1 staged while the peer stores of tile k still read theirs; the
+  // second tile costs two stages of the 227 KB); any other value: eight stages, one staging tile
+  return variant == 2 ? launch_variant<6, 2, false>(d, a, tl, pending_count, sm_count, s, n_tiles, n_chunks, none)
+                      : launch_variant<8, 1, false>(d, a, tl, pending_count, sm_count, s, n_tiles, n_chunks, none);
 }
 
 cudaError_t launch_fit_tc_se(const DesignView& d, const FitArgs& a, const TcLaunch& tl, uint32_t* pending_count,
                              int sm_count, cudaStream_t s, const SeArgs& se) {
   if (a.n <= 0) return cudaSuccess;
   const int n_tiles = (int)((a.n + TILE_M - 1) / TILE_M);
-  return launch_variant<8, 1, false, false, true>(d, a, tl, pending_count, sm_count, s, n_tiles, d.t_pad / KC,
-                                                  MultiView{}, se);
+  return launch_variant<8, 1, false, true>(d, a, tl, pending_count, sm_count, s, n_tiles, d.t_pad / KC, MultiView{}, se);
 }
 
 cudaError_t launch_fit_tc_bt(const DesignView& d, const FitArgs& a, const TcLaunch& tl, uint32_t* pending_count,
                              int sm_count, cudaStream_t s, const BtArgs& bt) {
   if (a.n <= 0) return cudaSuccess;
   const int n_tiles = (int)((a.n + TILE_M - 1) / TILE_M);
-  return launch_variant<8, 1, false, false, false, true>(d, a, tl, pending_count, sm_count, s, n_tiles, d.t_pad / KC,
-                                                         MultiView{}, SeArgs{}, bt);
+  return launch_variant<8, 1, false, false, true>(d, a, tl, pending_count, sm_count, s, n_tiles, d.t_pad / KC,
+                                                  MultiView{}, SeArgs{}, bt);
 }
 
 }  // namespace mmf

@@ -173,8 +173,8 @@ struct mmf_ctx {
   cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
   cudaEvent_t ev_a = nullptr, ev_b = nullptr, ev_k0 = nullptr, ev_k1 = nullptr;
   uint32_t* d_pending = nullptr;       // 3 counter sets of CTR_WORDS words {rows left PENDING, solve records queued,
-                                       // claimed, CTAs finished, producer done, ...}: 0/1 ping-pong between
-                                       // eager calls, 2 belongs to captured CUDA graphs (zeroed by a node of the graph)
+                                       // ...}: 0/1 ping-pong between eager calls, 2 belongs to captured CUDA graphs
+                                       // (zeroed by a node of the graph)
   int counter_set = 0;                 // set the next eager call uses
   bool set_clean[2] = {true, true};    // the set is known to be zero (cudaMemset at create, or zeroed by the previous
                                        // eager call's tensor-core kernel); anything else makes the call memset its set
@@ -187,7 +187,6 @@ struct mmf_ctx {
   size_t recs_cap_bytes = 0;
   int64_t* d_rec_rows = nullptr;
   size_t rec_rows_cap_bytes = 0;
-  bool rec_rows_clean = false;         // every entry is -1 (what the streaming solve needs to find; its kernels restore it)
   float* d_gamma = nullptr;            // [n][P] + d_c[n]: hand-off from the fit kernels to predict_tc_kernel
   size_t gamma_cap_bytes = 0;
   float* d_c = nullptr;
@@ -514,10 +513,8 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
     // work list of rows whose record is ready for solve_rows_kernel
     const int64_t cap = n;
     int rc = grow((void**)&ctx->d_recs, &ctx->recs_cap_bytes, (size_t)cap * sizeof(SolveRec));
-    const int64_t* rows_before = ctx->d_rec_rows;
     if (rc == MMF_OK) rc = grow((void**)&ctx->d_rec_rows, &ctx->rec_rows_cap_bytes, (size_t)cap * sizeof(int64_t));
     if (rc != MMF_OK) return rc;
-    if (ctx->d_rec_rows != rows_before) ctx->rec_rows_clean = false;
     a.recs = ctx->d_recs;
     a.rec_rows = ctx->d_rec_rows;
     a.rec_cap = (uint32_t)cap;
@@ -536,26 +533,9 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
   if (capturing || !ctx->set_clean[cs]) CU_TRY(cudaMemsetAsync(counters, 0, CTR_WORDS * sizeof(uint32_t), s));
   if (!capturing) ctx->set_clean[cs] = false;             // dirty from here on, whatever happens below
   if (kernel == MMF_KERNEL_TC && !capturing) a.zero_next = ctx->d_pending + CTR_WORDS * (cs ^ 1);
-  // Streaming solve (opt-in, mmf_config.stream_solve = 1): the series with gaps are solved WHILE the tensor-core kernel is
-  // still streaming (solve_stream_kernel launched right behind it with programmatic stream serialisation) instead of in
-  // a pass of their own afterwards.  The work list starts out as -1; the producer publishes row indices into it.  It
-  // only overlaps when a consumer block fits beside the fit CTA on an SM, which the fit kernel's register and shared
-  // memory use (one CTA per SM) does not leave room for, so it is off by default.
-  // (standard-error calls always take the product configuration and the post-pass solve)
-  const bool stream_solve = kernel == MMF_KERNEL_TC && may_mask && !capturing && n >= 32768 && ctx->cfg.stream_solve == 1 &&
-                            se == nullptr;
-  if (stream_solve) {
-    if (!ctx->rec_rows_clean) CU_TRY(cudaMemsetAsync(ctx->d_rec_rows, 0xFF, ctx->rec_rows_cap_bytes, s));
-    ctx->rec_rows_clean = true;                            // the call's closing solve_rows pass resets what it consumed
-    a.stream_ctl = counters + 2;
-  } else if (may_mask) {
-    ctx->rec_rows_clean = false;
-  }
   if (kernel == MMF_KERNEL_TC) {
     TcLaunch tl;
     int rc = encode_2d(tl.tmap_y, y, (uint64_t)d.t_fit, (uint64_t)n, (uint64_t)ld_y * 4, 32, 128);
-    if (rc == MMF_OK && fit_tc_balanced_rows(n, ctx->sm_count, ctx->cfg.tc_variant) > 0)
-      rc = encode_2d(tl.tmap_y8, y, (uint64_t)d.t_fit, (uint64_t)n, (uint64_t)ld_y * 4, 32, 8);
     if (rc != MMF_OK) return rc;
     memcpy(tl.tmap_at, ctx->plan.tmap_at, 128);
     if (se != nullptr) {
@@ -573,13 +553,9 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
       FitArgs m = a;
       m.only_pending = 1;
       m.pending_count = counters;
-      if (stream_solve) {
-        CU_TRY(launch_solve_stream(d, m, ctx->sm_count, s));
-        ++*launches;
-      }
       CU_TRY(launch_fit_warp(d, m, ctx->sm_count, s, se));
-      CU_TRY(launch_solve_rows(d, m, ctx->sm_count, s, nullptr, se));   // records the general pass queued (and, without the
-      *launches += 2;                                        // streaming solve, all of them)
+      CU_TRY(launch_solve_rows(d, m, ctx->sm_count, s, nullptr, se));   // the records both passes queued
+      *launches += 2;
     }
   } else {
     CU_TRY(launch_fit_warp(d, a, ctx->sm_count, s, se));
@@ -1323,7 +1299,6 @@ int mmf_fit_forecast_ragged_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t
     if (rc == MMF_OK) rc = grow((void**)&ctx->d_rec_rows, &ctx->rec_rows_cap_bytes, (size_t)n * sizeof(int64_t));
     if (rc != MMF_OK) return rc;
     a.recs = ctx->d_recs; a.rec_rows = ctx->d_rec_rows; a.rec_cap = (uint32_t)n;
-    ctx->rec_rows_clean = false;                           // ragged launches use the work list without the streaming solve
   }
   const int cs = ctx->counter_set;
   uint32_t* counters = ctx->d_pending + CTR_WORDS * cs;

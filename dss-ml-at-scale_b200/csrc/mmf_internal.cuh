@@ -57,7 +57,6 @@ struct MultiView {                         // all null / 0 for an ordinary singl
   uint32_t* pending_by_cal;                // [n_cal]: rows per calendar the fast path left to the general pass
   int32_t n_cal;
   int32_t n_tiles;
-  int32_t bal_rows;                        // balanced single-calendar launch: rows per CTA (multiple of 8), else 0
 };
 
 // One series with gaps, handed to the thread-per-series solve kernel (256 B, indexed by row).
@@ -102,9 +101,8 @@ struct FitArgs {
   uint32_t rec_cap;         //   == n
   int32_t only_pending;     // 1: process only rows whose status == MMF_STATUS_PENDING
   const uint32_t* pending_count;  // nullable; if non-null and *pending_count == 0 the kernel exits at once
-  uint32_t* zero_next;      // nullable: 2 counters of the NEXT call's set, zeroed by the tensor-core kernel (no memset node)
-  uint32_t* stream_ctl;     // nullable: {claimed, CTAs finished, producer done} of the streaming solve (solve_stream_kernel
-                            // consumes the queued records WHILE the tensor-core kernel is still producing them)
+  uint32_t* zero_next;      // nullable: the NEXT call's counter set (CTR_WORDS words), zeroed by the tensor-core kernel
+                            // (no memset node)
   int64_t row_base;         // ragged fallback launches cover one calendar's rows: absolute row of this launch's row 0
   int32_t cal_id;           //   ... and that calendar's index (written into the records the launch queues)
 };
@@ -149,11 +147,7 @@ cudaError_t launch_solve_rows(const DesignView& d, const FitArgs& a, int sm_coun
 // se rows of the gap-free rows of a fit + predict_tc call: out_se[i, k] = sigma_i * sfac[pred_start + k] for every row
 // whose status is MMF_STATUS_OK right after fit_tc_kernel (launched before the passes that finish the other rows)
 cudaError_t launch_se_outer(const FitArgs& a, const SeArgs& se, int sm_count, cudaStream_t s);
-// the same solve as a CONSUMER that runs beside fit_tc_kernel (launched right behind it with programmatic stream
-// serialisation; fit_tc_kernel releases it once all its CTAs are resident): records are solved as the epilogue
-// publishes them, the kernel retires when the producer has finished and the work list is drained
-cudaError_t launch_solve_stream(const DesignView& d, const FitArgs& a, int sm_count, cudaStream_t s);
-constexpr int CTR_WORDS = 8;             // one counter set: {pending, records queued, claimed, CTAs finished, producer done, -, -, -}
+constexpr int CTR_WORDS = 8;             // one counter set: {rows left pending, solve records queued, 6 unused words}
 
 // fitted values + forecasts for MANY prediction rows (the reference's "Demand_Fitted for every date"
 // contract, 02:484-494): out[n, n_pred] = c + gamma A_pred^T as a wgmma GEMM with TMA-stored tiles
@@ -181,11 +175,9 @@ cudaError_t launch_predict_tc(const DesignView& d, const FitArgs& a, const Predi
 struct TcLaunch {
   alignas(64) unsigned char tmap_y[128];    // box {32 t, 128 series}
   alignas(64) unsigned char tmap_at[128];
-  alignas(64) unsigned char tmap_y8[128];   // box {32 t, 8 series}: the short last tile of a balanced launch's CTA
 };
-// variant: 0 / 1 = <8 smem stages, 1 forecast staging tile>, tiles dealt round robin (the product), 2 = <6 stages,
-// 2 staging tiles>, 3 = balanced row ranges per CTA (both experiments that did not pay, kept for the record)
-int fit_tc_balanced_rows(int64_t n, int sm_count, int variant);
+// variant: 2 = <6 smem stages, 2 forecast staging tiles>, anything else = <8 stages, 1 staging tile> (the product);
+// 128-row tiles dealt round robin over the SMs either way
 cudaError_t launch_fit_tc(const DesignView& d, const FitArgs& a, const TcLaunch& tl,
                           uint32_t* pending_count, int sm_count, cudaStream_t s, int variant = 0,
                           const MultiView* multi = nullptr);

@@ -53,23 +53,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
-// ---- gpu-scope acquire / release (producer-consumer hand-off between kernels running side by side) ----------
-__device__ __forceinline__ void st_release_u32(uint32_t* p, uint32_t v) {
-  asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
-  uint32_t v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void st_release_s64(int64_t* p, int64_t v) {
-  asm volatile("st.release.gpu.global.s64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ int64_t ld_acquire_s64(const int64_t* p) {
-  int64_t v;
-  asm volatile("ld.acquire.gpu.global.s64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-  return v;
-}
+// ---- programmatic dependent launch ----------------------------------------------------------------------------
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
 // ---- TMA -------------------------------------------------------------------

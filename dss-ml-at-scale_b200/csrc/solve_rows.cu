@@ -123,8 +123,7 @@ __device__ __forceinline__ bool vec_out_ok(const FitArgs& a) {
   return v;
 }
 
-// The pass over the whole work list, after the producers have finished.  A record whose series is no longer
-// MMF_STATUS_DEFERRED was already solved by the streaming consumer below.
+// The pass over the whole work list, after the producers have finished.
 template <bool MULTI, bool SE = false>
 __global__ void __launch_bounds__(THREADS, 2)
 solve_rows_kernel(const DesignView d0, const FitArgs a, const CalMeta* __restrict__ cals, const SeArgs se) {
@@ -141,65 +140,7 @@ solve_rows_kernel(const DesignView d0, const FitArgs a, const CalMeta* __restric
       row_next = a.rec_rows[i + stride];
       prefetch_rec(a.recs + row_next);
     }
-    if (a.stream_ctl != nullptr) {
-      a.rec_rows[i] = -1;                               // the work list of a streaming call is left as it was found: all -1
-      if (a.status[row] != MMF_STATUS_DEFERRED) continue;
-    }
     solve_one<MULTI, SE>(d0, a, cals, row, vec_out, se);
-  }
-}
-
-// The same solve as a CONSUMER running beside fit_tc_kernel.  A warp claims 32 consecutive work-list slots and every
-// lane waits for its slot to be published (the producer stores the row index last, with release semantics; the list
-// starts out as -1).  When the producer's last CTA has raised `done`, the count of queued records is final: a lane
-// whose slot lies beyond it -- and with it every later slot -- has nothing left to do.
-__device__ __forceinline__ uint64_t timer_ns() {
-  uint64_t t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
-__device__ __forceinline__ int64_t ld_acquire_s64(const int64_t* p) {
-  int64_t v;
-  asm volatile("ld.acquire.gpu.global.s64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
-  uint32_t v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-
-__global__ void __launch_bounds__(THREADS, 2)
-solve_stream_kernel(const DesignView d0, const FitArgs a) {
-  const int lane = threadIdx.x & 31;
-  const bool vec_out = vec_out_ok(a);
-  for (;;) {
-    uint32_t base = 0;
-    if (lane == 0) base = atomicAdd(a.stream_ctl, 32u);
-    base = __shfl_sync(0xffffffffu, base, 0);
-    const uint32_t idx = base + lane;
-    int64_t row = -1;
-    bool exhausted = idx >= a.rec_cap;
-    if (!exhausted) {
-      uint64_t t0 = 0;
-      for (unsigned spins = 0;; ++spins) {
-        row = ld_acquire_s64(a.rec_rows + idx);
-        if (row >= 0) break;
-        if (ld_acquire_u32(a.stream_ctl + 2) != 0u) {            // every producer CTA has finished
-          if (idx >= *reinterpret_cast<volatile uint32_t*>(a.rec_count)) { exhausted = true; break; }
-          row = ld_acquire_s64(a.rec_rows + idx);                 // queued before `done`: visible now
-          if (row >= 0) break;
-        }
-        __nanosleep(spins < 64 ? 100 : 1000);
-        if ((spins & 1023u) == 1023u) {                           // a protocol bug traps instead of hanging the GPU
-          if (t0 == 0) t0 = timer_ns();
-          else if (timer_ns() - t0 > 4000000000ull) __trap();
-        }
-      }
-    }
-    if (row >= 0) solve_one<false>(d0, a, nullptr, row, vec_out);
-    // (the slot is reset to -1 by the closing solve_rows pass, which walks the whole list once more)
-    if (__any_sync(0xffffffffu, exhausted)) break;                // slots are claimed in order: nothing lies beyond
   }
 }
 
@@ -225,25 +166,6 @@ cudaError_t launch_solve_rows(const DesignView& d, const FitArgs& a, int sm_coun
   if (se != nullptr) return cudaLaunchKernelEx(&cfg, solve_rows_kernel<false, true>, d, a, cals, *se);
   return cals != nullptr ? cudaLaunchKernelEx(&cfg, solve_rows_kernel<true>, d, a, cals, none)
                          : cudaLaunchKernelEx(&cfg, solve_rows_kernel<false>, d, a, cals, none);
-}
-
-cudaError_t launch_solve_stream(const DesignView& d, const FitArgs& a, int sm_count, cudaStream_t s) {
-  if (a.recs == nullptr || a.rec_cap == 0 || a.stream_ctl == nullptr) return cudaSuccess;
-  // two blocks per SM in the grid: one fits beside a resident fit_tc CTA, the second takes the SM over when that CTA
-  // retires and helps drain what is left
-  const int64_t want = ((int64_t)a.rec_cap + THREADS - 1) / THREADS;
-  const int64_t cap = (int64_t)sm_count * 2;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(want < cap ? want : cap));
-  cfg.blockDim = dim3(THREADS);
-  cfg.dynamicSmemBytes = 0;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;      // starts when every fit_tc CTA is resident
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, solve_stream_kernel, d, a);
 }
 
 }  // namespace mmf

@@ -163,7 +163,9 @@ class Stats:
 
 
 class ForecastEngine:
-    """One library context: streams, staging buffers, the planned calendar design."""
+    """One library context: streams, staging buffers, the planned calendar design.
+
+    ``stream_solve`` is accepted for compatibility and has no effect."""
 
     def __init__(self, device: int | None = None, kernel: str = "auto", assume_finite: bool = False,
                  chunk_series: int = 0, stream: int | None = None, tc_variant: int = 0,
@@ -180,8 +182,8 @@ class ForecastEngine:
         # cross PCIe ("auto" / "on" / "off"); exact or not used -- the forecasts are bit-equal either way
         cfg.host_narrow = {"auto": 0, "on": 1, "off": 2}[host_narrow]
         cfg.host_threads = int(host_threads)
-        # series with gaps: True = solve them beside the streaming kernel (solve_stream_kernel; experimental), False = in
-        # a pass of their own after it
+        # no effect: the library accepts and ignores the field (series with gaps are always solved in a pass of their
+        # own after the tensor-core kernel)
         cfg.stream_solve = 1 if stream_solve else 0
         h = C.c_void_p()
         N.check(self._lib.mmf_create(C.byref(cfg), C.byref(h)))

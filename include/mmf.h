@@ -70,17 +70,16 @@ typedef struct mmf_config {
   int32_t device;          /* CUDA device ordinal, -1 = current device */
   int32_t kernel;          /* MMF_KERNEL_* */
   int32_t assume_finite;   /* 1: caller guarantees y has no NaN/Inf, skip the masked fix-up pass */
-  int32_t tc_variant;      /* tuning of the tensor-core kernel, same results whichever: 0 / 1 = the product (128-row tiles dealt
-                              round robin over the SMs), 2 = the experimental <6-stage, 2 staging tiles> instantiation,
-                              3 = the experimental balanced launch (one row range per SM) */
+  int32_t tc_variant;      /* tuning of the tensor-core kernel, same results whichever: 2 = the <6-stage, 2 staging tiles>
+                              instantiation, any other value = the product (<8 stages, 1 staging tile>) */
   int64_t chunk_series;    /* host-buffer path: series per pipelined chunk (0 = library default) */
   void*   stream;          /* cudaStream_t to enqueue on (NULL = library-owned stream) */
   int32_t host_narrow;     /* host-buffer path: 0 = automatic, 1 = always try, 2 = never: narrow float32 chunks to
                               uint16 on host threads when every value is an integer in [0, 65534] (exactly, or the
                               chunk goes as float32), so that half the bytes cross PCIe; widened back on the device */
   int32_t host_threads;    /* threads of that narrowing pool (0 = half of the process's cores, at most 16) */
-  int32_t stream_solve;    /* series with gaps: 0 = solved in a pass of their own after the tensor-core kernel (default), 1 = by a
-                              consumer kernel launched BESIDE it (experimental: pays only with a register-capped build) */
+  int32_t stream_solve;    /* accepted and ignored: series with gaps are always solved in a pass of their own after
+                              the tensor-core kernel */
   int32_t reserved1;
 } mmf_config;
 
@@ -168,8 +167,8 @@ int mmf_fit_forecast_int(mmf_ctx* ctx, const void* y, int32_t dtype, int64_t n, 
  * out_pred and out_status are bit-equal to mmf_fit_forecast_f32 on the same inputs.  out_se [n, ld_se] (ld_se >=
  * n_pred; only columns [0, n_pred) of a row are written), out_sigma [n], out_dof [n] are each nullable, but not all
  * three.  Device buffers only (host pointers: MMF_E_UNSUPPORTED); enqueue-only unless `stats` is non-NULL.  The
- * call always runs the product tensor-core configuration and solves series with gaps in a pass of their own after
- * it, whatever mmf_config.tc_variant and stream_solve say; mmf_config.kernel is honoured.
+ * call always runs the product tensor-core configuration, whatever mmf_config.tc_variant says; mmf_config.kernel is
+ * honoured.
  * replaces: the forecast variance / conf_int() the reference's per-group SARIMAX model offers beside the mean. */
 int mmf_fit_forecast_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y,
                             int32_t pred_start, int32_t n_pred,

@@ -483,33 +483,31 @@ def test_host_narrowing_is_exact_or_not_used():
     dev.close()
 
 
-def test_streaming_solve_matches_the_separate_pass():
-    """mmf_config.stream_solve = 1: the queued records of series with gaps are consumed by solve_stream_kernel while
-    the tensor-core kernel is still producing them (release/acquire work list, PDL launch).  Same records, same arithmetic:
-    bit-equal forecasts and statuses to the default (a solve pass after the streaming kernel), also on a second call
-    (the work list must be left clean) and when the default path runs in between."""
+def test_retired_tuning_options_have_no_effect():
+    """mmf_config.tc_variant = 3 (a balanced launch) and stream_solve = 1 (a solve of the series with gaps beside the
+    tensor-core kernel) are accepted and ignored: forecasts, statuses and coefficients are bit-equal to the default and
+    the call launches the same kernels -- on a batch large enough, and with enough gaps, for either to have applied."""
     import torch
     n, t, h = 70_000, 400, 28
     y, start = mmf.synth.daily_store_item_demand(n, t, seed=91, nan_frac=0.01)
     y[5, :9] = np.nan                                         # general pass (fit_warp) queues a record of its own
     y[6, :] = np.nan
     yd = mmf.device_packed(y)
-    a = mmf.ForecastEngine()
-    b = mmf.ForecastEngine(stream_solve=True)
-    for eng in (a, b):
+    base = mmf.ForecastEngine(kernel="tc")
+    base.plan_calendar(start, t, "D", h, "future")
+    want = base.fit_forecast(yd, t, h, want_status=True, want_beta=True, want_stats=True)
+    torch.cuda.synchronize()
+    assert want["stats"].n_pending > 0 and int((want["status"] == 0).sum()) < n
+    for variant, stream_solve in ((3, False), (0, True), (3, True)):
+        eng = mmf.ForecastEngine(kernel="tc", tc_variant=variant, stream_solve=stream_solve)
         eng.plan_calendar(start, t, "D", h, "future")
-    want = a.fit_forecast(yd, t, h, want_status=True)
-    for rep in range(3):
-        got = b.fit_forecast(yd, t, h, want_status=True)
+        got = eng.fit_forecast(yd, t, h, want_status=True, want_beta=True, want_stats=True)
         torch.cuda.synchronize()
-        assert torch.equal(got["status"], want["status"]), rep
-        assert np.array_equal(got["pred"].cpu().numpy(), want["pred"].cpu().numpy(), equal_nan=True), rep
-        if rep == 1:                                          # a small batch takes the default path on the same context
-            small = b.fit_forecast(yd[:1000], t, h)
-            torch.cuda.synchronize()
-            assert np.array_equal(small.cpu().numpy(), want["pred"][:1000].cpu().numpy(), equal_nan=True)
-    a.close()
-    b.close()
+        for k in ("pred", "status", "beta"):
+            assert torch.equal(got[k].view(torch.int32), want[k].view(torch.int32)), (variant, stream_solve, k)
+        assert got["stats"].kernel_launches == want["stats"].kernel_launches, (variant, stream_solve)
+        eng.close()
+    base.close()
 
 
 def test_ragged_holdout_matches_oracle_and_per_bucket_calls():
@@ -581,13 +579,12 @@ def test_forecast_groups_many_calendars_holdout_mode_one_ragged_launch():
     _le(err.max(), 40 * tolerance(df["Demand"].to_numpy()), "ragged holdout DataFrame batch vs per-group oracle UDF")
 
 
-# ---- balanced launches of small batches (fit_tc_kernel<.., BAL>) ---------------------------------------------
+# ---- batches of less than one wave of 128-row tiles on the tensor-core kernel ---------------------------------------
 @pytest.mark.parametrize("n", [1, 7, 8, 9, 127, 129, 1000, 10_000, 20_011])
 @pytest.mark.parametrize("mode", ["future", "holdout"])
-def test_balanced_launch_is_bit_equal_to_round_robin_tiles(n, mode):
-    """Small batches give every SM one contiguous row range (short last tile loaded as 8-row boxes) instead of
-    dealing 128-row tiles round robin.  Rows are independent in the GEMM: forecasts, coefficients and statuses must
-    be BIT-identical, with gaps, leading gaps and mostly-missing rows in the batch, and equal to the oracle's."""
+def test_small_tc_batches_match_the_oracle(n, mode):
+    """Batches of 1 to 20,011 rows (one short tile, a tile and a row, under and about one wave of tiles) with gaps,
+    leading gaps and mostly-missing rows: statuses equal to the oracle's, forecasts within the tolerance."""
     import torch
     t, h = 365, 28
     yd, start = mmf.synth.daily_store_item_demand_torch(n, t, seed=77 + n, nan_frac=0.02)
@@ -595,21 +592,16 @@ def test_balanced_launch_is_bit_equal_to_round_robin_tiles(n, mode):
     if n > 3:
         yd[3, 10:] = float("nan")                # (almost) empty row
     y = yd.cpu().numpy()
-    got = {}
-    for variant in (1, 3):
-        eng = mmf.ForecastEngine(kernel="tc", tc_variant=variant)
-        res = mmf.forecast_packed(yd, start, "D", h, mode, engine=eng, want_status=True, want_beta=True)
-        torch.cuda.synchronize()
-        got[variant] = (res["pred"].cpu().numpy(), res["status"].cpu().numpy(), res["beta"].cpu().numpy())
-        eng.close()
-    assert np.array_equal(got[1][1], got[3][1])
-    assert np.array_equal(got[1][0], got[3][0], equal_nan=True)
-    assert np.array_equal(got[1][2], got[3][2], equal_nan=True)
+    eng = mmf.ForecastEngine(kernel="tc")
+    res = mmf.forecast_packed(yd, start, "D", h, mode, engine=eng, want_status=True)
+    torch.cuda.synchronize()
+    pred, status = res["pred"].cpu().numpy(), res["status"].cpu().numpy()
+    eng.close()
     want, wst = O.fit_forecast_packed_c(y, *_design(start, t, h, mode))
-    assert np.array_equal(got[3][1], wst)
+    assert np.array_equal(status, wst)
     ok = (wst == 0) & (np.arange(n) % 5 != 0) & (np.arange(n) != 3)      # ~7 scattered gaps: well conditioned
     if ok.any():
-        _le(np.abs(got[3][0][ok] - want[ok]).max(), 4 * tolerance(y[ok]), (n, mode))
+        _le(np.abs(pred[ok] - want[ok]).max(), 4 * tolerance(y[ok]), (n, mode))
 
 
 def test_gappy_rows_do_not_depend_on_their_position_in_the_launch():
@@ -623,7 +615,7 @@ def test_gappy_rows_do_not_depend_on_their_position_in_the_launch():
     t, h = 400, 28
     n = sm * 128 + 3000
     yd, start = mmf.synth.daily_store_item_demand_torch(n, t, seed=5, nan_frac=0.02)
-    eng = mmf.ForecastEngine(kernel="tc", tc_variant=1)
+    eng = mmf.ForecastEngine(kernel="tc")
     eng.plan_calendar(start, t, "D", h, "future")
     whole = eng.fit_forecast(yd, t, h, want_status=True)
     part = eng.fit_forecast(yd[sm * 128:], t, h, want_status=True)

@@ -2,8 +2,8 @@
 float64 oracle, or against a property that must hold exactly.
 
 A. Batches of more than 2^20 rows, which run_device (csrc/mmf_api.cu) fits slab by slab.  Every row is compared with
-   the oracle.  Forecasts, holdout tables, coefficients, statuses, model selection, broadcast stores, CUDA-graph
-   replays and the streaming solve must be bit-equal to the same rows fitted as separate calls of at most 2^20 rows.
+   the oracle.  Forecasts, holdout tables, coefficients, statuses, model selection, broadcast stores and CUDA-graph
+   replays must be bit-equal to the same rows fitted as separate calls of at most 2^20 rows.
    stats.n_pending must count the rows of every slab.
 B. Model selection (csrc/select.cu) against a vectorised float64 selection oracle, row by row: the choice is optimal
    up to fp32 noise on every row.  Also the edges: one candidate, eight, rejected lists, n_hold = 1 and 3,500, exact
@@ -378,23 +378,6 @@ def test_slabbed_capture_replays_equal_eager_calls(big):
         assert _same_bits(status, want["status"]), rep
     graph.close()
     eng.close()
-
-
-def test_slabbed_stream_solve_is_bit_equal_to_the_default(big):
-    """ForecastEngine(stream_solve=True) on the several-slab batch, two calls in a row: bit-equal to the default"""
-    import torch
-    yd, start = big["yd"], big["start"]
-    a, b = mmf.ForecastEngine(), mmf.ForecastEngine(stream_solve=True)
-    for eng in (a, b):
-        eng.plan_calendar(start, T_BIG, "D", 28, "future")
-    want = a.fit_forecast(yd, T_BIG, 28, want_status=True, want_beta=True)
-    for rep in range(2):
-        got = b.fit_forecast(yd, T_BIG, 28, want_status=True, want_beta=True)
-        torch.cuda.synchronize()
-        for k in ("pred", "status", "beta"):
-            assert _same_bits(got[k], want[k]), (rep, k)
-    a.close()
-    b.close()
 
 
 # =====================================================================================================================

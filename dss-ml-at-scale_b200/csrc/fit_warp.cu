@@ -100,7 +100,8 @@ __device__ __forceinline__ double warp_sum_d(double v) {
 template <bool SE>
 __device__ __noinline__ int solve_masked(const DesignView& d, const ARows& A, const float* __restrict__ yr,
                                          int nmiss, const unsigned short* __restrict__ miss_list,
-                                         WarpScratch& scr, float (&g)[P], int lane, float& zz, unsigned& omask) {
+                                         WarpScratch& scr, float (&g)[P], int lane, float& zz, unsigned& omask,
+                                         bool gram_direct) {
   const int t_fit = d.t_fit;
   int pi[DPL], pj[DPL];
 #pragma unroll
@@ -113,8 +114,10 @@ __device__ __noinline__ int solve_masked(const DesignView& d, const ARows& A, co
   }
   // Mostly-missing rows: G_i = I - D would cancel catastrophically in fp32, so accumulate the Gram
   // directly over the (few) observed rows instead of downdating over the (many) missing ones.
-  const bool direct = 2 * nmiss > t_fit;
+  bool direct = 2 * nmiss > t_fit;
   float dacc[DPL];
+#pragma unroll 1
+  for (int pass = 0; pass < 2; ++pass) {
 #pragma unroll
   for (int k = 0; k < DPL; ++k) dacc[k] = 0.f;
   if (!direct && nmiss <= MISS_CAP && t_fit <= 65535) {
@@ -165,6 +168,17 @@ __device__ __noinline__ int solve_masked(const DesignView& d, const ARows& A, co
 #pragma unroll
       for (int k = 0; k < DPL; ++k) dacc[k] = dsum[k] + dacc[k];
     }
+  }
+  if (!gram_direct || direct) break;
+  // the general pass after the tensor-core kernel (gram_direct): its rows start with a gap, and when the missing rows
+  // carry more than 40 % of the design's leverage (trace D > 0.4 x kept columns) I - D cancels to pivots near
+  // MMF_PIVOT_TOL even with fewer than half of the values missing -- sum the Gram over the observed rows instead
+  float tr = 0.f;
+#pragma unroll
+  for (int k = 0; k < DPL; ++k)
+    if (lane + 32 * k < NPAIR && pi[k] == pj[k] && ((d.kept_mask >> pi[k]) & 1u)) tr += dacc[k];
+  if (warp_sum(tr) <= 0.4f * static_cast<float>(__popc(d.kept_mask & 0xFFFFu))) break;
+  direct = true;
   }
   __syncwarp();
 #pragma unroll
@@ -417,7 +431,8 @@ fit_warp_kernel(const DesignView d, const FitArgs a, const int smem_rows, const 
       for (int q = 0; q < S; ++q)
         if (q == s) { need = act[q] && any[q] && miss[q] > 0; nm = miss[q]; }
       if (!need) continue;                          // warp-uniform
-      if (a.recs != nullptr && nm <= SOLVE_MISS_CAP && nm <= MISS_CAP && 2 * nm <= t_fit && t_fit <= 65535) {
+      // (not in the general pass after the tensor-core kernel: its rows are solved here, on a Gram over the observed rows)
+      if (a.recs != nullptr && !a.only_pending && nm <= SOLVE_MISS_CAP && nm <= MISS_CAP && 2 * nm <= t_fit && t_fit <= 65535) {
         // common case: hand the series to the thread-per-series solve kernel (moments + missing positions)
         SolveRec& rec = a.recs[row0 + s];
         float bl = 0.f, cs = 0.f;
@@ -460,7 +475,8 @@ fit_warp_kernel(const DesignView d, const FitArgs a, const int smem_rows, const 
       }
       float zz = 0.f;
       unsigned outmask = 0u;
-      const int rs = solve_masked<SE>(d, A, yr0 + s * a.ld_y, nm, scr.miss_t[s], scr, g, lane, zz, outmask);
+      const int rs = solve_masked<SE>(d, A, yr0 + s * a.ld_y, nm, scr.miss_t[s], scr, g, lane, zz, outmask,
+                                      a.only_pending != 0);
 #pragma unroll
       for (int q = 0; q < S; ++q) {
         if (q == s) {

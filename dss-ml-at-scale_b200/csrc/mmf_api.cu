@@ -407,8 +407,15 @@ int build_multi(MultiPlan& m, const double* X_all, int32_t n_cal, const int32_t*
     tmax = std::max(tmax, t_fit[c]);
     tmin = std::min(tmin, t_fit[c]);
   }
+  if (total_rows > (size_t)INT32_MAX) return fail(MMF_E_UNSUPPORTED, "too many design rows in one ragged plan");
   for (size_t i = 0; i < total_rows * (size_t)p; ++i)
     if (!std::isfinite(X_all[i])) return fail(MMF_E_INVALID, "design matrix has a non-finite entry at %zu", i);
+  if (has_constant) {                                      // every argument check comes before the previous plan is freed
+    size_t off = 0;
+    for (int c = 0; c < n_cal; off += (size_t)n_rows[c], ++c)
+      for (int32_t t = 0; t < n_rows[c]; ++t)
+        if (X_all[(off + t) * (size_t)p] != 1.0) return fail(MMF_E_INVALID, "has_constant=1 but calendar %d has X[%d,0] != 1", c, t);
+  }
   CU_TRY(cudaStreamSynchronize(sync));
   free_multi(m);
   m.n_cal = n_cal; m.n_pred = many ? 1 : n_pred; m.has_constant = has_constant ? 1 : 0;
@@ -425,9 +432,6 @@ int build_multi(MultiPlan& m, const double* X_all, int32_t n_cal, const int32_t*
   double W[P * P];
   for (int c = 0; c < n_cal; ++c) {
     const double* X = X_all + row_off * (size_t)p;
-    if (has_constant)
-      for (int32_t t = 0; t < n_rows[c]; ++t)
-        if (X[(size_t)t * p] != 1.0) return fail(MMF_E_INVALID, "has_constant=1 but calendar %d has X[%d,0] != 1", c, t);
     CalMeta& cm = m.cals[c];
     whiten_calendar(X, n_rows[c], p, t_fit[c], W, &cm.kept_mask, A);
     cm.t_fit = t_fit[c]; cm.n_chunks = (t_fit[c] + 31) / 32; cm.n_rows = n_rows[c];
@@ -441,7 +445,6 @@ int build_multi(MultiPlan& m, const double* X_all, int32_t n_cal, const int32_t*
       for (int q = 0; q < P; ++q) a4c[(((size_t)(q >> 2) * cm.n_rows_pad) + t) * 4 + (q & 3)] = A[(size_t)t * P + q];
     row_off += (size_t)n_rows[c];
   }
-  if (row_off > (size_t)INT32_MAX) return fail(MMF_E_UNSUPPORTED, "too many design rows in one ragged plan");
   CU_TRY(cudaMalloc(&m.d_cals, (size_t)n_cal * sizeof(CalMeta)));
   CU_TRY(cudaMalloc(&m.d_at, at.size() * sizeof(float)));
   CU_TRY(cudaMalloc(&m.d_apred, apred.size() * sizeof(float)));

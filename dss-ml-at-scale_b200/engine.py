@@ -260,7 +260,7 @@ class ForecastEngine:
             raise ValueError("starts and t_lens must have the same non-zero length")
         if mode not in ("future", "holdout"):
             raise ValueError(f"mode must be 'holdout' or 'future', got {mode!r}")
-        blocks, dates, n_rows, t_fit, p_start, n_pred = [], [], [], [], [], []
+        blocks, dates, t_fit, p_start, n_pred = [], [], [], [], []
         for st, tl in zip(starts, t_lens):
             if mode == "future":
                 days = D.calendar_grid(st, tl + horizon, freq)
@@ -272,15 +272,32 @@ class ForecastEngine:
                 tf, ps, npd = tl - horizon, 0, tl
             blocks.append(D.design_matrix(days, tf, design))
             dates.append(np.asarray(days[ps:ps + npd], dtype="datetime64[D]"))
-            n_rows.append(len(days)); t_fit.append(tf); p_start.append(ps); n_pred.append(npd)
-        X = np.ascontiguousarray(np.concatenate(blocks, axis=0), dtype=np.float64)
-        arr = [np.array(v, dtype=np.int32) for v in (n_rows, t_fit, p_start, n_pred)]
-        N.check(self._lib.mmf_plan_calendars(self._h, X.ctypes.data, len(starts), arr[0].ctypes.data, arr[1].ctypes.data,
-                                             arr[2].ctypes.data, arr[3].ctypes.data, X.shape[1],
-                                             1 if D.design_has_constant(design) else 0))
-        # (n_cal, columns of the output table, columns y must have)
-        self._ragged = (len(starts), int(max(n_pred)), int(max(t_fit)), mode)
+            t_fit.append(tf); p_start.append(ps); n_pred.append(npd)
+        self.plan_designs(blocks, t_fit, p_start, n_pred, D.design_has_constant(design))
+        self._ragged = self._ragged[:3] + (mode,)        # holdout tables are NaN-filled even when one window fits all
         return np.stack(dates) if mode == "future" else dates
+
+    def plan_designs(self, Xs, t_fit, pred_start, n_pred, has_constant: bool) -> None:
+        """Plan a ragged batch on caller designs (``mmf_plan_calendars``): calendar ``c`` has the raw design ``Xs[c]``
+        ``[n_rows_c, p]`` (float64, one ``p <= 16`` for all), fits rows ``[0, t_fit[c])`` and evaluates rows
+        ``[pred_start[c], pred_start[c] + n_pred[c])``.  One common ``n_pred <= 64`` is written by the fit kernel's
+        epilogue; anything else by the predict kernel, and ``fit_forecast_ragged`` then returns a NaN-filled table as
+        wide as the largest ``n_pred[c]``."""
+        blocks = [np.asarray(X, dtype=np.float64) for X in Xs]
+        if not blocks or any(b.ndim != 2 or b.shape[1] != blocks[0].shape[1] for b in blocks):
+            raise ValueError("Xs must be a non-empty list of 2-D designs with the same number of columns")
+        arr = [np.array(v, dtype=np.int32) for v in ([b.shape[0] for b in blocks], t_fit, pred_start, n_pred)]
+        if any(a.shape != (len(blocks),) for a in arr[1:]):
+            raise ValueError("t_fit, pred_start and n_pred need one entry per design")
+        X = np.ascontiguousarray(np.concatenate(blocks, axis=0))
+        N.check(self._lib.mmf_plan_calendars(self._h, X.ctypes.data, len(blocks), arr[0].ctypes.data, arr[1].ctypes.data,
+                                             arr[2].ctypes.data, arr[3].ctypes.data, X.shape[1],
+                                             1 if has_constant else 0))
+        npd = arr[3]
+        # (n_cal, columns of the output table, columns y must have, who writes the table: the fit kernel's epilogue
+        # ("future") or the predict kernel ("holdout"), as mmf_plan_calendars decides)
+        one_window = bool((npd == npd[0]).all() and npd[0] <= 64)
+        self._ragged = (len(blocks), int(npd.max()), int(arr[1].max()), "future" if one_window else "holdout")
 
     def fit_forecast_ragged(self, y, cal_row_start, out=None, status=None, want_status: bool = False,
                             want_stats: bool = False):

@@ -14,6 +14,7 @@ import pytest
 import mmf
 from conftest import ROOT, record_err, tolerance
 from oracle import mmf_oracle as O
+from test_gpu_ragged import _frame_ratio
 
 pytestmark = pytest.mark.gpu
 
@@ -429,10 +430,9 @@ def test_forecast_groups_many_calendars_future_mode_uses_one_ragged_launch():
     assert len(got) == len(want) == 60 * 8
     assert (got["SKU"].to_numpy() == want["SKU"].to_numpy()).all()
     assert (got["Date"].dt.date.to_numpy() == want["Date"].to_numpy()).all()
-    err = np.abs(got["Demand_Fitted"].to_numpy() - want["Demand_Fitted"].to_numpy())
-    # weekly histories of 40-90 points extrapolated 8 weeks: leverage of a few units; scale the tolerance like the
-    # packed tests do (forecast_leverage) with a bound that holds for every calendar of this batch
-    _le(err.max(), 40 * tolerance(df["Demand"].to_numpy()), "ragged DataFrame batch vs per-group oracle UDF")
+    # weekly histories of 40-90 points extrapolated 8 weeks: every group within tolerance x max(1, the leverage of its
+    # own calendar) x its mask factor
+    _le(_frame_ratio(df, got, want, **kw, design="trend_season_exog"), 1.0, "ragged DataFrame batch vs per-group oracle UDF")
 
 
 # ---- host-side narrowing of float32 chunks (half the PCIe bytes), exact or not used ------------------------------------
@@ -575,8 +575,8 @@ def test_forecast_groups_many_calendars_holdout_mode_one_ragged_launch():
     assert (got["SKU"].to_numpy() == want["SKU"].to_numpy()).all()
     assert (got["Date"].dt.date.to_numpy() == want["Date"].to_numpy()).all()
     assert np.array_equal(got["Demand"].to_numpy(), want["Demand"].to_numpy(), equal_nan=True)
-    err = np.abs(got["Demand_Fitted"].to_numpy() - want["Demand_Fitted"].to_numpy())
-    _le(err.max(), 40 * tolerance(df["Demand"].to_numpy()), "ragged holdout DataFrame batch vs per-group oracle UDF")
+    _le(_frame_ratio(df, got, want, "W-MON", 40, "holdout", "trend_season_exog"), 1.0,
+        "ragged holdout DataFrame batch vs per-group oracle UDF")
 
 
 # ---- batches of less than one wave of 128-row tiles on the tensor-core kernel ---------------------------------------

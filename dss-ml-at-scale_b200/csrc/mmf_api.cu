@@ -95,6 +95,7 @@ struct Plan {
   float* d_w = nullptr;
   float* d_ap_hi = nullptr;   // [n_rows][P] tf32-hi / tf32-lo of A: B operand of predict_tc_kernel
   float* d_ap_lo = nullptr;
+  uint32_t* d_nz = nullptr;    // [n_rows] non-zero masks of the whitened rows (AR calls: the used columns of the dof rule)
   float* d_sfac = nullptr;    // [n_rows] sqrt(1 + |a_t|^2) (float64 on the host): se of gap-free rows / sigma
   alignas(64) unsigned char tmap_at[128];
   alignas(64) unsigned char tmap_bhi[128];
@@ -222,7 +223,7 @@ void free_multi(MultiPlan& m) {
 
 void free_plan(Plan& p) {
   cudaFree(p.d_a4); cudaFree(p.d_at); cudaFree(p.d_apred); cudaFree(p.d_w); cudaFree(p.d_ap_hi); cudaFree(p.d_ap_lo);
-  cudaFree(p.d_sfac);
+  cudaFree(p.d_sfac); cudaFree(p.d_nz);
   p = Plan{};
 }
 
@@ -380,6 +381,11 @@ int build_plan(Plan& pl, const double* X, int32_t n_rows, int32_t p, int32_t t_f
   }
   CU_TRY(cudaMalloc(&pl.d_sfac, sfac.size() * sizeof(float)));
   CU_TRY(cudaMemcpy(pl.d_sfac, sfac.data(), sfac.size() * sizeof(float), cudaMemcpyHostToDevice));
+  std::vector<uint32_t> nz(n_rows, 0u);
+  for (int32_t t = 0; t < n_rows; ++t)
+    for (int q = 0; q < P; ++q) nz[t] |= (A[(size_t)t * P + q] != 0.f ? 1u : 0u) << q;
+  CU_TRY(cudaMalloc(&pl.d_nz, nz.size() * sizeof(uint32_t)));
+  CU_TRY(cudaMemcpy(pl.d_nz, nz.data(), nz.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
   int rc = encode_2d(pl.tmap_at, pl.d_at, (uint64_t)pl.t_pad, (uint64_t)(2 * P), (uint64_t)pl.t_pad * 4, 32, 2 * P);
   if (rc != MMF_OK) return rc;
   rc = encode_2d(pl.tmap_bhi, pl.d_ap_hi, (uint64_t)P, (uint64_t)n_rows, (uint64_t)P * 4, P, 128, CU_TENSOR_MAP_SWIZZLE_64B);
@@ -482,7 +488,7 @@ int build_multi(MultiPlan& m, const double* X_all, int32_t n_cal, const int32_t*
 int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pred_start, int32_t n_pred,
                     float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s, int* launches,
                     int* kernel_used, float* const* out_more, int n_out, int multimem, const SelectArgs* sel,
-                    const SeArgs* se = nullptr) {
+                    const SeArgs* se = nullptr, const ArArgs* ar = nullptr) {
   const DesignView d = view_of(ctx->plan);
   FitArgs a{};
   a.y = y; a.n = n; a.ld_y = ld_y; a.pred_start = pred_start; a.n_pred = n_pred;
@@ -498,8 +504,9 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
                           n <= (int64_t)0x7fffffff - 128;
   if (sel != nullptr && !predict_ok)
     return fail(MMF_E_UNSUPPORTED, "model selection needs a 16-B aligned output with ld_out %% 4 == 0");
-  const bool many_pred = sel != nullptr || (n_pred > 64 && kernel != MMF_KERNEL_WARP && predict_ok);
-  if (many_pred) {
+  // AR calls (ar != nullptr) hand gamma / c to ar_kernel, which writes the table itself: no predict_tc requirement
+  const bool many_pred = ar == nullptr && (sel != nullptr || (n_pred > 64 && kernel != MMF_KERNEL_WARP && predict_ok));
+  if (many_pred || ar != nullptr) {
     int rc = grow((void**)&ctx->d_gamma, &ctx->gamma_cap_bytes, (size_t)n * P * sizeof(float));
     if (rc == MMF_OK) rc = grow((void**)&ctx->d_c, &ctx->c_cap_bytes, (size_t)n * sizeof(float));
     if (rc != MMF_OK) return rc;
@@ -572,6 +579,10 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
     CU_TRY(launch_select(d, a, *sel, ctx->sm_count, s));
     ++*launches;
   }
+  if (ar != nullptr) {
+    CU_TRY(launch_ar(d, a, *ar, s));
+    ++*launches;
+  }
   if (many_pred) {
     PredictLaunch pl;
     memcpy(pl.tmap_bhi, ctx->plan.tmap_bhi, 128);
@@ -616,7 +627,8 @@ int64_t slab_rows(const mmf_ctx* ctx, int64_t n) {
 int run_device(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pred_start, int32_t n_pred,
                float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s, int* launches,
                int* kernel_used, float* const* out_more = nullptr, int n_out = 1, int multimem = 0,
-               const SelectArgs* sel = nullptr, uint32_t* slab_pending = nullptr, const SeArgs* se = nullptr) {
+               const SelectArgs* sel = nullptr, uint32_t* slab_pending = nullptr, const SeArgs* se = nullptr,
+               const ArArgs* ar = nullptr) {
   const int64_t slab = slab_rows(ctx, n);
   for (int64_t off = 0, i = 0; off < n; off += slab, ++i) {
     const int64_t m = std::min(slab, n - off);
@@ -635,9 +647,17 @@ int run_device(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pr
       se_slab.sigma += off;
       if (se_slab.dof) se_slab.dof += off;
     }
+    ArArgs ar_slab{};
+    if (ar != nullptr) {
+      ar_slab = *ar;
+      if (ar_slab.phi) ar_slab.phi += off * MMF_AR_MAX;
+      if (ar_slab.order) ar_slab.order += off;
+      if (ar_slab.sigma) ar_slab.sigma += off;
+    }
     const int rc = run_device_slab(ctx, y + off * ld_y, m, ld_y, pred_start, n_pred, out + off * ld_out, ld_out,
                                    beta ? beta + off * P : nullptr, status + off, s, launches, kernel_used, more, n_out,
-                                   multimem, sel != nullptr ? &sel_slab : nullptr, se != nullptr ? &se_slab : nullptr);
+                                   multimem, sel != nullptr ? &sel_slab : nullptr, se != nullptr ? &se_slab : nullptr,
+                                   ar != nullptr ? &ar_slab : nullptr);
     if (rc != MMF_OK) return rc;
     if (slab_pending != nullptr) {
       if (*kernel_used == MMF_KERNEL_TC)
@@ -1182,6 +1202,69 @@ int mmf_fit_forecast_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
   return MMF_OK;
 }
 
+int mmf_fit_forecast_ar_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order, int32_t pred_start,
+                            int32_t n_pred, float* out_pred, int64_t ld_out, float* out_phi, int32_t* out_order,
+                            float* out_sigma, int32_t* out_status, mmf_stats* stats) {
+  if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
+  GrowScope grow_scope(ctx);
+  if (!ctx->plan.valid) return fail(MMF_E_NOPLAN, "mmf_plan_design has not been called");
+  const Plan& pl = ctx->plan;
+  if (n < 0) return fail(MMF_E_INVALID, "n < 0");
+  if (n > 0 && (!y || !out_pred)) return fail(MMF_E_INVALID, "y or out_pred is NULL");
+  if (ar_order < 1 || ar_order > MMF_AR_MAX) return fail(MMF_E_INVALID, "ar_order=%d outside [1,%d]", ar_order, MMF_AR_MAX);
+  if (ld_y < pl.t_fit) return fail(MMF_E_INVALID, "ld_y=%lld < t_fit=%d", (long long)ld_y, pl.t_fit);
+  if (n_pred < 1 || pred_start < 0 || (int64_t)pred_start + n_pred > pl.n_rows)
+    return fail(MMF_E_INVALID, "prediction rows [%d,%d) outside the planned design (%d rows)", pred_start,
+                pred_start + n_pred, pl.n_rows);
+  if (ld_out < n_pred) return fail(MMF_E_INVALID, "ld_out=%lld < n_pred=%d", (long long)ld_out, n_pred);
+  if (stats) memset(stats, 0, sizeof(*stats));
+  if (n == 0) return MMF_OK;
+  CU_TRY(cudaSetDevice(ctx->device));
+  if (!is_device_ptr(y) || !is_device_ptr(out_pred) || (out_phi && !is_device_ptr(out_phi)) ||
+      (out_order && !is_device_ptr(out_order)) || (out_sigma && !is_device_ptr(out_sigma)) ||
+      (out_status && !is_device_ptr(out_status)))
+    return fail(MMF_E_UNSUPPORTED, "mmf_fit_forecast_ar_f32 takes device buffers only");
+  int32_t* status = out_status;
+  if (!status) {
+    int rc = grow_status_scratch(ctx, n, ctx->stream);
+    if (rc != MMF_OK) return rc;
+    status = ctx->d_status_scratch;
+  }
+  ArArgs ar{};
+  ar.p = ar_order; ar.phi = out_phi; ar.order = out_order; ar.sigma = out_sigma; ar.nz = pl.d_nz;
+  const int64_t slab = slab_rows(ctx, n);
+  const int64_t n_slabs = (n + slab - 1) / slab;
+  uint32_t* slab_pending = nullptr;
+  if (stats && n_slabs > 1) {
+    const mmf_ctx* saved = g_grow_ctx;
+    g_grow_ctx = nullptr;
+    const int rc = grow((void**)&ctx->d_slab_pending, &ctx->slab_pending_cap, (size_t)n_slabs * sizeof(uint32_t));
+    g_grow_ctx = saved;
+    if (rc != MMF_OK) return rc;
+    slab_pending = ctx->d_slab_pending;
+  }
+  int launches = 0, kernel_used = 0;
+  if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, ctx->stream));
+  int rc = run_device(ctx, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, nullptr, status, ctx->stream, &launches,
+                      &kernel_used, nullptr, 1, 0, nullptr, slab_pending, nullptr, &ar);
+  if (rc != MMF_OK) return rc;
+  if (stats) {
+    CU_TRY(cudaEventRecord(ctx->ev_k1, ctx->stream));
+    CU_TRY(cudaEventSynchronize(ctx->ev_k1));
+    CU_TRY(cudaEventElapsedTime(&stats->kernel_ms, ctx->ev_k0, ctx->ev_k1));
+    stats->total_ms = stats->kernel_ms;
+    std::vector<uint32_t> pend((size_t)n_slabs, 0u);
+    if (slab_pending != nullptr)
+      CU_TRY(cudaMemcpy(pend.data(), slab_pending, pend.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    else if (kernel_used == MMF_KERNEL_TC)
+      CU_TRY(cudaMemcpy(pend.data(), ctx->d_pending + CTR_WORDS * ctx->last_set, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    for (uint32_t v : pend) stats->n_pending += v;
+    stats->n_series = n;
+    stats->kernel_launches = launches;
+    stats->kernel_used = kernel_used;
+  }
+  return MMF_OK;
+}
 
 // ---- ragged batches: many calendars, one launch ------------------------------------------------------------------
 int mmf_plan_calendars(mmf_ctx* ctx, const double* X_all, int32_t n_cal, const int32_t* n_rows, const int32_t* t_fit,

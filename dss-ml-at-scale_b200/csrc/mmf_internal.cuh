@@ -216,6 +216,17 @@ struct SelectArgs {
 };
 cudaError_t launch_select(const DesignView& d, const FitArgs& a, const SelectArgs& sel, int sm_count, cudaStream_t s);
 
+// regression with AR(p) errors (ar.cu, DESIGN.md section 2 item 9): runs behind the fit passes of a gamma / c hand-off
+// call, reads a.status / a.out_gamma / a.out_c, writes out[row, 0 .. n_pred) itself (any ld_out, any base pointer)
+struct ArArgs {
+  int32_t p;                      // 1 .. MMF_AR_MAX, the same for every series of the call
+  float* phi;                     // nullable [n][MMF_AR_MAX]: Yule-Walker coefficients, 0 beyond the series' order
+  int32_t* order;                 // nullable [n]: the series' order p_i
+  float* sigma;                   // nullable [n]: innovation standard deviation
+  const uint32_t* nz;             // [n_rows] of the planned design: bit q set when whitened column q is non-zero on row t
+};
+cudaError_t launch_ar(const DesignView& d, const FitArgs& a, const ArArgs& ar, cudaStream_t s);
+
 // integer series -> float32 staging rows, sentinel -> NaN (widen.cu); dtype = MMF_DT_I16 / U16 / I32
 cudaError_t launch_widen(int dtype, const void* src, int64_t ld_src, float* dst, int64_t ld_dst, int64_t n, int32_t t,
                          int sm_count, cudaStream_t s);

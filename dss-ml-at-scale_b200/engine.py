@@ -493,6 +493,37 @@ class ForecastEngine:
                                  st.kernel_launches, {N.KERNEL_WARP: "warp", N.KERNEL_TC: "tc"}.get(st.kernel_used, "?"))
         return res
 
+    def fit_forecast_ar(self, y, ar_order: int, pred_start: int, n_pred: int, want_stats: bool = False):
+        """Regression with AR(``ar_order``) errors (``mmf_fit_forecast_ar_f32``, DESIGN.md section 2 item 9): the plain
+        fit, then Yule-Walker AR coefficients of each series' residuals.  ``y`` is a float32 CUDA tensor.  Returns
+        ``{"pred", "phi", "order", "sigma", "status"}`` (torch tensors on y's device): ``pred[i, j]`` the one-step-ahead
+        prediction (in sample) or dynamic forecast from t_fit (beyond it) of design row ``pred_start + j``,
+        ``phi[i, :MMF_AR_MAX]`` the coefficients (zero beyond ``order[i]``, the order the series supports), ``sigma[i]``
+        the innovation standard deviation.  ``status`` is bit-equal to ``fit_forecast``'s."""
+        import torch
+        if self.t_fit is None:
+            raise RuntimeError("plan()/plan_calendar() must be called first")
+        yp, n, t_have, ld_y = _describe(y, "y")
+        if not (_is_torch(y) and y.is_cuda and y.dtype == torch.float32) or t_have < self.t_fit:
+            raise ValueError(f"y must be a float32 CUDA tensor with at least t_fit={self.t_fit} columns")
+        self.set_stream(torch.cuda.current_stream(y.device).cuda_stream)
+        out = torch.empty((n, n_pred), device=y.device, dtype=torch.float32)
+        phi = torch.empty((n, N.AR_MAX), device=y.device, dtype=torch.float32)
+        order = torch.empty(n, device=y.device, dtype=torch.int32)
+        sigma = torch.empty(n, device=y.device, dtype=torch.float32)
+        status = torch.empty(n, device=y.device, dtype=torch.int32)
+        st = N.MmfStats() if want_stats else None
+        N.check(self._lib.mmf_fit_forecast_ar_f32(self._h, yp, n, ld_y, int(ar_order), int(pred_start), int(n_pred),
+                                                  out.data_ptr(), out.stride(0), phi.data_ptr(), order.data_ptr(),
+                                                  sigma.data_ptr(), status.data_ptr(),
+                                                  C.byref(st) if st is not None else None))
+        res = {"pred": out, "phi": phi, "order": order, "sigma": sigma, "status": status}
+        if st is not None:
+            self.launches += st.kernel_launches
+            res["stats"] = Stats(st.kernel_ms, st.total_ms, st.n_series, st.n_pending, st.h2d_bytes, st.d2h_bytes,
+                                 st.kernel_launches, {N.KERNEL_WARP: "warp", N.KERNEL_TC: "tc"}.get(st.kernel_used, "?"))
+        return res
+
     def capture(self, y, pred_start: int, n_pred: int, out=None, status=None):
         """Record one device-resident ``fit_forecast`` call as a CUDA graph.  Small batches are launch-bound (three
         kernel launches plus the Python/ctypes hop cost more than the kernels themselves): ``graph.replay()``

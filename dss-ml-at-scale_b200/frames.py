@@ -23,6 +23,7 @@ import pandas as pd
 
 from . import design as D
 from .engine import ForecastEngine, alloc_packed, default_engine
+from ._native import AR_MAX
 
 FORECAST_HORIZON = 40                      # 02:341
 DEFAULT_KEYS = ("Product", "SKU")          # 02:526
@@ -337,20 +338,25 @@ def _host(x):
     return x.cpu().numpy() if hasattr(x, "cpu") else np.asarray(x)
 
 
-def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, interval=False):
+def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, interval=False, ar=None):
     """Run the engine over every bucket: yields (bucket, out_days, n_pred, y_host, pred_host, se_host or None).
-    ``interval``: prediction standard errors too (``fit_forecast_se``), one call per calendar bucket."""
+    ``interval``: prediction standard errors too (``fit_forecast_se``), one call per calendar bucket.
+    ``ar``: regression with AR(ar) errors (``fit_forecast_ar``), one call per calendar bucket."""
     if interval and select is not None:
         raise ValueError("interval= is not offered with select= (model selection returns point forecasts)")
     t_fit_min = min((b.t_len - (horizon if mode == "holdout" else 0)) for b in buckets) if buckets else 0
-    if (select is None and not interval and len(buckets) >= RAGGED_MIN_BUCKETS and (mode == "holdout" or 1 <= horizon <= 64)
+    if (select is None and not interval and ar is None and len(buckets) >= RAGGED_MIN_BUCKETS and (mode == "holdout" or 1 <= horizon <= 64)
             and hasattr(eng, "fit_forecast_ragged") and t_fit_min >= 33 and all(b.t_len <= 65535 for b in buckets)):
         yield from _fit_buckets_ragged(buckets, eng, freq, horizon, mode, design, on_device)
         return
     for b in buckets:
         out_days, pred_start, n_pred = eng.plan_calendar(b.start, b.t_len, freq, horizon, mode, design)
         se = None
-        if interval:
+        if ar is not None:
+            from .engine import device_packed
+            yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
+            pred = _host(eng.fit_forecast_ar(yd, ar, pred_start, n_pred)["pred"])
+        elif interval:
             from .engine import device_packed
             yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
             res = eng.fit_forecast_se(yd, pred_start, n_pred)
@@ -378,6 +384,17 @@ def _z_of(interval):
     if not 0.0 < level < 1.0:
         raise ValueError(f"interval must be a level in (0, 1), got {interval!r}")
     return NormalDist().inv_cdf(0.5 + level / 2.0)
+
+
+def _ar_order(ar, select, interval):
+    """validated AR order of ``ar=`` (None: the plain model)"""
+    if ar is None:
+        return None
+    if select is not None or interval is not None:
+        raise ValueError("ar= is not offered with select= or interval= (AR forecasts come without either)")
+    if isinstance(ar, bool) or not isinstance(ar, (int, np.integer)) or not 1 <= int(ar) <= AR_MAX:
+        raise ValueError(f"ar must be an AR order in [1, {AR_MAX}], got {ar!r}")
+    return int(ar)
 
 
 def _bounds(pred, se, z):
@@ -483,7 +500,7 @@ def _single_group_fast(pdf, keys, date_col, value_col, freq, horizon, mode, desi
 def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Demand",
                     freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                     engine: ForecastEngine | None = None, pack: str = "host", select=None,
-                    null_keys_on_gaps: bool = False, interval=None) -> pd.DataFrame:
+                    null_keys_on_gaps: bool = False, interval=None, ar=None) -> pd.DataFrame:
     """Fit + forecast every group in ``pdf``; returns ``tuning_schema`` rows
     (keys..., Date, Demand, Demand_Fitted), groups in key order, dates ascending.
 
@@ -508,19 +525,24 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     quantile ``z = NormalDist().inv_cdf(0.5 + level / 2)`` and ``se`` the prediction standard error of each row
     (``ForecastEngine.fit_forecast_se``; NaN where a series has no residual degrees of freedom).  Every calendar bucket
     then takes its own call.  ``interval=None`` leaves the frame as it was.
+
+    ``ar=p`` (1 <= p <= 8) fits regression with AR(p) errors (``ForecastEngine.fit_forecast_ar``, DESIGN.md section 2
+    item 9): ``Demand_Fitted`` holds one-step-ahead predictions on the fit dates and the dynamic forecast after them.
+    The schema is unchanged; every calendar bucket takes its own call.  Not offered with ``select=`` or ``interval=``.
     """
     eng = engine or default_engine()
     keys = list(keys)
     fitted_col = value_col + "_Fitted"
     z = _z_of(interval)
-    if pack == "host" and select is None and z is None and isinstance(pdf, pd.DataFrame):
+    ar = _ar_order(ar, select, interval)
+    if pack == "host" and select is None and z is None and ar is None and isinstance(pdf, pd.DataFrame):
         one = _single_group_fast(pdf, keys, date_col, value_col, freq, horizon, mode, design, eng, null_keys_on_gaps)
         if one is not None:
             return one
     buckets = _buckets_for(pdf, keys, date_col, value_col, freq, pack, eng)
     parts, lengths = [], []
     for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
-                                                              pack == "device", z is not None):
+                                                              pack == "device", z is not None, ar):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n), n_pred)
         # key columns keep the dtype they came in with (no per-row string inference on N x T values)
@@ -611,12 +633,12 @@ def backtest_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
 def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Demand",
                    freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                    engine: ForecastEngine | None = None, pack: str = "host", select=None,
-                   null_keys_on_gaps: bool = False, interval=None):
+                   null_keys_on_gaps: bool = False, interval=None, ar=None):
     """Arrow ``Table``/``RecordBatch`` in -> Arrow ``Table`` with ``tuning_schema`` out (the ``mapInArrow``
     flavour of the boundary).  No pandas frame of the rows on either side: keys are dictionary-encoded on the way
     in and expanded from a dictionary on the way out, dates and values are NumPy views of Arrow buffers.
     ``interval=level`` adds the ``{value}_Lower`` / ``{value}_Upper`` columns of ``forecast_groups`` (schema:
-    ``tuning_schema(..., interval=True)``)."""
+    ``tuning_schema(..., interval=True)``).  ``ar=p`` fits regression with AR(p) errors, as in ``forecast_groups``."""
     import pyarrow as pa
 
     if isinstance(table, pa.RecordBatch):
@@ -624,11 +646,12 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     eng = engine or default_engine()
     keys = list(keys)
     z = _z_of(interval)
+    ar = _ar_order(ar, select, interval)
     schema = tuning_schema(keys, date_col, value_col, interval=z is not None)
     buckets = _buckets_for(table, keys, date_col, value_col, freq, pack, eng)
     parts, lengths = [], []
     for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
-                                                              pack == "device", z is not None):
+                                                              pack == "device", z is not None, ar):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n, dtype=np.int32), n_pred)
         cols = []

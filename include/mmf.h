@@ -31,13 +31,15 @@
 extern "C" {
 #endif
 
-#define MMF_VERSION 104          /* 0.1.4 */
+#define MMF_VERSION 105          /* 0.1.5 */
 #define MMF_P 16                 /* design columns (zero-pad narrower designs) */
 #define MMF_PIVOT_TOL 1e-3f      /* per-series relative Cholesky pivot threshold */
 #define MMF_CAL_TOL 1e-10        /* aliasing threshold on the float64 calendar Gram */
 #define MMF_SELECT_MAX_HOLD 3500 /* held-out rows mmf_fit_select_forecast_f32 accepts (64 B of shared memory each) */
 #define MMF_BT_MAX_ORIGINS 8     /* backtest origins per call (mmf_plan_backtest) */
 #define MMF_BT_NMETRIC 4         /* backtest metrics per (origin, series): MSE, MAE, bias, MAPE */
+#define MMF_AR_MAX 8             /* largest AR order of mmf_fit_forecast_ar_f32 */
+#define MMF_AR_KAPPA_MAX 0.999   /* Levinson-Durbin stops before a partial autocorrelation |kappa| >= this */
 
 /* return codes */
 #define MMF_OK 0
@@ -175,6 +177,27 @@ int mmf_fit_forecast_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
                             float* out_pred, int64_t ld_out,
                             float* out_se, int64_t ld_se,
                             float* out_sigma, int32_t* out_dof,
+                            int32_t* out_status, mmf_stats* stats);
+
+/* Regression with AR(p) errors (DESIGN.md section 2 item 9): the plain fit (gamma, c, kept columns and out_status bit-equal
+ * to mmf_fit_forecast_f32 on the same inputs), then per series, from the residuals e_t = y_t - c - a_t.gamma of the observed
+ * fit rows:
+ *   r_k = (1/n_obs) sum e_t e_{t-k} over the pairs with both rows observed (k = 0..ar_order, float64, not demeaned);
+ *   order p_i = 0 when dof = n_obs - used columns <= ar_order, else the last order float64 Levinson-Durbin completes
+ *   before r_0 <= 0 or |kappa_j| >= MMF_AR_KAPPA_MAX; phi_1..phi_{p_i} Yule-Walker, sigma_eps^2 = r_0 prod (1 - kappa_j^2);
+ *   filled residuals u_s = e_s (observed) or sum_j phi_j u_{s-j} (missing, and every s >= t_fit), u_s = 0 for s < 0;
+ *   out_pred[i, t - pred_start] = c + a_t.gamma + sum_j phi_j u_{t-j}: one-step-ahead in sample, the dynamic forecast
+ *   from origin t_fit beyond it.  y is never read at or beyond t_fit.
+ * 1 <= ar_order <= MMF_AR_MAX.  out_phi [n][MMF_AR_MAX] (zero beyond the series' order), out_order [n] and out_sigma [n]
+ * (sqrt(sigma_eps^2)) are nullable; empty series (status 1) get order 0, phi 0, sigma NaN and NaN predictions.  Device
+ * buffers only (host pointers: MMF_E_UNSUPPORTED); any ld_out >= n_pred and any base pointer, only columns [0, n_pred)
+ * written; enqueue-only unless `stats` is non-NULL; mmf_config.kernel and assume_finite are honoured.  Refused arguments
+ * write nothing.
+ * replaces: SARIMAX(p, 0, 0) + exog fit and predict of the reference's per-group model (02:441-450, 472-488 with p > 0),
+ * for a caller-fixed order and the two-step (OLS, then Yule-Walker on the residuals) estimator. */
+int mmf_fit_forecast_ar_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
+                            int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out,
+                            float* out_phi, int32_t* out_order, float* out_sigma,
                             int32_t* out_status, mmf_stats* stats);
 
 /* ---- ragged batches: groups on MANY calendars in one launch ---------------------------------------------

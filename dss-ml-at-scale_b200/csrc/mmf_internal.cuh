@@ -147,7 +147,9 @@ cudaError_t launch_solve_rows(const DesignView& d, const FitArgs& a, int sm_coun
 // se rows of the gap-free rows of a fit + predict_tc call: out_se[i, k] = sigma_i * sfac[pred_start + k] for every row
 // whose status is MMF_STATUS_OK right after fit_tc_kernel (launched before the passes that finish the other rows)
 cudaError_t launch_se_outer(const FitArgs& a, const SeArgs& se, int sm_count, cudaStream_t s);
-constexpr int CTR_WORDS = 8;             // one counter set: {rows left pending, solve records queued, 6 unused words}
+constexpr int CTR_WORDS = 8;             // one counter set: {rows left pending, solve records queued, tiles claimed by
+                                         // fit_tc beyond its first wave, 5 unused words}
+constexpr int CTR_TILE_CLAIM = 2;
 
 // fitted values + forecasts for MANY prediction rows (the reference's "Demand_Fitted for every date"
 // contract, 02:484-494): out[n, n_pred] = c + gamma A_pred^T as a wgmma GEMM with TMA-stored tiles

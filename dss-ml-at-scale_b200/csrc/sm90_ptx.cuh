@@ -170,6 +170,19 @@ __device__ __forceinline__ void bulk_wait_all_elect() {        // ... and have b
       "elect.sync _|pe, 0xffffffff;\n\t"
       "@pe cp.async.bulk.wait_group 0;\n\t}" ::: "memory");
 }
+// plain stores with an L2 eviction policy (a policy register made by createpolicy, not the TMA hint constants above)
+__device__ __forceinline__ uint64_t l2_evict_first_policy() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ void stg128_hint(void* dst, float4 v, uint64_t policy) {
+  asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;"
+               ::"l"(dst), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(policy) : "memory");
+}
+__device__ __forceinline__ void stg32_hint(void* dst, uint32_t v, uint64_t policy) {
+  asm volatile("st.global.L2::cache_hint.b32 [%0], %1, %2;" ::"l"(dst), "r"(v), "l"(policy) : "memory");
+}
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }

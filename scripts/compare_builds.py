@@ -1,0 +1,130 @@
+"""Runs the same seeded workloads through two builds of libmmf.so and checks that every output is bit-identical.
+
+Each build runs in its own process (the library is chosen with MMF_LIB when the package loads) and saves its outputs
+to an .npz; the parent process then compares them array by array, NaN payloads included.  Exit code 1 on any
+difference.  Needs one GPU.
+
+    python scripts/compare_builds.py --lib-a before.so --lib-b dss-ml-at-scale_b200/libmmf.so [--n 262144] [--out DIR]
+
+Workloads (synthetic daily demand, 1,095 days, 28-day horizon):
+  future           future mode, the flagship call
+  holdout          holdout mode (the reference's contract: a value for every date)
+  missing2         2 % of the values missing in every series
+  gaps10           a 10-day gap in 2 % of the series, plus rows whose first 8 values are all missing
+  ragged64         64 calendars of 400 to 1,095 days in one ragged launch
+  se               the standard-error call
+  backtest4        a backtest at K = 4 origins
+"""
+import argparse
+import os
+import subprocess
+import sys
+import tempfile
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+T, H = 1095, 28
+
+
+def produce(path, n):
+    import torch
+    sys.path.insert(0, ROOT)
+    import mmf
+    dev = torch.device("cuda", 0)
+    y, start = mmf.synth.daily_store_item_demand_torch(n, T, seed=4321, device=dev)
+    out = {}
+
+    def keep(name, **arrays):
+        for k, v in arrays.items():
+            out[f"{name}.{k}"] = v.detach().cpu().numpy() if hasattr(v, "detach") else np.asarray(v)
+
+    eng = mmf.ForecastEngine(device=0)
+    _, ps, npred = eng.plan_calendar(start, T, "D", H, "future")
+    r = eng.fit_forecast(y, ps, npred, want_status=True)
+    keep("future", pred=r["pred"], status=r["status"])
+
+    g = torch.Generator(device=dev).manual_seed(7)
+    ym = mmf.device_packed(y, device=dev)         # keeps the 16-B row pitch the tensor-core path reads
+    ym[torch.rand(ym.shape, generator=g, device=dev) < 0.02] = float("nan")
+    r = eng.fit_forecast(ym, ps, npred, want_status=True)
+    keep("missing2", pred=r["pred"], status=r["status"])
+
+    yg = mmf.device_packed(y, device=dev)
+    rows = torch.randperm(n, generator=g, device=dev)[: n // 50]
+    first = torch.randint(30, T - 30, (rows.numel(),), generator=g, device=dev)
+    for k in range(10):
+        yg[rows, first + k] = float("nan")
+    yg[rows[:64], :8] = float("nan")            # no finite value among the first 8: the centring rule's corner
+    yg[rows[64:128], :5] = float("nan")
+    r = eng.fit_forecast(yg, ps, npred, want_status=True)
+    keep("gaps10", pred=r["pred"], status=r["status"])
+
+    r = eng.fit_forecast_se(ym, ps, npred)
+    keep("se", **r)
+    eng.close()
+
+    engh = mmf.ForecastEngine(device=0)
+    _, psh, nph = engh.plan_calendar(start, T, "D", H, "holdout")
+    r = engh.fit_forecast(yg, psh, nph, want_status=True)
+    keep("holdout", pred=r["pred"], status=r["status"])
+    engh.close()
+
+    engr = mmf.ForecastEngine(device=0)
+    C = 64
+    t_lens = np.linspace(400, T, C).astype(int)
+    starts = [np.datetime64(start, "D") + np.timedelta64(int(T - tl), "D") for tl in t_lens]
+    engr.plan_calendars(starts, t_lens, "D", H)
+    cal_rows = np.linspace(0, n, C + 1).astype(np.int64)
+    r = engr.fit_forecast_ragged(ym, cal_rows, want_status=True)
+    keep("ragged64", pred=r["pred"], status=r["status"])
+    engr.close()
+
+    engb = mmf.ForecastEngine(device=0)
+    engb.plan_backtest(start, T, "D", H, n_origins=4)
+    r = engb.backtest(yg)
+    keep("backtest4", **r)
+    engb.close()
+    torch.cuda.synchronize()
+    np.savez(path, **out)
+
+
+def same_bits(a, b):
+    if a.shape != b.shape or a.dtype != b.dtype:
+        return False
+    return np.array_equal(np.ascontiguousarray(a).view(np.uint8), np.ascontiguousarray(b).view(np.uint8))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--lib-a", required=True)
+    ap.add_argument("--lib-b", required=True)
+    ap.add_argument("--n", type=int, default=262144, help="series per workload")
+    ap.add_argument("--out", default=None, help="keep the two .npz files here")
+    ap.add_argument("--produce", default=None, help=argparse.SUPPRESS)
+    args = ap.parse_args()
+    if args.produce:
+        produce(args.produce, args.n)
+        return
+    out_dir = args.out or tempfile.mkdtemp(prefix="mmf_cmp_")
+    os.makedirs(out_dir, exist_ok=True)
+    files = []
+    for tag, lib in (("a", args.lib_a), ("b", args.lib_b)):
+        path = os.path.join(out_dir, f"outputs_{tag}.npz")
+        env = dict(os.environ, MMF_LIB=os.path.abspath(lib))
+        subprocess.run([sys.executable, os.path.abspath(__file__), "--lib-a", lib, "--lib-b", lib, "--n", str(args.n),
+                        "--produce", path], env=env, check=True)
+        files.append(path)
+    a, b = np.load(files[0]), np.load(files[1])
+    bad = []
+    for k in sorted(set(a.files) | set(b.files)):
+        if k not in a.files or k not in b.files or not same_bits(a[k], b[k]):
+            bad.append(k)
+        print(f"{k:24s} {'DIFFERS' if k in bad else 'bit-identical'}", flush=True)
+    if bad:
+        sys.exit(f"{len(bad)} outputs differ between {args.lib_a} and {args.lib_b}: {', '.join(bad)}")
+    print(f"all {len(a.files)} outputs bit-identical")
+
+
+if __name__ == "__main__":
+    main()

@@ -567,10 +567,12 @@ fit_warp_kernel(const DesignView d, const FitArgs a, const int smem_rows, const 
 
 }  // namespace
 
+constexpr size_t FIT_WARP_SMEM_MAX = 200 * 1024;
+
 size_t fit_warp_smem_bytes(const DesignView& d, int* smem_rows) {
   // one CTA per SM: keep as many design rows resident as fit beside the per-warp scratch
   const size_t scratch = sizeof(WarpScratch) * WARPS;
-  const size_t budget = 200 * 1024 - scratch;
+  const size_t budget = FIT_WARP_SMEM_MAX - scratch;
   int rows = d.n_rows_pad;
   const int max_rows = (int)(budget / (4 * sizeof(float4))) & ~31;
   if (rows > max_rows) rows = max_rows;
@@ -583,7 +585,9 @@ cudaError_t launch_fit_warp(const DesignView& d, const FitArgs& a, int sm_count,
   int smem_rows = 0;
   const size_t smem = fit_warp_smem_bytes(d, &smem_rows);
   auto kern = se != nullptr ? fit_warp_kernel<true> : fit_warp_kernel<false>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  // the attribute is per function and process-wide: always the same value, the most any design needs, so that a
+  // context on another host thread cannot lower it between this launch's set and the launch
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FIT_WARP_SMEM_MAX);
   if (e != cudaSuccess) return e;
   int per_sm = 0;
   e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, THREADS, smem);

@@ -173,6 +173,7 @@ struct mmf_ctx {
   bool own_stream = false;
   cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
   cudaEvent_t ev_a = nullptr, ev_b = nullptr, ev_k0 = nullptr, ev_k1 = nullptr;
+  cudaEvent_t ev_switch = nullptr;     // mmf_set_stream: the new stream waits for what the old one holds
   uint32_t* d_pending = nullptr;       // 3 counter sets of CTR_WORDS words {rows left PENDING, solve records queued,
                                        // ...}: 0/1 ping-pong between eager calls, 2 belongs to captured CUDA graphs
                                        // (zeroed by a node of the graph)
@@ -744,6 +745,7 @@ int mmf_create(const mmf_config* cfg, mmf_ctx** out) {
   if ((e = cudaStreamCreateWithFlags(&ctx->s_h2d, cudaStreamNonBlocking)) != cudaSuccess) return bail(e, "cudaStreamCreate");
   if ((e = cudaStreamCreateWithFlags(&ctx->s_d2h, cudaStreamNonBlocking)) != cudaSuccess) return bail(e, "cudaStreamCreate");
   cudaEventCreate(&ctx->ev_a); cudaEventCreate(&ctx->ev_b); cudaEventCreate(&ctx->ev_k0); cudaEventCreate(&ctx->ev_k1);
+  if ((e = cudaEventCreateWithFlags(&ctx->ev_switch, cudaEventDisableTiming)) != cudaSuccess) return bail(e, "cudaEventCreate");
   for (int i = 0; i < NBUF; ++i) {
     cudaEventCreateWithFlags(&ctx->st[i].ev_h2d, cudaEventDisableTiming);
     cudaEventCreateWithFlags(&ctx->st[i].ev_comp, cudaEventDisableTiming);
@@ -789,6 +791,7 @@ int mmf_destroy(mmf_ctx* ctx) {
   if (ctx->ev_b) cudaEventDestroy(ctx->ev_b);
   if (ctx->ev_k0) cudaEventDestroy(ctx->ev_k0);
   if (ctx->ev_k1) cudaEventDestroy(ctx->ev_k1);
+  if (ctx->ev_switch) cudaEventDestroy(ctx->ev_switch);
   if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
   if (ctx->s_h2d) cudaStreamDestroy(ctx->s_h2d);
   if (ctx->s_d2h) cudaStreamDestroy(ctx->s_d2h);
@@ -798,8 +801,29 @@ int mmf_destroy(mmf_ctx* ctx) {
 
 int mmf_set_stream(mmf_ctx* ctx, void* cuda_stream) {
   if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
-  if (ctx->own_stream && ctx->stream) { cudaStreamSynchronize(ctx->stream); cudaStreamDestroy(ctx->stream); }
-  ctx->stream = (cudaStream_t)cuda_stream;      // NULL = legacy default stream
+  cudaStream_t next = (cudaStream_t)cuda_stream;  // NULL = legacy default stream
+  if (next == ctx->stream) return MMF_OK;         // the common case: nothing to order
+  if (ctx->own_stream && ctx->stream) {
+    cudaStreamSynchronize(ctx->stream);
+    cudaStreamDestroy(ctx->stream);
+  } else {
+    // Every call shares the context's counter sets and scratch, and the host's record of which counter set is zero
+    // assumes the calls run in the order they were made: the new stream waits for the work enqueued on the old one.
+    // Not when either stream is capturing: an event recorded in a capture cannot order work outside it, and
+    // torch.cuda.graph synchronises the device before a capture begins.  The new stream is asked first: querying the
+    // legacy stream during a global-mode capture would invalidate that capture.
+    CU_TRY(cudaSetDevice(ctx->device));
+    cudaStreamCaptureStatus cap_next = cudaStreamCaptureStatusNone, cap_prev = cudaStreamCaptureStatusNone;
+    CU_TRY(cudaStreamIsCapturing(next, &cap_next));
+    if (cap_next == cudaStreamCaptureStatusNone) {
+      CU_TRY(cudaStreamIsCapturing(ctx->stream, &cap_prev));
+      if (cap_prev == cudaStreamCaptureStatusNone) {
+        CU_TRY(cudaEventRecord(ctx->ev_switch, ctx->stream));
+        CU_TRY(cudaStreamWaitEvent(next, ctx->ev_switch, 0));
+      }
+    }
+  }
+  ctx->stream = next;
   ctx->own_stream = false;
   return MMF_OK;
 }

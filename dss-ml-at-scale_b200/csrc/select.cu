@@ -99,7 +99,10 @@ cudaError_t launch_select(const DesignView& d, const FitArgs& a, const SelectArg
   const unsigned grid = (unsigned)(want < cap ? want : cap);
   const size_t smem = (size_t)sel.n_hold * P * sizeof(float);       // <= MMF_SELECT_MAX_HOLD * 64 B (validated at the ABI)
   if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    // the attribute is per function and process-wide: always the same value, the largest any call needs, so that a
+    // context on another host thread cannot lower it between this call's set and its launch
+    cudaError_t e = cudaFuncSetAttribute(select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)(MMF_SELECT_MAX_HOLD * P * sizeof(float)));
     if (e != cudaSuccess) return e;
   }
   select_kernel<<<grid, THREADS, smem, s>>>(d, a, sel);

@@ -103,7 +103,13 @@ int mmf_device_count(int32_t* count);
 /* replaces: the Spark Python worker that hosts the UDF (one ctx per worker process) */
 int mmf_create(const mmf_config* cfg, mmf_ctx** out);
 int mmf_destroy(mmf_ctx* ctx);
-int mmf_set_stream(mmf_ctx* ctx, void* cuda_stream);   /* borrow e.g. torch's current stream */
+/* Borrow a stream, e.g. torch's current one; NULL = the legacy default stream.  The context's calls share its counter
+ * sets and scratch, so they must run on the device in the order they were made.  When `cuda_stream` differs from the
+ * stream in use, the new stream waits (an event, no host synchronisation) for everything already enqueued on the old
+ * one.  Setting the stream in use again costs nothing.  No wait is added while either stream is capturing: a capture
+ * cannot order work outside it (torch.cuda.graph synchronises the device before it begins).  A borrowed stream must
+ * stay valid until the next mmf_set_stream or mmf_destroy. */
+int mmf_set_stream(mmf_ctx* ctx, void* cuda_stream);
 int mmf_synchronize(mmf_ctx* ctx);
 
 /* ---- design plan --------------------------------------------------------
@@ -121,6 +127,9 @@ int mmf_plan_design(mmf_ctx* ctx, const double* X, int32_t n_rows, int32_t p,
  * mmf_pin_scratch(ctx, +1) after a capture makes every later call that would have to move that memory (a larger
  * batch, mmf_plan_design) fail with MMF_E_UNSUPPORTED instead of leaving the graph with dangling pointers;
  * mmf_pin_scratch(ctx, -1) when the graph is destroyed.  Counted: one +1 per live graph.
+ * A replay does not pass through mmf_set_stream, and every graph of a context shares one counter set and the scratch
+ * with the eager calls: replay on the stream the context's calls use, or order it with them yourself.  Replays
+ * running concurrently with each other, or with eager calls on another stream, are not supported.
  * replaces: nothing in the reference (Spark re-launches a Python task per group, 02:523-528); it is the H100
  * answer to that per-task launch overhead for small batches.                                                   */
 int mmf_pin_scratch(mmf_ctx* ctx, int32_t delta);

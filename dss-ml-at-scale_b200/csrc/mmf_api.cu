@@ -489,7 +489,7 @@ int build_multi(MultiPlan& m, const double* X_all, int32_t n_cal, const int32_t*
 int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pred_start, int32_t n_pred,
                     float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s, int* launches,
                     int* kernel_used, float* const* out_more, int n_out, int multimem, const SelectArgs* sel,
-                    const SeArgs* se = nullptr, const ArArgs* ar = nullptr) {
+                    const SeArgs* se = nullptr, const ArArgs* ar = nullptr, const ArSelArgs* arsel = nullptr) {
   const DesignView d = view_of(ctx->plan);
   FitArgs a{};
   a.y = y; a.n = n; a.ld_y = ld_y; a.pred_start = pred_start; a.n_pred = n_pred;
@@ -581,7 +581,7 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
     ++*launches;
   }
   if (ar != nullptr) {
-    CU_TRY(launch_ar(d, a, *ar, s));
+    CU_TRY(arsel != nullptr ? launch_ar_select(d, a, *ar, *arsel, s) : launch_ar(d, a, *ar, s));
     ++*launches;
   }
   if (many_pred) {
@@ -629,7 +629,7 @@ int run_device(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pr
                float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s, int* launches,
                int* kernel_used, float* const* out_more = nullptr, int n_out = 1, int multimem = 0,
                const SelectArgs* sel = nullptr, uint32_t* slab_pending = nullptr, const SeArgs* se = nullptr,
-               const ArArgs* ar = nullptr) {
+               const ArArgs* ar = nullptr, const ArSelArgs* arsel = nullptr) {
   const int64_t slab = slab_rows(ctx, n);
   for (int64_t off = 0, i = 0; off < n; off += slab, ++i) {
     const int64_t m = std::min(slab, n - off);
@@ -655,10 +655,17 @@ int run_device(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pr
       if (ar_slab.order) ar_slab.order += off;
       if (ar_slab.sigma) ar_slab.sigma += off;
     }
+    ArSelArgs arsel_slab{};
+    if (arsel != nullptr) {
+      arsel_slab = *arsel;
+      if (arsel_slab.choice) arsel_slab.choice += off;
+      if (arsel_slab.mse) arsel_slab.mse += off;
+      if (arsel_slab.cand_mse) arsel_slab.cand_mse += off * arsel_slab.n_cand;
+    }
     const int rc = run_device_slab(ctx, y + off * ld_y, m, ld_y, pred_start, n_pred, out + off * ld_out, ld_out,
                                    beta ? beta + off * P : nullptr, status + off, s, launches, kernel_used, more, n_out,
                                    multimem, sel != nullptr ? &sel_slab : nullptr, se != nullptr ? &se_slab : nullptr,
-                                   ar != nullptr ? &ar_slab : nullptr);
+                                   ar != nullptr ? &ar_slab : nullptr, arsel != nullptr ? &arsel_slab : nullptr);
     if (rc != MMF_OK) return rc;
     if (slab_pending != nullptr) {
       if (*kernel_used == MMF_KERNEL_TC)
@@ -1226,6 +1233,50 @@ int mmf_fit_forecast_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
   return MMF_OK;
 }
 
+// the enqueue / stats tail of the AR entry points (arguments already checked, n > 0, device set)
+static int run_ar_call(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pred_start, int32_t n_pred,
+                       float* out_pred, int64_t ld_out, int32_t* out_status, const ArArgs& ar, const ArSelArgs* arsel,
+                       mmf_stats* stats) {
+  int32_t* status = out_status;
+  if (!status) {
+    int rc = grow_status_scratch(ctx, n, ctx->stream);
+    if (rc != MMF_OK) return rc;
+    status = ctx->d_status_scratch;
+  }
+  const int64_t slab = slab_rows(ctx, n);
+  const int64_t n_slabs = (n + slab - 1) / slab;
+  uint32_t* slab_pending = nullptr;
+  if (stats && n_slabs > 1) {
+    const mmf_ctx* saved = g_grow_ctx;
+    g_grow_ctx = nullptr;
+    const int rc = grow((void**)&ctx->d_slab_pending, &ctx->slab_pending_cap, (size_t)n_slabs * sizeof(uint32_t));
+    g_grow_ctx = saved;
+    if (rc != MMF_OK) return rc;
+    slab_pending = ctx->d_slab_pending;
+  }
+  int launches = 0, kernel_used = 0;
+  if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, ctx->stream));
+  int rc = run_device(ctx, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, nullptr, status, ctx->stream, &launches,
+                      &kernel_used, nullptr, 1, 0, nullptr, slab_pending, nullptr, &ar, arsel);
+  if (rc != MMF_OK) return rc;
+  if (stats) {
+    CU_TRY(cudaEventRecord(ctx->ev_k1, ctx->stream));
+    CU_TRY(cudaEventSynchronize(ctx->ev_k1));
+    CU_TRY(cudaEventElapsedTime(&stats->kernel_ms, ctx->ev_k0, ctx->ev_k1));
+    stats->total_ms = stats->kernel_ms;
+    std::vector<uint32_t> pend((size_t)n_slabs, 0u);
+    if (slab_pending != nullptr)
+      CU_TRY(cudaMemcpy(pend.data(), slab_pending, pend.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    else if (kernel_used == MMF_KERNEL_TC)
+      CU_TRY(cudaMemcpy(pend.data(), ctx->d_pending + CTR_WORDS * ctx->last_set, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    for (uint32_t v : pend) stats->n_pending += v;
+    stats->n_series = n;
+    stats->kernel_launches = launches;
+    stats->kernel_used = kernel_used;
+  }
+  return MMF_OK;
+}
+
 int mmf_fit_forecast_ar_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order, int32_t pred_start,
                             int32_t n_pred, float* out_pred, int64_t ld_out, float* out_phi, int32_t* out_order,
                             float* out_sigma, int32_t* out_status, mmf_stats* stats) {
@@ -1248,46 +1299,51 @@ int mmf_fit_forecast_ar_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
       (out_order && !is_device_ptr(out_order)) || (out_sigma && !is_device_ptr(out_sigma)) ||
       (out_status && !is_device_ptr(out_status)))
     return fail(MMF_E_UNSUPPORTED, "mmf_fit_forecast_ar_f32 takes device buffers only");
-  int32_t* status = out_status;
-  if (!status) {
-    int rc = grow_status_scratch(ctx, n, ctx->stream);
-    if (rc != MMF_OK) return rc;
-    status = ctx->d_status_scratch;
-  }
   ArArgs ar{};
   ar.p = ar_order; ar.phi = out_phi; ar.order = out_order; ar.sigma = out_sigma; ar.nz = pl.d_nz;
-  const int64_t slab = slab_rows(ctx, n);
-  const int64_t n_slabs = (n + slab - 1) / slab;
-  uint32_t* slab_pending = nullptr;
-  if (stats && n_slabs > 1) {
-    const mmf_ctx* saved = g_grow_ctx;
-    g_grow_ctx = nullptr;
-    const int rc = grow((void**)&ctx->d_slab_pending, &ctx->slab_pending_cap, (size_t)n_slabs * sizeof(uint32_t));
-    g_grow_ctx = saved;
-    if (rc != MMF_OK) return rc;
-    slab_pending = ctx->d_slab_pending;
-  }
-  int launches = 0, kernel_used = 0;
-  if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, ctx->stream));
-  int rc = run_device(ctx, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, nullptr, status, ctx->stream, &launches,
-                      &kernel_used, nullptr, 1, 0, nullptr, slab_pending, nullptr, &ar);
-  if (rc != MMF_OK) return rc;
-  if (stats) {
-    CU_TRY(cudaEventRecord(ctx->ev_k1, ctx->stream));
-    CU_TRY(cudaEventSynchronize(ctx->ev_k1));
-    CU_TRY(cudaEventElapsedTime(&stats->kernel_ms, ctx->ev_k0, ctx->ev_k1));
-    stats->total_ms = stats->kernel_ms;
-    std::vector<uint32_t> pend((size_t)n_slabs, 0u);
-    if (slab_pending != nullptr)
-      CU_TRY(cudaMemcpy(pend.data(), slab_pending, pend.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
-    else if (kernel_used == MMF_KERNEL_TC)
-      CU_TRY(cudaMemcpy(pend.data(), ctx->d_pending + CTR_WORDS * ctx->last_set, sizeof(uint32_t), cudaMemcpyDeviceToHost));
-    for (uint32_t v : pend) stats->n_pending += v;
-    stats->n_series = n;
-    stats->kernel_launches = launches;
-    stats->kernel_used = kernel_used;
-  }
-  return MMF_OK;
+  return run_ar_call(ctx, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, stats);
+}
+
+int mmf_fit_select_ar_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
+                          const int32_t* orders, int32_t n_orders, int32_t pred_start, int32_t n_pred,
+                          float* out_pred, int64_t ld_out, int32_t* out_choice, float* out_mse, float* out_cand_mse,
+                          float* out_phi, int32_t* out_order, float* out_sigma, int32_t* out_status, mmf_stats* stats) {
+  if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
+  GrowScope grow_scope(ctx);
+  if (!ctx->plan.valid) return fail(MMF_E_NOPLAN, "mmf_plan_design has not been called");
+  const Plan& pl = ctx->plan;
+  if (n < 0) return fail(MMF_E_INVALID, "n < 0");
+  if (n > 0 && (!y || !out_pred)) return fail(MMF_E_INVALID, "y or out_pred is NULL");
+  if (!orders || n_orders < 1 || n_orders > MMF_ARSEL_MAX_CAND)
+    return fail(MMF_E_INVALID, "n_orders=%d outside [1,%d] (or orders is NULL)", n_orders, MMF_ARSEL_MAX_CAND);
+  for (int j = 0; j < n_orders; ++j)
+    if (orders[j] < 0 || orders[j] > MMF_AR_MAX || (j > 0 && orders[j] <= orders[j - 1]))
+      return fail(MMF_E_INVALID, "orders must be ascending and distinct in [0,%d] (orders[%d]=%d)", MMF_AR_MAX, j,
+                  orders[j]);
+  if (n_hold < 1 || (int64_t)pl.t_fit + n_hold > pl.n_rows)
+    return fail(MMF_E_INVALID, "held-out rows [%d,%lld) outside the planned design (%d rows)", pl.t_fit,
+                (long long)pl.t_fit + n_hold, pl.n_rows);
+  if (ld_y < (int64_t)pl.t_fit + n_hold)
+    return fail(MMF_E_INVALID, "ld_y=%lld < t_fit + n_hold=%lld", (long long)ld_y, (long long)pl.t_fit + n_hold);
+  if (n_pred < 1 || pred_start < 0 || (int64_t)pred_start + n_pred > pl.n_rows)
+    return fail(MMF_E_INVALID, "prediction rows [%d,%d) outside the planned design (%d rows)", pred_start,
+                pred_start + n_pred, pl.n_rows);
+  if (ld_out < n_pred) return fail(MMF_E_INVALID, "ld_out=%lld < n_pred=%d", (long long)ld_out, n_pred);
+  if (stats) memset(stats, 0, sizeof(*stats));
+  if (n == 0) return MMF_OK;
+  CU_TRY(cudaSetDevice(ctx->device));
+  if (!is_device_ptr(y) || !is_device_ptr(out_pred) || (out_choice && !is_device_ptr(out_choice)) ||
+      (out_mse && !is_device_ptr(out_mse)) || (out_cand_mse && !is_device_ptr(out_cand_mse)) ||
+      (out_phi && !is_device_ptr(out_phi)) || (out_order && !is_device_ptr(out_order)) ||
+      (out_sigma && !is_device_ptr(out_sigma)) || (out_status && !is_device_ptr(out_status)))
+    return fail(MMF_E_UNSUPPORTED, "mmf_fit_select_ar_f32 takes device buffers only");
+  ArArgs ar{};
+  ar.p = orders[n_orders - 1]; ar.phi = out_phi; ar.order = out_order; ar.sigma = out_sigma; ar.nz = pl.d_nz;
+  ArSelArgs sel{};
+  sel.n_hold = n_hold; sel.n_cand = n_orders;
+  for (int j = 0; j < n_orders; ++j) sel.cand[j] = orders[j];
+  sel.choice = out_choice; sel.mse = out_mse; sel.cand_mse = out_cand_mse;
+  return run_ar_call(ctx, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, &sel, stats);
 }
 
 // ---- ragged batches: many calendars, one launch ------------------------------------------------------------------

@@ -221,13 +221,27 @@ cudaError_t launch_select(const DesignView& d, const FitArgs& a, const SelectArg
 // regression with AR(p) errors (ar.cu, DESIGN.md section 2 item 9): runs behind the fit passes of a gamma / c hand-off
 // call, reads a.status / a.out_gamma / a.out_c, writes out[row, 0 .. n_pred) itself (any ld_out, any base pointer)
 struct ArArgs {
-  int32_t p;                      // 1 .. MMF_AR_MAX, the same for every series of the call
+  int32_t p;                      // 1 .. MMF_AR_MAX (selection: the largest candidate, 0 .. MMF_AR_MAX), one per call
   float* phi;                     // nullable [n][MMF_AR_MAX]: Yule-Walker coefficients, 0 beyond the series' order
   int32_t* order;                 // nullable [n]: the series' order p_i
   float* sigma;                   // nullable [n]: innovation standard deviation
   const uint32_t* nz;             // [n_rows] of the planned design: bit q set when whitened column q is non-zero on row t
 };
 cudaError_t launch_ar(const DesignView& d, const FitArgs& a, const ArArgs& ar, cudaStream_t s);
+
+// per-series AR order selection by hold-out MSE (ar.cu, DESIGN.md section 2 item 10): the ar_kernel passes with
+// ArArgs::p = the largest candidate, a scoring walk over the held-out rows [t_fit, t_fit + n_hold) per candidate, and
+// pass B with the winner's order
+struct ArSelArgs {
+  int32_t n_hold;                           // held-out rows: design rows [t_fit, t_fit + n_hold), y columns likewise
+  int32_t n_cand;                           // 1 .. MMF_ARSEL_MAX_CAND
+  int32_t cand[MMF_ARSEL_MAX_CAND];         // ascending distinct orders in [0, MMF_AR_MAX], last == ArArgs::p
+  int32_t* choice;                          // nullable [n]: the chosen order (-1 for empty series)
+  float* mse;                               // nullable [n]: hold-out MSE of the chosen order
+  float* cand_mse;                          // nullable [n][n_cand]: hold-out MSE of every candidate
+};
+cudaError_t launch_ar_select(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArSelArgs& sel,
+                             cudaStream_t s);
 
 // integer series -> float32 staging rows, sentinel -> NaN (widen.cu); dtype = MMF_DT_I16 / U16 / I32
 cudaError_t launch_widen(int dtype, const void* src, int64_t ld_src, float* dst, int64_t ld_dst, int64_t n, int32_t t,

@@ -524,6 +524,52 @@ class ForecastEngine:
                                  st.kernel_launches, {N.KERNEL_WARP: "warp", N.KERNEL_TC: "tc"}.get(st.kernel_used, "?"))
         return res
 
+    def fit_select_ar(self, y, n_hold: int, orders=(0, 1, 2, 3, 4), pred_start: int = 0, n_pred: int | None = None,
+                      want_stats: bool = False):
+        """Regression with AR(p) errors, p chosen per series by hold-out MSE (``mmf_fit_select_ar_f32``, DESIGN.md
+        section 2 item 10).  Candidate m of ``orders`` (ascending, distinct, 0 .. MMF_AR_MAX) is ``fit_forecast_ar``
+        with ``ar_order = m`` (m = 0: the plain regression); it is scored by the MSE of its dynamic forecast from t_fit
+        over the held-out design rows [t_fit, t_fit + n_hold) against y's columns there, and the first minimum wins.
+        ``y`` is a float32 CUDA tensor with at least t_fit + n_hold columns.  ``n_pred`` defaults to every design row
+        from ``pred_start`` on.  Returns ``{"pred", "choice", "mse", "cand_mse", "phi", "order", "sigma", "status"}``
+        (torch tensors on y's device): ``pred`` the chosen candidate's predictions, ``choice[i]`` its order (-1 for empty
+        series), ``mse[i]`` its hold-out MSE, ``cand_mse[i, j]`` that of ``orders[j]``, ``phi`` / ``order`` / ``sigma``
+        as in ``fit_forecast_ar`` for the chosen order."""
+        import torch
+        if self.t_fit is None:
+            raise RuntimeError("plan()/plan_calendar() must be called first")
+        orders = [int(m) for m in orders]
+        yp, n, t_have, ld_y = _describe(y, "y")
+        if not (_is_torch(y) and y.is_cuda and y.dtype == torch.float32) or t_have < self.t_fit + int(n_hold):
+            raise ValueError(f"y must be a float32 CUDA tensor with at least t_fit + n_hold={self.t_fit + int(n_hold)} "
+                             "columns")
+        if n_pred is None:
+            n_pred = self.n_rows - int(pred_start)
+        self.set_stream(torch.cuda.current_stream(y.device).cuda_stream)
+        dev = y.device
+        out = torch.empty((n, n_pred), device=dev, dtype=torch.float32)
+        choice = torch.empty(n, device=dev, dtype=torch.int32)
+        mse = torch.empty(n, device=dev, dtype=torch.float32)
+        cand_mse = torch.empty((n, len(orders)), device=dev, dtype=torch.float32)
+        phi = torch.empty((n, N.AR_MAX), device=dev, dtype=torch.float32)
+        order = torch.empty(n, device=dev, dtype=torch.int32)
+        sigma = torch.empty(n, device=dev, dtype=torch.float32)
+        status = torch.empty(n, device=dev, dtype=torch.int32)
+        cand = (C.c_int32 * max(len(orders), 1))(*orders)
+        st = N.MmfStats() if want_stats else None
+        N.check(self._lib.mmf_fit_select_ar_f32(self._h, yp, n, ld_y, int(n_hold), cand, len(orders), int(pred_start),
+                                                int(n_pred), out.data_ptr(), out.stride(0), choice.data_ptr(),
+                                                mse.data_ptr(), cand_mse.data_ptr(), phi.data_ptr(), order.data_ptr(),
+                                                sigma.data_ptr(), status.data_ptr(),
+                                                C.byref(st) if st is not None else None))
+        res = {"pred": out, "choice": choice, "mse": mse, "cand_mse": cand_mse, "phi": phi, "order": order,
+               "sigma": sigma, "status": status}
+        if st is not None:
+            self.launches += st.kernel_launches
+            res["stats"] = Stats(st.kernel_ms, st.total_ms, st.n_series, st.n_pending, st.h2d_bytes, st.d2h_bytes,
+                                 st.kernel_launches, {N.KERNEL_WARP: "warp", N.KERNEL_TC: "tc"}.get(st.kernel_used, "?"))
+        return res
+
     def capture(self, y, pred_start: int, n_pred: int, out=None, status=None):
         """Record one device-resident ``fit_forecast`` call as a CUDA graph.  Small batches are launch-bound (three
         kernel launches plus the Python/ctypes hop cost more than the kernels themselves): ``graph.replay()``

@@ -341,7 +341,8 @@ def _host(x):
 def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, interval=False, ar=None):
     """Run the engine over every bucket: yields (bucket, out_days, n_pred, y_host, pred_host, se_host or None).
     ``interval``: prediction standard errors too (``fit_forecast_se``), one call per calendar bucket.
-    ``ar``: regression with AR(ar) errors (``fit_forecast_ar``), one call per calendar bucket."""
+    ``ar``: regression with AR(ar) errors (``fit_forecast_ar``), one call per calendar bucket; a tuple of orders
+    chooses the order per series by hold-out MSE over the last ``horizon`` rows (``fit_select_ar``)."""
     if interval and select is not None:
         raise ValueError("interval= is not offered with select= (model selection returns point forecasts)")
     t_fit_min = min((b.t_len - (horizon if mode == "holdout" else 0)) for b in buckets) if buckets else 0
@@ -352,7 +353,11 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
     for b in buckets:
         out_days, pred_start, n_pred = eng.plan_calendar(b.start, b.t_len, freq, horizon, mode, design)
         se = None
-        if ar is not None:
+        if isinstance(ar, tuple):
+            from .engine import device_packed
+            yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
+            pred = _host(eng.fit_select_ar(yd, horizon, ar, pred_start, n_pred)["pred"])
+        elif ar is not None:
             from .engine import device_packed
             yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
             pred = _host(eng.fit_forecast_ar(yd, ar, pred_start, n_pred)["pred"])
@@ -386,12 +391,24 @@ def _z_of(interval):
     return NormalDist().inv_cdf(0.5 + level / 2.0)
 
 
-def _ar_order(ar, select, interval):
-    """validated AR order of ``ar=`` (None: the plain model)"""
+def _ar_order(ar, select, interval, mode="holdout"):
+    """validated AR order of ``ar=`` (None: the plain model), or the tuple of candidate orders of a sequence"""
     if ar is None:
         return None
     if select is not None or interval is not None:
         raise ValueError("ar= is not offered with select= or interval= (AR forecasts come without either)")
+    if isinstance(ar, (list, tuple, np.ndarray)):
+        orders = list(ar)
+        if not orders:
+            raise ValueError("ar= needs at least one candidate order")
+        if any(isinstance(m, bool) or not isinstance(m, (int, np.integer)) or not 0 <= int(m) <= AR_MAX for m in orders):
+            raise ValueError(f"ar= candidate orders must be integers in [0, {AR_MAX}], got {ar!r}")
+        orders = [int(m) for m in orders]
+        if any(b <= a for a, b in zip(orders, orders[1:])):
+            raise ValueError(f"ar= candidate orders must be ascending and distinct, got {ar!r}")
+        if mode != "holdout":
+            raise ValueError("ar= with candidate orders needs mode='holdout' (the last horizon rows score the candidates)")
+        return tuple(orders)
     if isinstance(ar, bool) or not isinstance(ar, (int, np.integer)) or not 1 <= int(ar) <= AR_MAX:
         raise ValueError(f"ar must be an AR order in [1, {AR_MAX}], got {ar!r}")
     return int(ar)
@@ -529,12 +546,16 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     ``ar=p`` (1 <= p <= 8) fits regression with AR(p) errors (``ForecastEngine.fit_forecast_ar``, DESIGN.md section 2
     item 9): ``Demand_Fitted`` holds one-step-ahead predictions on the fit dates and the dynamic forecast after them.
     The schema is unchanged; every calendar bucket takes its own call.  Not offered with ``select=`` or ``interval=``.
+    ``ar=(0, 1, 2, 3, 4)`` (ascending distinct orders in 0..8; the reference's ``p`` range by default) chooses each
+    series' order by the MSE of its dynamic forecast over the last ``horizon`` dates, the held-out rows of
+    ``mode='holdout'`` (``ForecastEngine.fit_select_ar``, DESIGN.md section 2 item 10); ``Demand_Fitted`` comes from each
+    series' winner.  Holdout mode only.
     """
     eng = engine or default_engine()
     keys = list(keys)
     fitted_col = value_col + "_Fitted"
     z = _z_of(interval)
-    ar = _ar_order(ar, select, interval)
+    ar = _ar_order(ar, select, interval, mode)
     if pack == "host" and select is None and z is None and ar is None and isinstance(pdf, pd.DataFrame):
         one = _single_group_fast(pdf, keys, date_col, value_col, freq, horizon, mode, design, eng, null_keys_on_gaps)
         if one is not None:
@@ -638,7 +659,8 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     flavour of the boundary).  No pandas frame of the rows on either side: keys are dictionary-encoded on the way
     in and expanded from a dictionary on the way out, dates and values are NumPy views of Arrow buffers.
     ``interval=level`` adds the ``{value}_Lower`` / ``{value}_Upper`` columns of ``forecast_groups`` (schema:
-    ``tuning_schema(..., interval=True)``).  ``ar=p`` fits regression with AR(p) errors, as in ``forecast_groups``."""
+    ``tuning_schema(..., interval=True)``).  ``ar=p`` fits regression with AR(p) errors and ``ar=(0, 1, 2, 3, 4)`` chooses the order per series, as in
+    ``forecast_groups``."""
     import pyarrow as pa
 
     if isinstance(table, pa.RecordBatch):
@@ -646,7 +668,7 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     eng = engine or default_engine()
     keys = list(keys)
     z = _z_of(interval)
-    ar = _ar_order(ar, select, interval)
+    ar = _ar_order(ar, select, interval, mode)
     schema = tuning_schema(keys, date_col, value_col, interval=z is not None)
     buckets = _buckets_for(table, keys, date_col, value_col, freq, pack, eng)
     parts, lengths = [], []

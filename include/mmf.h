@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define MMF_VERSION 105          /* 0.1.5 */
+#define MMF_VERSION 106          /* 0.1.6 */
 #define MMF_P 16                 /* design columns (zero-pad narrower designs) */
 #define MMF_PIVOT_TOL 1e-3f      /* per-series relative Cholesky pivot threshold */
 #define MMF_CAL_TOL 1e-10        /* aliasing threshold on the float64 calendar Gram */
@@ -40,6 +40,7 @@ extern "C" {
 #define MMF_BT_NMETRIC 4         /* backtest metrics per (origin, series): MSE, MAE, bias, MAPE */
 #define MMF_AR_MAX 8             /* largest AR order of mmf_fit_forecast_ar_f32 */
 #define MMF_AR_KAPPA_MAX 0.999   /* Levinson-Durbin stops before a partial autocorrelation |kappa| >= this */
+#define MMF_ARSEL_MAX_CAND 9     /* candidate AR orders per mmf_fit_select_ar_f32 call (0 .. MMF_AR_MAX) */
 
 /* return codes */
 #define MMF_OK 0
@@ -208,6 +209,36 @@ int mmf_fit_forecast_ar_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
                             int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out,
                             float* out_phi, int32_t* out_order, float* out_sigma,
                             int32_t* out_status, mmf_stats* stats);
+
+/* Regression with AR(p) errors, the order p chosen per series by hold-out MSE (DESIGN.md section 2 item 10).  The fit rows
+ * are [0, t_fit) of the planned design, the held-out rows [t_fit, t_fit + n_hold) of the design and of y.
+ *   candidate m >= 1 is mmf_fit_forecast_ar_f32 with ar_order = m (the same residuals, r_k, dof rule, Levinson-Durbin,
+ *   phi, sigma and fill); candidate 0 is the plain regression c + a_t.gamma (phi 0, order 0, sigma = sqrt(r_0));
+ *   score of m: the MSE of the dynamic forecast from origin t_fit over the held-out rows (the predictions of
+ *   mmf_fit_forecast_ar_f32(ar_order = m, pred_start = t_fit, n_pred = n_hold)) against y[t_fit, t_fit + n_hold), over
+ *   the points where both are finite, summed in float64, stored as float32, NaN where no point is scored.  Held-out y
+ *   never enters the recursion: the score is multi-step, not one-step-ahead;
+ *   choice: the first minimum of the float64 MSE in list order (equal models go to the smaller order); the last listed
+ *   candidate when no point is scored.
+ * out_pred[i, t - pred_start] is then the prediction of the chosen candidate: bit-equal to mmf_fit_forecast_ar_f32
+ * (ar_order = choice) for choice >= 1 (pred, phi, order, sigma, status), c + a_t.gamma for choice 0.  y is read on
+ * [0, t_fit + n_hold) only; held-out values reach the output only through the choice.
+ * orders [n_orders] is a host array of 1 .. MMF_ARSEL_MAX_CAND ascending distinct orders in [0, MMF_AR_MAX];
+ * 1 <= n_hold, t_fit + n_hold <= the planned rows, ld_y >= t_fit + n_hold.  out_choice [n] (the chosen order, -1 for
+ * empty series), out_mse [n] (its hold-out MSE), out_cand_mse [n][n_orders] (every candidate's), out_phi [n][MMF_AR_MAX],
+ * out_order [n] (the effective order, <= the choice), out_sigma [n] and out_status [n] are nullable.  Empty series
+ * (status 1) get choice -1, order 0, phi 0 and NaN sigma, MSEs and predictions.  Otherwise the contract of
+ * mmf_fit_forecast_ar_f32: device buffers only, any ld_out >= n_pred and any base pointer, enqueue-only unless `stats`
+ * is non-NULL, mmf_config.kernel and assume_finite honoured, refused arguments write nothing.
+ * replaces: the reference's per-group tuning loop over p (02:435-488: SARIMAX candidates fit on the train rows, scored by
+ * the MSE of their forecast over the last FORECAST_HORIZON rows, 02:453-459, the best order refit and predicted,
+ * 02:472-488) as an exhaustive search over p with d = q = 0, not TPE over (p, d, q). */
+int mmf_fit_select_ar_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
+                          const int32_t* orders, int32_t n_orders, int32_t pred_start, int32_t n_pred,
+                          float* out_pred, int64_t ld_out,
+                          int32_t* out_choice, float* out_mse, float* out_cand_mse,
+                          float* out_phi, int32_t* out_order, float* out_sigma,
+                          int32_t* out_status, mmf_stats* stats);
 
 /* ---- ragged batches: groups on MANY calendars in one launch ---------------------------------------------
  * The reference re-indexes every group on its own calendar (sort_values + asfreq per group, 02:422-423), so one

@@ -144,6 +144,14 @@ struct BtPlan {
   float* d_tmat = nullptr;             // [K][P][P] T_k = W^-1 W_k
 };
 
+// ARIMA plan (DESIGN.md section 4.15): the differenced designs D_d, d = 1 .. max_diff, each planned by build_plan as
+// mmf_plan_design would plan it (no centring); n_rows / t_fit are the level rows of the calendar
+struct ArimaPlan {
+  bool valid = false;
+  int32_t max_diff = 0, n_rows = 0, t_fit = 0;
+  Plan diff[MMF_DIFF_MAX];
+};
+
 constexpr int NBUF = 3;
 
 struct Staging {
@@ -202,6 +210,8 @@ struct mmf_ctx {
   Plan plan;
   MultiPlan multi;
   BtPlan bt;
+  ArimaPlan arima;
+  float* d_z = nullptr;  size_t z_cap_bytes = 0;           // ARIMA calls: z' of one slab, round4(t_fit - d) per row
   float* d_bt_mom = nullptr;  size_t bt_mom_cap = 0;   // backtest scratch, per slab: moments at the earlier origins,
   SolveRec* d_bt_recs = nullptr;  size_t bt_recs_cap = 0;   // [K][slab] records, [K][slab] work lists,
   int64_t* d_bt_rows = nullptr;  size_t bt_rows_cap = 0;
@@ -226,6 +236,11 @@ void free_plan(Plan& p) {
   cudaFree(p.d_a4); cudaFree(p.d_at); cudaFree(p.d_apred); cudaFree(p.d_w); cudaFree(p.d_ap_hi); cudaFree(p.d_ap_lo);
   cudaFree(p.d_sfac); cudaFree(p.d_nz);
   p = Plan{};
+}
+
+void free_arima(ArimaPlan& m) {
+  for (Plan& p : m.diff) free_plan(p);
+  m = ArimaPlan{};
 }
 
 void free_bt(BtPlan& b) {
@@ -486,11 +501,26 @@ int build_multi(MultiPlan& m, const double* X_all, int32_t n_cal, const int32_t*
 }
 
 // Enqueue the fit of ONE slab of device-resident rows on `s`.  status must be non-null.
-int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pred_start, int32_t n_pred,
-                    float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s, int* launches,
-                    int* kernel_used, float* const* out_more, int n_out, int multimem, const SelectArgs* sel,
-                    const SeArgs* se = nullptr, const ArArgs* ar = nullptr, const ArSelArgs* arsel = nullptr) {
-  const DesignView d = view_of(ctx->plan);
+// ARIMA calls (arima != nullptr, with ar): y / ld_y are the slab's levels; diff_kernel writes z' into the context's
+// scratch first, and the fit passes and arima_kernel read z' with `plan` = the plan of D_d.
+int run_device_slab(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, int64_t ld_y, int32_t pred_start,
+                    int32_t n_pred, float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s,
+                    int* launches, int* kernel_used, float* const* out_more, int n_out, int multimem,
+                    const SelectArgs* sel, const SeArgs* se = nullptr, const ArArgs* ar = nullptr,
+                    const ArSelArgs* arsel = nullptr, const ArimaArgs* arima = nullptr) {
+  const DesignView d = view_of(plan);
+  ArimaArgs ma{};
+  if (arima != nullptr) {
+    ma = *arima;
+    ma.y = y;
+    const int64_t ld_z = (plan.t_fit + 3) & ~3;              // 16-B row pitch: fit_tc's TMA path
+    int rc = grow((void**)&ctx->d_z, &ctx->z_cap_bytes, (size_t)n * ld_z * sizeof(float));
+    if (rc != MMF_OK) return rc;
+    CU_TRY(launch_diff(ma, ctx->d_z, ld_z, n, ctx->sm_count, s));
+    ++*launches;
+    y = ctx->d_z;
+    ld_y = ld_z;
+  }
   FitArgs a{};
   a.y = y; a.n = n; a.ld_y = ld_y; a.pred_start = pred_start; a.n_pred = n_pred;
   a.out = out; a.ld_out = ld_out; a.out_beta = beta; a.status = status;
@@ -548,7 +578,7 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
     TcLaunch tl;
     int rc = encode_2d(tl.tmap_y, y, (uint64_t)d.t_fit, (uint64_t)n, (uint64_t)ld_y * 4, 32, 128);
     if (rc != MMF_OK) return rc;
-    memcpy(tl.tmap_at, ctx->plan.tmap_at, 128);
+    memcpy(tl.tmap_at, plan.tmap_at, 128);
     if (se != nullptr) {
       CU_TRY(launch_fit_tc_se(d, a, tl, counters, ctx->sm_count, s, *se));
       ++*launches;
@@ -581,13 +611,14 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
     ++*launches;
   }
   if (ar != nullptr) {
-    CU_TRY(arsel != nullptr ? launch_ar_select(d, a, *ar, *arsel, s) : launch_ar(d, a, *ar, s));
+    CU_TRY(arima != nullptr ? launch_arima(d, a, *ar, ma, s)
+                            : arsel != nullptr ? launch_ar_select(d, a, *ar, *arsel, s) : launch_ar(d, a, *ar, s));
     ++*launches;
   }
   if (many_pred) {
     PredictLaunch pl;
-    memcpy(pl.tmap_bhi, ctx->plan.tmap_bhi, 128);
-    memcpy(pl.tmap_blo, ctx->plan.tmap_blo, 128);
+    memcpy(pl.tmap_bhi, plan.tmap_bhi, 128);
+    memcpy(pl.tmap_blo, plan.tmap_blo, 128);
     // the map stops at the last whole 16 B of a row (TMA clips with 16-B granularity); the kernel stores the
     // n_pred % 4 columns behind it itself, so the caller's columns from n_pred on are never written
     pl.n_tma = n_pred & ~3;
@@ -611,10 +642,10 @@ int run_device_slab(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32
 // slab, not to the batch.  One slab for batches up to a million rows; beyond that the slab is sized so the scratch
 // stays under ~5 % of the input (10 M x 365: 4 slabs, 0.7 GB instead of 2.6 GB).  Slabs run back to back on the
 // stream; the scratch of slab i is free again when slab i+1 starts (stream order).
-int64_t slab_rows(const mmf_ctx* ctx, int64_t n) {
+int64_t slab_rows(const Plan& plan, int64_t n) {
   int64_t slab = n;
   if (n > (int64_t)1 << 20) {
-    const double input_bytes = (double)n * (double)ctx->plan.t_fit * 4.0;
+    const double input_bytes = (double)n * (double)plan.t_fit * 4.0;
     slab = std::max<int64_t>((int64_t)1 << 20, (int64_t)(0.05 * input_bytes / (double)(sizeof(SolveRec) + sizeof(int64_t))));
     slab = std::min(n, (slab + 127) & ~(int64_t)127);                 // whole 128-row tiles
     const int64_t n_slabs = (n + slab - 1) / slab;
@@ -625,12 +656,13 @@ int64_t slab_rows(const mmf_ctx* ctx, int64_t n) {
 
 // slab_pending (nullable, one word per slab): each slab's count of rows handed to the general pass is copied there
 // before the next slab's tensor-core kernel zeroes the counter set it was kept in (0 for a slab fit by the warp kernel).
-int run_device(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pred_start, int32_t n_pred,
-               float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s, int* launches,
-               int* kernel_used, float* const* out_more = nullptr, int n_out = 1, int multimem = 0,
+// `plan`: the design every slab is fit against (ctx->plan, or the differenced plan of an ARIMA call)
+int run_device(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, int64_t ld_y, int32_t pred_start,
+               int32_t n_pred, float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s,
+               int* launches, int* kernel_used, float* const* out_more = nullptr, int n_out = 1, int multimem = 0,
                const SelectArgs* sel = nullptr, uint32_t* slab_pending = nullptr, const SeArgs* se = nullptr,
-               const ArArgs* ar = nullptr, const ArSelArgs* arsel = nullptr) {
-  const int64_t slab = slab_rows(ctx, n);
+               const ArArgs* ar = nullptr, const ArSelArgs* arsel = nullptr, const ArimaArgs* arima = nullptr) {
+  const int64_t slab = slab_rows(plan, n);
   for (int64_t off = 0, i = 0; off < n; off += slab, ++i) {
     const int64_t m = std::min(slab, n - off);
     float* more[MAX_OUT - 1] = {};
@@ -662,10 +694,10 @@ int run_device(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pr
       if (arsel_slab.mse) arsel_slab.mse += off;
       if (arsel_slab.cand_mse) arsel_slab.cand_mse += off * arsel_slab.n_cand;
     }
-    const int rc = run_device_slab(ctx, y + off * ld_y, m, ld_y, pred_start, n_pred, out + off * ld_out, ld_out,
+    const int rc = run_device_slab(ctx, plan, y + off * ld_y, m, ld_y, pred_start, n_pred, out + off * ld_out, ld_out,
                                    beta ? beta + off * P : nullptr, status + off, s, launches, kernel_used, more, n_out,
                                    multimem, sel != nullptr ? &sel_slab : nullptr, se != nullptr ? &se_slab : nullptr,
-                                   ar != nullptr ? &ar_slab : nullptr, arsel != nullptr ? &arsel_slab : nullptr);
+                                   ar != nullptr ? &ar_slab : nullptr, arsel != nullptr ? &arsel_slab : nullptr, arima);
     if (rc != MMF_OK) return rc;
     if (slab_pending != nullptr) {
       if (*kernel_used == MMF_KERNEL_TC)
@@ -771,6 +803,8 @@ int mmf_destroy(mmf_ctx* ctx) {
   free_plan(ctx->plan);
   free_multi(ctx->multi);
   free_bt(ctx->bt);
+  free_arima(ctx->arima);
+  cudaFree(ctx->d_z);
   cudaFree(ctx->d_bt_mom); cudaFree(ctx->d_bt_recs); cudaFree(ctx->d_bt_rows); cudaFree(ctx->d_bt_ctr); cudaFree(ctx->d_bt_pred);
   for (int i = 0; i < NBUF; ++i) {
     Staging& s = ctx->st[i];
@@ -917,7 +951,7 @@ static int fit_forecast_impl(mmf_ctx* ctx, const void* y_any, int32_t dtype, int
     // Several slabs: every slab's tensor-core kernel zeroes the counter set the slab before it used, so the pending
     // count of each slab is copied aside as it completes and summed here.  A call with stats synchronises and so is
     // never captured: this scratch is not part of any graph and may grow while one is pinned.
-    const int64_t slab = slab_rows(ctx, n);
+    const int64_t slab = slab_rows(ctx->plan, n);
     const int64_t n_slabs = (n + slab - 1) / slab;
     uint32_t* slab_pending = nullptr;
     if (stats && n_slabs > 1) {
@@ -929,8 +963,8 @@ static int fit_forecast_impl(mmf_ctx* ctx, const void* y_any, int32_t dtype, int
       slab_pending = ctx->d_slab_pending;
     }
     if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, ctx->stream));
-    int rc = run_device(ctx, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_beta, status, ctx->stream,
-                        &launches, &kernel_used, nullptr, 1, 0, nullptr, slab_pending);
+    int rc = run_device(ctx, ctx->plan, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_beta, status,
+                        ctx->stream, &launches, &kernel_used, nullptr, 1, 0, nullptr, slab_pending);
     if (rc != MMF_OK) return rc;
     if (stats) {
       CU_TRY(cudaEventRecord(ctx->ev_k1, ctx->stream));
@@ -1105,7 +1139,8 @@ static int fit_forecast_impl(mmf_ctx* ctx, const void* y_any, int32_t dtype, int
       float* bk = out_beta ? (b_dev ? out_beta + off * P : s.d_beta) : nullptr;
       int32_t* sk = (out_status && s_dev) ? out_status + off : s.d_status;
       if (it >= NBUF) CU_TRY(cudaStreamWaitEvent(ctx->stream, s.ev_d2h, 0));        // output staging drained
-      int rc = run_device(ctx, yk, m, ldk, pred_start, n_pred, ok, ldo, bk, sk, ctx->stream, &launches, &kernel_used);
+      int rc = run_device(ctx, ctx->plan, yk, m, ldk, pred_start, n_pred, ok, ldo, bk, sk, ctx->stream, &launches,
+                          &kernel_used);
       if (rc != MMF_OK) return rc;
       CU_TRY(cudaEventRecord(s.ev_comp, ctx->stream));
       bool any_d2h = false;
@@ -1199,7 +1234,7 @@ int mmf_fit_forecast_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
     if (rc != MMF_OK) return rc;
     se.sigma = ctx->d_sigma_scratch;
   }
-  const int64_t slab = slab_rows(ctx, n);
+  const int64_t slab = slab_rows(ctx->plan, n);
   const int64_t n_slabs = (n + slab - 1) / slab;
   uint32_t* slab_pending = nullptr;
   if (stats && n_slabs > 1) {
@@ -1212,8 +1247,8 @@ int mmf_fit_forecast_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
   }
   int launches = 0, kernel_used = 0;
   if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, ctx->stream));
-  int rc = run_device(ctx, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, nullptr, status, ctx->stream, &launches,
-                      &kernel_used, nullptr, 1, 0, nullptr, slab_pending, &se);
+  int rc = run_device(ctx, ctx->plan, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, nullptr, status, ctx->stream,
+                      &launches, &kernel_used, nullptr, 1, 0, nullptr, slab_pending, &se);
   if (rc != MMF_OK) return rc;
   if (stats) {
     CU_TRY(cudaEventRecord(ctx->ev_k1, ctx->stream));
@@ -1234,16 +1269,16 @@ int mmf_fit_forecast_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
 }
 
 // the enqueue / stats tail of the AR entry points (arguments already checked, n > 0, device set)
-static int run_ar_call(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pred_start, int32_t n_pred,
-                       float* out_pred, int64_t ld_out, int32_t* out_status, const ArArgs& ar, const ArSelArgs* arsel,
-                       mmf_stats* stats) {
+static int run_ar_call(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, int64_t ld_y, int32_t pred_start,
+                       int32_t n_pred, float* out_pred, int64_t ld_out, int32_t* out_status, const ArArgs& ar,
+                       const ArSelArgs* arsel, const ArimaArgs* arima, mmf_stats* stats) {
   int32_t* status = out_status;
   if (!status) {
     int rc = grow_status_scratch(ctx, n, ctx->stream);
     if (rc != MMF_OK) return rc;
     status = ctx->d_status_scratch;
   }
-  const int64_t slab = slab_rows(ctx, n);
+  const int64_t slab = slab_rows(plan, n);
   const int64_t n_slabs = (n + slab - 1) / slab;
   uint32_t* slab_pending = nullptr;
   if (stats && n_slabs > 1) {
@@ -1256,8 +1291,8 @@ static int run_ar_call(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, in
   }
   int launches = 0, kernel_used = 0;
   if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, ctx->stream));
-  int rc = run_device(ctx, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, nullptr, status, ctx->stream, &launches,
-                      &kernel_used, nullptr, 1, 0, nullptr, slab_pending, nullptr, &ar, arsel);
+  int rc = run_device(ctx, plan, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, nullptr, status, ctx->stream,
+                      &launches, &kernel_used, nullptr, 1, 0, nullptr, slab_pending, nullptr, &ar, arsel, arima);
   if (rc != MMF_OK) return rc;
   if (stats) {
     CU_TRY(cudaEventRecord(ctx->ev_k1, ctx->stream));
@@ -1301,7 +1336,7 @@ int mmf_fit_forecast_ar_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
     return fail(MMF_E_UNSUPPORTED, "mmf_fit_forecast_ar_f32 takes device buffers only");
   ArArgs ar{};
   ar.p = ar_order; ar.phi = out_phi; ar.order = out_order; ar.sigma = out_sigma; ar.nz = pl.d_nz;
-  return run_ar_call(ctx, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, stats);
+  return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, nullptr, stats);
 }
 
 int mmf_fit_select_ar_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
@@ -1343,7 +1378,89 @@ int mmf_fit_select_ar_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y,
   sel.n_hold = n_hold; sel.n_cand = n_orders;
   for (int j = 0; j < n_orders; ++j) sel.cand[j] = orders[j];
   sel.choice = out_choice; sel.mse = out_mse; sel.cand_mse = out_cand_mse;
-  return run_ar_call(ctx, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, &sel, stats);
+  return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, &sel, nullptr, stats);
+}
+
+// ---- regression with ARIMA(p, d, 0) errors (DESIGN.md section 2 item 11) ------------------------------------------
+int mmf_plan_arima(mmf_ctx* ctx, const double* X, int32_t n_rows, int32_t p, int32_t t_fit, int32_t max_diff) {
+  if (!ctx || !X) return fail(MMF_E_INVALID, "ctx or X is NULL");
+  if (p < 1 || p > P) return fail(MMF_E_INVALID, "p=%d outside [1,%d]", p, P);
+  if (max_diff < 1 || max_diff > MMF_DIFF_MAX)
+    return fail(MMF_E_INVALID, "max_diff=%d outside [1,%d]", max_diff, MMF_DIFF_MAX);
+  if (t_fit - max_diff < 1 || n_rows < t_fit)
+    return fail(MMF_E_INVALID, "need 1 <= t_fit - max_diff and t_fit <= n_rows (t_fit=%d n_rows=%d max_diff=%d)", t_fit,
+                n_rows, max_diff);
+  for (int64_t i = 0; i < (int64_t)n_rows * p; ++i)
+    if (!std::isfinite(X[i])) return fail(MMF_E_INVALID, "design matrix has a non-finite entry at %lld", (long long)i);
+  // every argument check comes before the previous ARIMA plan is freed (the mmf_plan_calendars rule).
+  // D_d row s = Delta^d x_{s+d} in float64.  A column whose differences on the fit rows are cancellation residue of the
+  // raw column (largest |value| <= 1e-12 x the raw column's there) is zeroed, so the whitening drops it instead of
+  // scaling rounding noise up to unit norm (Delta^2 of a linear trend).
+  std::vector<double> raw_max(p, 0.0);
+  for (int32_t t = 0; t < t_fit; ++t)
+    for (int j = 0; j < p; ++j) raw_max[j] = std::max(raw_max[j], std::fabs(X[(int64_t)t * p + j]));
+  std::vector<std::vector<double>> D(max_diff);
+  for (int d = 1; d <= max_diff; ++d) {
+    const double* prev = d == 1 ? X : D[d - 2].data();
+    std::vector<double>& Dd = D[d - 1];
+    Dd.resize((size_t)(n_rows - d) * p);
+    for (int32_t s = 0; s < n_rows - d; ++s)
+      for (int j = 0; j < p; ++j) Dd[(size_t)s * p + j] = prev[(size_t)(s + 1) * p + j] - prev[(size_t)s * p + j];
+  }
+  for (int d = 1; d <= max_diff; ++d) {
+    std::vector<double>& Dd = D[d - 1];
+    for (int j = 0; j < p; ++j) {
+      double mx = 0.0;
+      for (int32_t s = 0; s < t_fit - d; ++s) mx = std::max(mx, std::fabs(Dd[(size_t)s * p + j]));
+      if (mx <= 1e-12 * raw_max[j])
+        for (int32_t s = 0; s < n_rows - d; ++s) Dd[(size_t)s * p + j] = 0.0;
+    }
+  }
+  CU_TRY(cudaSetDevice(ctx->device));
+  CU_TRY(cudaStreamSynchronize(ctx->stream));
+  free_arima(ctx->arima);
+  for (int d = 1; d <= max_diff; ++d) {
+    const int rc = build_plan(ctx->arima.diff[d - 1], D[d - 1].data(), n_rows - d, p, t_fit - d, 0);
+    if (rc != MMF_OK) { free_arima(ctx->arima); return rc; }
+  }
+  ctx->arima.max_diff = max_diff;
+  ctx->arima.n_rows = n_rows;
+  ctx->arima.t_fit = t_fit;
+  ctx->arima.valid = true;
+  return MMF_OK;
+}
+
+int mmf_fit_forecast_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
+                               int32_t diff_order, int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out,
+                               float* out_phi, int32_t* out_order, float* out_sigma, int32_t* out_status,
+                               mmf_stats* stats) {
+  if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
+  GrowScope grow_scope(ctx);
+  if (!ctx->arima.valid) return fail(MMF_E_NOPLAN, "mmf_plan_arima has not been called");
+  const ArimaPlan& ap = ctx->arima;
+  if (n < 0) return fail(MMF_E_INVALID, "n < 0");
+  if (n > 0 && (!y || !out_pred)) return fail(MMF_E_INVALID, "y or out_pred is NULL");
+  if (ar_order < 0 || ar_order > MMF_AR_MAX) return fail(MMF_E_INVALID, "ar_order=%d outside [0,%d]", ar_order, MMF_AR_MAX);
+  if (diff_order < 1 || diff_order > ap.max_diff)
+    return fail(MMF_E_INVALID, "diff_order=%d outside [1,%d] (the planned max_diff)", diff_order, ap.max_diff);
+  if (ld_y < ap.t_fit) return fail(MMF_E_INVALID, "ld_y=%lld < t_fit=%d", (long long)ld_y, ap.t_fit);
+  if (n_pred < 1 || pred_start < 0 || (int64_t)pred_start + n_pred > ap.n_rows)
+    return fail(MMF_E_INVALID, "prediction rows [%d,%d) outside the planned design (%d rows)", pred_start,
+                pred_start + n_pred, ap.n_rows);
+  if (ld_out < n_pred) return fail(MMF_E_INVALID, "ld_out=%lld < n_pred=%d", (long long)ld_out, n_pred);
+  if (stats) memset(stats, 0, sizeof(*stats));
+  if (n == 0) return MMF_OK;
+  CU_TRY(cudaSetDevice(ctx->device));
+  if (!is_device_ptr(y) || !is_device_ptr(out_pred) || (out_phi && !is_device_ptr(out_phi)) ||
+      (out_order && !is_device_ptr(out_order)) || (out_sigma && !is_device_ptr(out_sigma)) ||
+      (out_status && !is_device_ptr(out_status)))
+    return fail(MMF_E_UNSUPPORTED, "mmf_fit_forecast_arima_f32 takes device buffers only");
+  const Plan& pl = ap.diff[diff_order - 1];
+  ArArgs ar{};
+  ar.p = ar_order; ar.phi = out_phi; ar.order = out_order; ar.sigma = out_sigma; ar.nz = pl.d_nz;
+  ArimaArgs ma{};
+  ma.y = y; ma.ld_y = ld_y; ma.t_fit = ap.t_fit; ma.d = diff_order;
+  return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, &ma, stats);
 }
 
 // ---- ragged batches: many calendars, one launch ------------------------------------------------------------------
@@ -1798,8 +1915,8 @@ int mmf_fit_forecast_bcast_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t 
   float* more[MAX_OUT - 1] = {};
   for (int i = 1; i < n_out; ++i) more[i - 1] = reinterpret_cast<float*>(out_ptrs[i]);
   int launches = 0, kernel_used = 0;
-  return run_device(ctx, y, n, ld_y, pred_start, n_pred, reinterpret_cast<float*>(out_ptrs[0]), ld_out, out_beta,
-                    status, ctx->stream, &launches, &kernel_used, more, n_out, multimem);
+  return run_device(ctx, ctx->plan, y, n, ld_y, pred_start, n_pred, reinterpret_cast<float*>(out_ptrs[0]), ld_out,
+                    out_beta, status, ctx->stream, &launches, &kernel_used, more, n_out, multimem);
 }
 
 int mmf_fit_select_forecast_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
@@ -1839,8 +1956,8 @@ int mmf_fit_select_forecast_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t
   sel.out_choice = out_choice;
   sel.out_mse = out_mse;
   int launches = 0, kernel_used = 0;
-  return run_device(ctx, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, nullptr, status, ctx->stream, &launches,
-                    &kernel_used, nullptr, 1, 0, &sel);
+  return run_device(ctx, ctx->plan, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, nullptr, status, ctx->stream,
+                    &launches, &kernel_used, nullptr, 1, 0, &sel);
 }
 
 // ---- device-side packer (pack.cu): every pointer is a device pointer, work is enqueued on the ctx stream

@@ -243,6 +243,20 @@ struct ArSelArgs {
 cudaError_t launch_ar_select(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArSelArgs& sel,
                              cudaStream_t s);
 
+// regression with ARIMA(p, d, 0) errors (arima.cu, DESIGN.md section 2 item 11).  The fit passes and arima_kernel run on
+// the differenced series z' (FitArgs::y, ld_y: the pitched scratch diff_kernel writes) with the plan of D_d;
+// FitArgs::pred_start / n_pred / out / ld_out are the LEVEL rows of the caller's window, which the fit passes ignore
+// (gamma / c hand-off, skip_pred)
+struct ArimaArgs {
+  const float* y;                 // levels [n, ld_y] (row 0 of the slab)
+  int64_t ld_y;
+  int32_t t_fit;                  // level fit rows; z' has t_fit - d
+  int32_t d;                      // 1 .. MMF_DIFF_MAX
+};
+// z'[i, s] = Delta^d y[i, s + d] for s in [0, t_fit - d) (NaN when any of its d + 1 levels is missing), rows of ld_z floats
+cudaError_t launch_diff(const ArimaArgs& ma, float* z, int64_t ld_z, int64_t n, int sm_count, cudaStream_t s);
+cudaError_t launch_arima(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma, cudaStream_t s);
+
 // integer series -> float32 staging rows, sentinel -> NaN (widen.cu); dtype = MMF_DT_I16 / U16 / I32
 cudaError_t launch_widen(int dtype, const void* src, int64_t ld_src, float* dst, int64_t ld_dst, int64_t n, int32_t t,
                          int sm_count, cudaStream_t s);

@@ -218,12 +218,15 @@ class ForecastEngine:
         self._calendar_key = None
 
     def plan_calendar(self, start, t_len: int, freq: str = "D", horizon: int = 28, mode: str = "future",
-                      design: str = "trend_season_exog"):
+                      design: str = "trend_season_exog", max_diff: int | None = None):
         """Build and plan the design for a bucket of series that start at ``start`` and have
         ``t_len`` grid rows.  Returns ``(dates_of_prediction_rows, pred_start, n_pred)``.
         The calendar planned last is remembered: the literal drop-in (one group per call, every group on the same
-        calendar, 02:523-528) whitens and uploads its design once per worker, not once per group."""
-        key = (str(np.datetime64(start, "D")), int(t_len), freq, int(horizon), mode, design)
+        calendar, 02:523-528) whitens and uploads its design once per worker, not once per group.
+        ``max_diff`` (1 .. MMF_DIFF_MAX) also plans the differenced designs of ``fit_forecast_arima`` on the same
+        calendar (``plan_arima``); None leaves the ARIMA plan as it is."""
+        key = (str(np.datetime64(start, "D")), int(t_len), freq, int(horizon), mode, design,
+               None if max_diff is None else int(max_diff))
         if getattr(self, "_calendar_key", None) == key:
             return self._calendar_plan
         if mode == "holdout":                       # reference semantics, 02:372-380 + 484-488
@@ -240,6 +243,8 @@ class ForecastEngine:
             raise ValueError(f"mode must be 'holdout' or 'future', got {mode!r}")
         X = D.design_matrix(days, t_fit, design)
         self.plan(X, t_fit, D.design_has_constant(design))
+        if max_diff is not None:
+            self.plan_arima(X, t_fit, max_diff)
         self._calendar_key = key
         self._calendar_plan = (days[pred_start:pred_start + n_pred], pred_start, n_pred)
         return self._calendar_plan
@@ -517,6 +522,48 @@ class ForecastEngine:
                                                   out.data_ptr(), out.stride(0), phi.data_ptr(), order.data_ptr(),
                                                   sigma.data_ptr(), status.data_ptr(),
                                                   C.byref(st) if st is not None else None))
+        res = {"pred": out, "phi": phi, "order": order, "sigma": sigma, "status": status}
+        if st is not None:
+            self.launches += st.kernel_launches
+            res["stats"] = Stats(st.kernel_ms, st.total_ms, st.n_series, st.n_pending, st.h2d_bytes, st.d2h_bytes,
+                                 st.kernel_launches, {N.KERNEL_WARP: "warp", N.KERNEL_TC: "tc"}.get(st.kernel_used, "?"))
+        return res
+
+    def plan_arima(self, X: np.ndarray, t_fit: int, max_diff: int = 2) -> None:
+        """Plan the differenced designs ``D_d = Delta^d X``, d = 1 .. ``max_diff``, of ``fit_forecast_arima``
+        (``mmf_plan_arima``, DESIGN.md section 2 item 11): a plan of its own beside the one ``plan`` makes."""
+        X = np.ascontiguousarray(X, dtype=np.float64)
+        if X.ndim != 2:
+            raise ValueError("X must be 2-D")
+        N.check(self._lib.mmf_plan_arima(self._h, X.ctypes.data, X.shape[0], X.shape[1], int(t_fit), int(max_diff)))
+        self._arima = (int(t_fit), int(X.shape[0]), int(max_diff))
+
+    def fit_forecast_arima(self, y, ar_order: int, diff_order: int, pred_start: int, n_pred: int,
+                           want_stats: bool = False):
+        """Regression with ARIMA(``ar_order``, ``diff_order``, 0) errors (``mmf_fit_forecast_arima_f32``, DESIGN.md
+        section 2 item 11): ``fit_forecast_ar`` on the differenced series and design, integrated back to levels.
+        ``y`` is a float32 CUDA tensor of levels.  Returns ``{"pred", "phi", "order", "sigma", "status"}`` (torch tensors
+        on y's device): ``pred[i, j]`` the level prediction of design row ``pred_start + j`` (one step ahead in sample,
+        the integrated dynamic forecast from t_fit beyond it, NaN for the first ``diff_order`` rows), ``phi`` / ``order``
+        / ``sigma`` / ``status`` those of the AR part on the differenced series."""
+        import torch
+        if getattr(self, "_arima", None) is None:
+            raise RuntimeError("plan_arima() (or plan_calendar(..., max_diff=d)) must be called first")
+        t_fit = self._arima[0]
+        yp, n, t_have, ld_y = _describe(y, "y")
+        if not (_is_torch(y) and y.is_cuda and y.dtype == torch.float32) or t_have < t_fit:
+            raise ValueError(f"y must be a float32 CUDA tensor with at least t_fit={t_fit} columns")
+        self.set_stream(torch.cuda.current_stream(y.device).cuda_stream)
+        out = torch.empty((n, n_pred), device=y.device, dtype=torch.float32)
+        phi = torch.empty((n, N.AR_MAX), device=y.device, dtype=torch.float32)
+        order = torch.empty(n, device=y.device, dtype=torch.int32)
+        sigma = torch.empty(n, device=y.device, dtype=torch.float32)
+        status = torch.empty(n, device=y.device, dtype=torch.int32)
+        st = N.MmfStats() if want_stats else None
+        N.check(self._lib.mmf_fit_forecast_arima_f32(self._h, yp, n, ld_y, int(ar_order), int(diff_order),
+                                                     int(pred_start), int(n_pred), out.data_ptr(), out.stride(0),
+                                                     phi.data_ptr(), order.data_ptr(), sigma.data_ptr(),
+                                                     status.data_ptr(), C.byref(st) if st is not None else None))
         res = {"pred": out, "phi": phi, "order": order, "sigma": sigma, "status": status}
         if st is not None:
             self.launches += st.kernel_launches

@@ -23,7 +23,7 @@ import pandas as pd
 
 from . import design as D
 from .engine import ForecastEngine, alloc_packed, default_engine
-from ._native import AR_MAX
+from ._native import AR_MAX, DIFF_MAX
 
 FORECAST_HORIZON = 40                      # 02:341
 DEFAULT_KEYS = ("Product", "SKU")          # 02:526
@@ -338,11 +338,12 @@ def _host(x):
     return x.cpu().numpy() if hasattr(x, "cpu") else np.asarray(x)
 
 
-def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, interval=False, ar=None):
+def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, interval=False, ar=None, diff=None):
     """Run the engine over every bucket: yields (bucket, out_days, n_pred, y_host, pred_host, se_host or None).
     ``interval``: prediction standard errors too (``fit_forecast_se``), one call per calendar bucket.
     ``ar``: regression with AR(ar) errors (``fit_forecast_ar``), one call per calendar bucket; a tuple of orders
-    chooses the order per series by hold-out MSE over the last ``horizon`` rows (``fit_select_ar``)."""
+    chooses the order per series by hold-out MSE over the last ``horizon`` rows (``fit_select_ar``).
+    ``diff``: regression with ARIMA(ar, diff, 0) errors (``fit_forecast_arima``), one call per calendar bucket."""
     if interval and select is not None:
         raise ValueError("interval= is not offered with select= (model selection returns point forecasts)")
     t_fit_min = min((b.t_len - (horizon if mode == "holdout" else 0)) for b in buckets) if buckets else 0
@@ -351,9 +352,17 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
         yield from _fit_buckets_ragged(buckets, eng, freq, horizon, mode, design, on_device)
         return
     for b in buckets:
-        out_days, pred_start, n_pred = eng.plan_calendar(b.start, b.t_len, freq, horizon, mode, design)
+        if diff is None:
+            out_days, pred_start, n_pred = eng.plan_calendar(b.start, b.t_len, freq, horizon, mode, design)
+        else:
+            out_days, pred_start, n_pred = eng.plan_calendar(b.start, b.t_len, freq, horizon, mode, design,
+                                                             max_diff=diff)
         se = None
-        if isinstance(ar, tuple):
+        if diff is not None:
+            from .engine import device_packed
+            yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
+            pred = _host(eng.fit_forecast_arima(yd, ar, diff, pred_start, n_pred)["pred"])
+        elif isinstance(ar, tuple):
             from .engine import device_packed
             yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
             pred = _host(eng.fit_select_ar(yd, horizon, ar, pred_start, n_pred)["pred"])
@@ -412,6 +421,19 @@ def _ar_order(ar, select, interval, mode="holdout"):
     if isinstance(ar, bool) or not isinstance(ar, (int, np.integer)) or not 1 <= int(ar) <= AR_MAX:
         raise ValueError(f"ar must be an AR order in [1, {AR_MAX}], got {ar!r}")
     return int(ar)
+
+
+def _diff_order(diff, ar, select, interval):
+    """validated differencing order of ``diff=`` (None: no differencing); ``ar`` must then be one order in 0..8"""
+    if diff is None:
+        return None
+    if select is not None or interval is not None:
+        raise ValueError("diff= is not offered with select= or interval= (ARIMA forecasts come without either)")
+    if isinstance(diff, bool) or not isinstance(diff, (int, np.integer)) or not 1 <= int(diff) <= DIFF_MAX:
+        raise ValueError(f"diff must be a differencing order in [1, {DIFF_MAX}], got {diff!r}")
+    if isinstance(ar, bool) or not isinstance(ar, (int, np.integer)) or not 0 <= int(ar) <= AR_MAX:
+        raise ValueError(f"diff= needs one integer AR order ar in [0, {AR_MAX}], got ar={ar!r}")
+    return int(diff)
 
 
 def _bounds(pred, se, z):
@@ -517,7 +539,7 @@ def _single_group_fast(pdf, keys, date_col, value_col, freq, horizon, mode, desi
 def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Demand",
                     freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                     engine: ForecastEngine | None = None, pack: str = "host", select=None,
-                    null_keys_on_gaps: bool = False, interval=None, ar=None) -> pd.DataFrame:
+                    null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None) -> pd.DataFrame:
     """Fit + forecast every group in ``pdf``; returns ``tuning_schema`` rows
     (keys..., Date, Demand, Demand_Fitted), groups in key order, dates ascending.
 
@@ -550,12 +572,20 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     series' order by the MSE of its dynamic forecast over the last ``horizon`` dates, the held-out rows of
     ``mode='holdout'`` (``ForecastEngine.fit_select_ar``, DESIGN.md section 2 item 10); ``Demand_Fitted`` comes from each
     series' winner.  Holdout mode only.
+
+    ``diff=d`` (1 or 2) with ``ar=p`` (0 <= p <= 8) fits regression with ARIMA(p, d, 0) errors
+    (``ForecastEngine.fit_forecast_arima``, DESIGN.md section 2 item 11): the AR(p) model of the d-times differenced
+    series on the differenced design, integrated back to levels.  ``Demand_Fitted`` holds one-step-ahead level
+    predictions on the fit dates (NaN / null on the first d dates of a group) and the integrated dynamic forecast after
+    them.  The schema is unchanged; every calendar bucket takes its own call.  ``diff=None`` leaves everything as it
+    was; ``diff`` is not offered with ``select=``, ``interval=`` or a tuple of AR orders.
     """
     eng = engine or default_engine()
     keys = list(keys)
     fitted_col = value_col + "_Fitted"
     z = _z_of(interval)
-    ar = _ar_order(ar, select, interval, mode)
+    diff = _diff_order(diff, ar, select, interval)
+    ar = int(ar) if diff is not None else _ar_order(ar, select, interval, mode)
     if pack == "host" and select is None and z is None and ar is None and isinstance(pdf, pd.DataFrame):
         one = _single_group_fast(pdf, keys, date_col, value_col, freq, horizon, mode, design, eng, null_keys_on_gaps)
         if one is not None:
@@ -563,7 +593,7 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     buckets = _buckets_for(pdf, keys, date_col, value_col, freq, pack, eng)
     parts, lengths = [], []
     for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
-                                                              pack == "device", z is not None, ar):
+                                                              pack == "device", z is not None, ar, diff):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n), n_pred)
         # key columns keep the dtype they came in with (no per-row string inference on N x T values)
@@ -654,13 +684,13 @@ def backtest_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
 def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Demand",
                    freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                    engine: ForecastEngine | None = None, pack: str = "host", select=None,
-                   null_keys_on_gaps: bool = False, interval=None, ar=None):
+                   null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None):
     """Arrow ``Table``/``RecordBatch`` in -> Arrow ``Table`` with ``tuning_schema`` out (the ``mapInArrow``
     flavour of the boundary).  No pandas frame of the rows on either side: keys are dictionary-encoded on the way
     in and expanded from a dictionary on the way out, dates and values are NumPy views of Arrow buffers.
     ``interval=level`` adds the ``{value}_Lower`` / ``{value}_Upper`` columns of ``forecast_groups`` (schema:
     ``tuning_schema(..., interval=True)``).  ``ar=p`` fits regression with AR(p) errors and ``ar=(0, 1, 2, 3, 4)`` chooses the order per series, as in
-    ``forecast_groups``."""
+    ``forecast_groups``; ``diff=d`` with ``ar=p`` fits ARIMA(p, d, 0) errors as there."""
     import pyarrow as pa
 
     if isinstance(table, pa.RecordBatch):
@@ -668,12 +698,13 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     eng = engine or default_engine()
     keys = list(keys)
     z = _z_of(interval)
-    ar = _ar_order(ar, select, interval, mode)
+    diff = _diff_order(diff, ar, select, interval)
+    ar = int(ar) if diff is not None else _ar_order(ar, select, interval, mode)
     schema = tuning_schema(keys, date_col, value_col, interval=z is not None)
     buckets = _buckets_for(table, keys, date_col, value_col, freq, pack, eng)
     parts, lengths = [], []
     for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
-                                                              pack == "device", z is not None, ar):
+                                                              pack == "device", z is not None, ar, diff):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n, dtype=np.int32), n_pred)
         cols = []

@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define MMF_VERSION 106          /* 0.1.6 */
+#define MMF_VERSION 107          /* 0.1.7 */
 #define MMF_P 16                 /* design columns (zero-pad narrower designs) */
 #define MMF_PIVOT_TOL 1e-3f      /* per-series relative Cholesky pivot threshold */
 #define MMF_CAL_TOL 1e-10        /* aliasing threshold on the float64 calendar Gram */
@@ -41,6 +41,7 @@ extern "C" {
 #define MMF_AR_MAX 8             /* largest AR order of mmf_fit_forecast_ar_f32 */
 #define MMF_AR_KAPPA_MAX 0.999   /* Levinson-Durbin stops before a partial autocorrelation |kappa| >= this */
 #define MMF_ARSEL_MAX_CAND 9     /* candidate AR orders per mmf_fit_select_ar_f32 call (0 .. MMF_AR_MAX) */
+#define MMF_DIFF_MAX 2           /* largest differencing order of mmf_fit_forecast_arima_f32 */
 
 /* return codes */
 #define MMF_OK 0
@@ -239,6 +240,38 @@ int mmf_fit_select_ar_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y,
                           int32_t* out_choice, float* out_mse, float* out_cand_mse,
                           float* out_phi, int32_t* out_order, float* out_sigma,
                           int32_t* out_status, mmf_stats* stats);
+
+/* ---- regression with ARIMA(p, d, 0) errors (DESIGN.md section 2 item 11) ----------------------------------------------
+ * mmf_plan_arima: X [n_rows, p] float64 as for mmf_plan_design, 1 <= max_diff <= MMF_DIFF_MAX, t_fit - max_diff >= 1.
+ * For d = 1 .. max_diff it plans the differenced design D_d, row s = Delta^d x_{s+d} (float64, s in [0, n_rows - d)), as
+ * mmf_plan_design(D_d, n_rows - d, p, t_fit - d, has_constant = 0) would: a differenced column whose largest |value| on
+ * the fit rows is at most 1e-12 x the largest |value| of the raw column there is set to 0 first (cancellation residue).
+ * A plan of its own: the mmf_plan_design, mmf_plan_calendars and mmf_plan_backtest plans stay in force.  Every argument
+ * is checked before the previous ARIMA plan is freed, so a refused plan keeps it.
+ * mmf_fit_forecast_arima_f32: for series i and d = diff_order (1 <= d <= the planned max_diff), 0 <= ar_order <= MMF_AR_MAX:
+ *   z_t = y_t - y_{t-1} (d = 1) or (y_t - y_{t-1}) - (y_{t-1} - y_{t-2}) (d = 2) in that fp32 order, for d <= t < t_fit,
+ *   missing when any of y_{t-d} .. y_t is; z'_s = z_{s+d};
+ *   zhat_t: mmf_fit_forecast_ar_f32(ar_order) on z' with the plan D_d (ar_order = 0: the plain fit, phi 0, sigma =
+ *   sqrt(r_0)), the prediction of z'_{t-d}: one step ahead in sample, the dynamic forecast from t_fit beyond it;
+ *   levels: ytilde_s = y_s for s < t_fit with y_s finite, else yhat_s (NaN for s < d);
+ *   yhat_t = zhat_t + ytilde_{t-1} (d = 1), yhat_t = (zhat_t + 2 ytilde_{t-1}) - ytilde_{t-2} (d = 2), each sum rounded
+ *   once in fp32 in that order (2 ytilde_{t-1} is exact); yhat_t = NaN for t < d.
+ * out_pred[i, t - pred_start] = yhat_t for the rows [pred_start, pred_start + n_pred) of the planned design: one step
+ * ahead in sample, the integrated dynamic forecast beyond t_fit.  y is read on [0, t_fit) only.  A missing fit value
+ * is replaced by its prediction, so later rows integrate from the filled level; a missing value before the first
+ * observed one makes the predictions NaN until an observed level restarts the chain.
+ * out_phi [n][MMF_AR_MAX], out_order [n], out_sigma [n] are those of the AR part on z'; out_status [n] is the status of
+ * the fit on z' (1 when z' has no observed fit row: NaN predictions, order 0, phi 0, sigma NaN).  All nullable except
+ * out_pred.  Otherwise the contract of mmf_fit_forecast_ar_f32: device buffers only, any ld_out >= n_pred and any base
+ * pointer with only columns [0, n_pred) written, enqueue-only unless `stats` is non-NULL, mmf_config.kernel and
+ * assume_finite honoured, refused arguments write nothing.  Scratch: one slab of rows x round4(t_fit - d) floats for z'.
+ * replaces: SARIMAX(p, d, 0) + exog fit and predict of the reference's per-group model (02:441-450, 472-488 with d > 0),
+ * for caller-fixed orders and the two-step estimator on the differenced series. */
+int mmf_plan_arima(mmf_ctx* ctx, const double* X, int32_t n_rows, int32_t p, int32_t t_fit, int32_t max_diff);
+int mmf_fit_forecast_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
+                               int32_t diff_order, int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out,
+                               float* out_phi, int32_t* out_order, float* out_sigma, int32_t* out_status,
+                               mmf_stats* stats);
 
 /* ---- ragged batches: groups on MANY calendars in one launch ---------------------------------------------
  * The reference re-indexes every group on its own calendar (sort_values + asfreq per group, 02:422-423), so one

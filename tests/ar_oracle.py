@@ -155,6 +155,76 @@ def coef_bounds(res, tau_fit):
             2.0 * dsig + 4 * FP32_EPS * np.nan_to_num(res["sigma"]))
 
 
+DEGENERATE_TAU = 4.0
+
+
+def degenerate_rows(res, tau_fit):
+    """Rows where the first-order bounds (coef_bounds, ar_bound) do not apply: the oracle's RMS residual sqrt(r_0) is at
+    most DEGENERATE_TAU x tau_fit, so |dr_k| <= 2 tau_fit sqrt(r_0) is not small next to r_0 (it is >= r_0 / 2).  This is
+    a series the regression fits to rounding level -- all zero, constant, an exact line or level plus weekly pattern in
+    the design's span: the GPU's residuals are fp32 noise of size ~tau_fit, the oracle's float64 noise, and the two run
+    Levinson-Durbin on unrelated noise.  Status-1 rows are never degenerate."""
+    return (np.asarray(res["status"]) != 1) & (np.sqrt(np.maximum(res["r"][:, 0], 0.0)) <= DEGENERATE_TAU * tau_fit)
+
+
+def impulse(phi, length: int):
+    """c [n, length, AR_MAX]: inside a dynamic stretch of the recursion u_s = sum_j phi_j u_{s-j} entered at position a,
+    u_{a+h} = sum_k c[:, h, k-1] u_{a-k} (k = 1..AR_MAX).  Signed, so for a stable phi it decays with h."""
+    phi = np.asarray(phi, dtype=np.float64)
+    n = phi.shape[0]
+    c = np.zeros((n, length, AR_MAX))
+    for h in range(length):
+        acc = np.zeros((n, AR_MAX))
+        if h < AR_MAX:
+            acc[:, :AR_MAX - h] = phi[:, h:]                        # phi_{h+k}: a state value reached directly
+        for j in range(1, min(h, AR_MAX) + 1):
+            acc += phi[:, j - 1:j] * c[:, h - j]
+        c[:, h] = acc
+    return c
+
+
+def _ar_magnitude(phi, obs, e_max, t_fit: int, pred_start: int, n_pred: int):
+    """bound on |AR part| of every requested row when every observed fit residual is at most e_max.  B_s bounds |u_s|:
+    e_max on an observed fit row; in a stretch of unobserved rows entered at a, sum_k |c_{s-a,k}| B_{a-k} with c the
+    signed impulse coefficients of phi (u before row 0 is 0).  The AR part is u_s itself on an unobserved row and
+    sum_j phi_j u_{s-j} (<= sum_j |phi_j| B_{s-j}, one step) on an observed one."""
+    phi = np.asarray(phi, dtype=np.float64)
+    n = phi.shape[0]
+    end = pred_start + n_pred
+    aphi = np.abs(phi)
+    c = np.abs(impulse(phi, max(end, 1)))
+    B = np.zeros((n, end + AR_MAX))                                  # B[:, AR_MAX + s]; columns < AR_MAX are s < 0
+    rows = np.arange(n)
+    lag = np.arange(1, AR_MAX + 1)
+    entry = np.zeros(n, dtype=np.int64)
+    out = np.zeros((n, n_pred))
+    for s in range(end):
+        if 0 < s <= t_fit:
+            entry = np.where(obs[:, s - 1], s, entry)
+        o = obs[:, s] if s < t_fit else np.zeros(n, dtype=bool)
+        state = B[rows[:, None], AR_MAX + entry[:, None] - lag[None, :]]
+        dyn = (c[rows, s - entry] * state).sum(axis=1)
+        one = (aphi * B[:, AR_MAX + s - lag]).sum(axis=1)
+        B[:, AR_MAX + s] = np.where(o, e_max, dyn)
+        if s >= pred_start:
+            out[:, s - pred_start] = np.where(o, one, dyn)
+    return out
+
+
+def degenerate_bound(res, phi_gpu, tau_fit, tau_pred, t_fit: int, pred_start: int, n_pred: int):
+    """Bound on |pred_gpu - pred_oracle| per element that holds on every row, degenerate ones included (DESIGN.md
+    section 6): the fitted values differ by at most tau_pred; each side's AR part is at most what its own phi -- through
+    the signed impulse coefficients, which decay for a stable phi -- makes of residuals of at most max|e_oracle|
+    (+ tau_fit on the GPU's side, whose residuals carry its fitted-value error).  No first-order term: it does not need
+    r_0 to be large next to tau.  Returned x 2, plus fp32 rounding."""
+    obs = res["obs"]
+    e_max = np.abs(res["e"]).max(axis=1)
+    a_gpu = _ar_magnitude(phi_gpu, obs, e_max + tau_fit, t_fit, pred_start, n_pred)
+    a_orc = _ar_magnitude(res["phi"], obs, e_max, t_fit, pred_start, n_pred)
+    rnd = 16 * FP32_EPS * np.nan_to_num(np.abs(res["pred"]))
+    return 2.0 * (tau_pred[:, None] + a_gpu + a_orc + rnd)
+
+
 def ar_bound(res, tau_fit, tau_pred, t_fit: int, pred_start: int, n_pred: int):
     """First-order bound on |pred_gpu - pred_oracle| per element (DESIGN.md section 6).
     tau_fit[i]: bound on the error of a plain fitted value on the fit rows (the parity tolerance x mask factor);

@@ -13,7 +13,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from ar_oracle import AR_MAX, FP32_EPS, ar_bound, fit_forecast_ar_packed
+from ar_oracle import AR_MAX, FP32_EPS, ar_bound, degenerate_bound, fit_forecast_ar_packed
 from oracle import mmf_oracle as O
 
 
@@ -84,16 +84,20 @@ def select_ar_packed(y, X, t_fit: int, n_hold: int, orders, pred_start: int, n_p
                 status=status, hold=hold, idx=idx, final=final)
 
 
-def mse_bound(sel, y, tau_fit, tau_hold, t_fit: int, n_hold: int, orders):
+def mse_bound(sel, y, tau_fit, tau_hold, t_fit: int, n_hold: int, orders, phi_gpu=None):
     """First-order bound on |MSE_gpu - MSE_oracle| per series and candidate [n, k] (DESIGN.md section 6):
       |dMSE_m| <= (1/N) sum_s (2 |e_s| b_s + b_s^2) + 2 eps |MSE_m|   (float32 storage)
     e_s = y_s - the oracle's forecast, b_s = ar_bound of candidate m on the held-out rows (candidate 0: tau_hold, the
-    plain tolerance x the leverage of the held-out rows), N the scored points.  tau_fit / tau_hold are per series."""
+    plain tolerance x the leverage of the held-out rows), N the scored points.  tau_fit / tau_hold are per series.
+    With phi_gpu (one [n, AR_MAX] array per candidate: the GPU's coefficients of candidate m), b_s is
+    ar_oracle.degenerate_bound instead, which also holds on degenerate rows."""
     y_hold = np.asarray(y, dtype=np.float64)[:, t_fit:t_fit + n_hold]
     out = np.zeros(sel["cand_mse"].shape)
     for j, m in enumerate(orders):
         h = sel["hold"][j]
-        if m >= 1:
+        if m >= 1 and phi_gpu is not None:
+            b = degenerate_bound(h, phi_gpu[j], tau_fit, tau_hold, t_fit, t_fit, n_hold)
+        elif m >= 1:
             b = ar_bound(h, tau_fit, tau_hold, t_fit, t_fit, n_hold)
         else:
             b = np.repeat(np.asarray(tau_hold, dtype=np.float64)[:, None], n_hold, axis=1)

@@ -96,6 +96,8 @@ struct Plan {
   float* d_ap_hi = nullptr;   // [n_rows][P] tf32-hi / tf32-lo of A: B operand of predict_tc_kernel
   float* d_ap_lo = nullptr;
   uint32_t* d_nz = nullptr;    // [n_rows] non-zero masks of the whitened rows (AR calls: the used columns of the dof rule)
+  int32_t x_cols = 0;          // mmf_plan_design: columns and 64-bit hash of the raw X (host side; a (p, d) selection
+  uint64_t x_hash = 0;         // refuses an ARIMA plan built from another X)
   float* d_sfac = nullptr;    // [n_rows] sqrt(1 + |a_t|^2) (float64 on the host): se of gap-free rows / sigma
   alignas(64) unsigned char tmap_at[128];
   alignas(64) unsigned char tmap_bhi[128];
@@ -149,6 +151,8 @@ struct BtPlan {
 struct ArimaPlan {
   bool valid = false;
   int32_t max_diff = 0, n_rows = 0, t_fit = 0;
+  int32_t x_cols = 0;                  // columns and 64-bit hash of the raw X the designs were differenced from
+  uint64_t x_hash = 0;
   Plan diff[MMF_DIFF_MAX];
 };
 
@@ -212,6 +216,8 @@ struct mmf_ctx {
   BtPlan bt;
   ArimaPlan arima;
   float* d_z = nullptr;  size_t z_cap_bytes = 0;           // ARIMA calls: z' of one slab, round4(t_fit - d) per row
+  ArimaSelBest* d_asel_best = nullptr;  size_t asel_best_cap = 0;   // (p, d) selection, per slab: running best,
+  int32_t* d_asel_status = nullptr;  size_t asel_status_cap = 0;    // and the status of the fit of the current d
   float* d_bt_mom = nullptr;  size_t bt_mom_cap = 0;   // backtest scratch, per slab: moments at the earlier origins,
   SolveRec* d_bt_recs = nullptr;  size_t bt_recs_cap = 0;   // [K][slab] records, [K][slab] work lists,
   int64_t* d_bt_rows = nullptr;  size_t bt_rows_cap = 0;
@@ -263,6 +269,14 @@ int grow(void** ptr, size_t* cap, size_t need) {
   if (e != cudaSuccess) return fail(MMF_E_NOMEM, "cudaMalloc(%zu) failed: %s", need, cudaGetErrorString(e));
   *cap = need;
   return MMF_OK;
+}
+
+// FNV-1a over the bytes of a planned X: plans built from the same X carry the same hash
+uint64_t hash_x(const double* X, int64_t count) {
+  const unsigned char* b = reinterpret_cast<const unsigned char*>(X);
+  uint64_t h = 14695981039346656037ull;
+  for (int64_t i = 0; i < count * (int64_t)sizeof(double); ++i) h = (h ^ b[i]) * 1099511628211ull;
+  return h;
 }
 
 bool is_device_ptr(const void* p) {
@@ -502,17 +516,22 @@ int build_multi(MultiPlan& m, const double* X_all, int32_t n_cal, const int32_t*
 
 // Enqueue the fit of ONE slab of device-resident rows on `s`.  status must be non-null.
 // ARIMA calls (arima != nullptr, with ar): y / ld_y are the slab's levels; diff_kernel writes z' into the context's
-// scratch first, and the fit passes and arima_kernel read z' with `plan` = the plan of D_d.
+// scratch first, and the fit passes and arima_kernel read z' with `plan` = the plan of D_d.  (p, d) selection calls
+// (asel != nullptr) run this once per listed d and end in arima_select_kernel; their d = 0 pass (arima->d == 0) fits y
+// itself with the mmf_plan_design plan.
 int run_device_slab(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, int64_t ld_y, int32_t pred_start,
                     int32_t n_pred, float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s,
                     int* launches, int* kernel_used, float* const* out_more, int n_out, int multimem,
                     const SelectArgs* sel, const SeArgs* se = nullptr, const ArArgs* ar = nullptr,
-                    const ArSelArgs* arsel = nullptr, const ArimaArgs* arima = nullptr) {
+                    const ArSelArgs* arsel = nullptr, const ArimaArgs* arima = nullptr,
+                    const ArimaSelArgs* asel = nullptr) {
   const DesignView d = view_of(plan);
   ArimaArgs ma{};
   if (arima != nullptr) {
     ma = *arima;
     ma.y = y;
+  }
+  if (arima != nullptr && ma.d > 0) {
     const int64_t ld_z = (plan.t_fit + 3) & ~3;              // 16-B row pitch: fit_tc's TMA path
     int rc = grow((void**)&ctx->d_z, &ctx->z_cap_bytes, (size_t)n * ld_z * sizeof(float));
     if (rc != MMF_OK) return rc;
@@ -611,8 +630,9 @@ int run_device_slab(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, i
     ++*launches;
   }
   if (ar != nullptr) {
-    CU_TRY(arima != nullptr ? launch_arima(d, a, *ar, ma, s)
-                            : arsel != nullptr ? launch_ar_select(d, a, *ar, *arsel, s) : launch_ar(d, a, *ar, s));
+    CU_TRY(asel != nullptr    ? launch_arima_select(d, a, *ar, ma, *asel, s)
+           : arima != nullptr ? launch_arima(d, a, *ar, ma, s)
+           : arsel != nullptr ? launch_ar_select(d, a, *ar, *arsel, s) : launch_ar(d, a, *ar, s));
     ++*launches;
   }
   if (many_pred) {
@@ -805,6 +825,7 @@ int mmf_destroy(mmf_ctx* ctx) {
   free_bt(ctx->bt);
   free_arima(ctx->arima);
   cudaFree(ctx->d_z);
+  cudaFree(ctx->d_asel_best); cudaFree(ctx->d_asel_status);
   cudaFree(ctx->d_bt_mom); cudaFree(ctx->d_bt_recs); cudaFree(ctx->d_bt_rows); cudaFree(ctx->d_bt_ctr); cudaFree(ctx->d_bt_pred);
   for (int i = 0; i < NBUF; ++i) {
     Staging& s = ctx->st[i];
@@ -893,7 +914,12 @@ int mmf_plan_design(mmf_ctx* ctx, const double* X, int32_t n_rows, int32_t p, in
   CU_TRY(cudaSetDevice(ctx->device));
   CU_TRY(cudaStreamSynchronize(ctx->stream));
   free_plan(ctx->plan);
-  return build_plan(ctx->plan, X, n_rows, p, t_fit, has_constant);
+  const int rc = build_plan(ctx->plan, X, n_rows, p, t_fit, has_constant);
+  if (rc == MMF_OK) {
+    ctx->plan.x_cols = p;
+    ctx->plan.x_hash = hash_x(X, (int64_t)n_rows * p);
+  }
+  return rc;
 }
 
 int mmf_pin_scratch(mmf_ctx* ctx, int32_t delta) {
@@ -1426,6 +1452,8 @@ int mmf_plan_arima(mmf_ctx* ctx, const double* X, int32_t n_rows, int32_t p, int
   ctx->arima.max_diff = max_diff;
   ctx->arima.n_rows = n_rows;
   ctx->arima.t_fit = t_fit;
+  ctx->arima.x_cols = p;
+  ctx->arima.x_hash = hash_x(X, (int64_t)n_rows * p);
   ctx->arima.valid = true;
   return MMF_OK;
 }
@@ -1461,6 +1489,134 @@ int mmf_fit_forecast_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t 
   ArimaArgs ma{};
   ma.y = y; ma.ld_y = ld_y; ma.t_fit = ap.t_fit; ma.d = diff_order;
   return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, &ma, stats);
+}
+
+// ---- (p, d) selection by hold-out MSE on levels (DESIGN.md section 2 item 12) -------------------------------------------
+int mmf_fit_select_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
+                             const int32_t* orders, int32_t n_orders, const int32_t* diffs, int32_t n_diffs,
+                             int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out,
+                             int32_t* out_choice_p, int32_t* out_choice_d, float* out_mse, float* out_cand_mse,
+                             float* out_phi, int32_t* out_order, float* out_sigma, int32_t* out_status,
+                             mmf_stats* stats) {
+  if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
+  GrowScope grow_scope(ctx);
+  if (n < 0) return fail(MMF_E_INVALID, "n < 0");
+  if (n > 0 && (!y || !out_pred)) return fail(MMF_E_INVALID, "y or out_pred is NULL");
+  if (!orders || n_orders < 1 || n_orders > MMF_ARSEL_MAX_CAND)
+    return fail(MMF_E_INVALID, "n_orders=%d outside [1,%d] (or orders is NULL)", n_orders, MMF_ARSEL_MAX_CAND);
+  for (int j = 0; j < n_orders; ++j)
+    if (orders[j] < 0 || orders[j] > MMF_AR_MAX || (j > 0 && orders[j] <= orders[j - 1]))
+      return fail(MMF_E_INVALID, "orders must be ascending and distinct in [0,%d] (orders[%d]=%d)", MMF_AR_MAX, j,
+                  orders[j]);
+  if (!diffs || n_diffs < 1 || n_diffs > MMF_DIFF_MAX + 1)
+    return fail(MMF_E_INVALID, "n_diffs=%d outside [1,%d] (or diffs is NULL)", n_diffs, MMF_DIFF_MAX + 1);
+  for (int j = 0; j < n_diffs; ++j)
+    if (diffs[j] < 0 || diffs[j] > MMF_DIFF_MAX || (j > 0 && diffs[j] <= diffs[j - 1]))
+      return fail(MMF_E_INVALID, "diffs must be ascending and distinct in [0,%d] (diffs[%d]=%d)", MMF_DIFF_MAX, j,
+                  diffs[j]);
+  // a listed d = 0 fits y with the mmf_plan_design plan; a listed d >= 1 fits z' with the mmf_plan_arima plan
+  const bool use_plain = diffs[0] == 0, use_arima = diffs[n_diffs - 1] >= 1;
+  const Plan& pl = ctx->plan;
+  const ArimaPlan& ap = ctx->arima;
+  if (use_plain && !pl.valid) return fail(MMF_E_NOPLAN, "diffs lists 0 and mmf_plan_design has not been called");
+  if (use_arima && !ap.valid) return fail(MMF_E_NOPLAN, "diffs lists d >= 1 and mmf_plan_arima has not been called");
+  if (use_arima && diffs[n_diffs - 1] > ap.max_diff)
+    return fail(MMF_E_INVALID, "diffs lists d=%d above the planned max_diff=%d", diffs[n_diffs - 1], ap.max_diff);
+  if (use_plain && use_arima &&
+      (pl.n_rows != ap.n_rows || pl.t_fit != ap.t_fit || pl.x_cols != ap.x_cols || pl.x_hash != ap.x_hash))
+    return fail(MMF_E_INVALID, "the mmf_plan_design and mmf_plan_arima plans were built from different designs "
+                "(rows %d / %d, t_fit %d / %d, columns %d / %d)", pl.n_rows, ap.n_rows, pl.t_fit, ap.t_fit, pl.x_cols,
+                ap.x_cols);
+  const int32_t T = use_plain ? pl.t_fit : ap.t_fit;
+  const int32_t n_rows = use_plain ? pl.n_rows : ap.n_rows;
+  if (n_hold < 1 || (int64_t)T + n_hold > n_rows)
+    return fail(MMF_E_INVALID, "held-out rows [%d,%lld) outside the planned design (%d rows)", T, (long long)T + n_hold,
+                n_rows);
+  if (ld_y < (int64_t)T + n_hold)
+    return fail(MMF_E_INVALID, "ld_y=%lld < t_fit + n_hold=%lld", (long long)ld_y, (long long)T + n_hold);
+  if (n_pred < 1 || pred_start < 0 || (int64_t)pred_start + n_pred > n_rows)
+    return fail(MMF_E_INVALID, "prediction rows [%d,%d) outside the planned design (%d rows)", pred_start,
+                pred_start + n_pred, n_rows);
+  if (ld_out < n_pred) return fail(MMF_E_INVALID, "ld_out=%lld < n_pred=%d", (long long)ld_out, n_pred);
+  if (stats) memset(stats, 0, sizeof(*stats));
+  if (n == 0) return MMF_OK;
+  CU_TRY(cudaSetDevice(ctx->device));
+  if (!is_device_ptr(y) || !is_device_ptr(out_pred) || (out_choice_p && !is_device_ptr(out_choice_p)) ||
+      (out_choice_d && !is_device_ptr(out_choice_d)) || (out_mse && !is_device_ptr(out_mse)) ||
+      (out_cand_mse && !is_device_ptr(out_cand_mse)) || (out_phi && !is_device_ptr(out_phi)) ||
+      (out_order && !is_device_ptr(out_order)) || (out_sigma && !is_device_ptr(out_sigma)) ||
+      (out_status && !is_device_ptr(out_status)))
+    return fail(MMF_E_UNSUPPORTED, "mmf_fit_select_arima_f32 takes device buffers only");
+
+  // slabs as the plain fit of the level rows would cut them; per slab, one fit and one arima_select_kernel per listed d
+  const Plan& level_plan = use_plain ? pl : ap.diff[0];
+  const int64_t slab = slab_rows(level_plan, n);
+  const int64_t n_slabs = (n + slab - 1) / slab;
+  int rc = grow((void**)&ctx->d_asel_best, &ctx->asel_best_cap, (size_t)slab * sizeof(ArimaSelBest));
+  if (rc == MMF_OK) rc = grow((void**)&ctx->d_asel_status, &ctx->asel_status_cap, (size_t)slab * sizeof(int32_t));
+  if (rc != MMF_OK) return rc;
+  uint32_t* slab_pending = nullptr;        // rows each fit handed to the general pass (stats)
+  if (stats) {
+    const mmf_ctx* saved = g_grow_ctx;
+    g_grow_ctx = nullptr;
+    rc = grow((void**)&ctx->d_slab_pending, &ctx->slab_pending_cap, (size_t)(n_slabs * n_diffs) * sizeof(uint32_t));
+    g_grow_ctx = saved;
+    if (rc != MMF_OK) return rc;
+    slab_pending = ctx->d_slab_pending;
+  }
+  const cudaStream_t s = ctx->stream;
+  int launches = 0, kernel_used = 0;
+  if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, s));
+  for (int64_t off = 0, i = 0; off < n; off += slab, ++i) {
+    const int64_t m = std::min(slab, n - off);
+    for (int k = 0; k < n_diffs; ++k) {
+      const int dd = diffs[k];
+      const Plan& plan = dd == 0 ? pl : ap.diff[dd - 1];
+      ArArgs ar{};
+      ar.p = orders[n_orders - 1];
+      ar.phi = out_phi ? out_phi + off * MMF_AR_MAX : nullptr;
+      ar.order = out_order ? out_order + off : nullptr;
+      ar.sigma = out_sigma ? out_sigma + off : nullptr;
+      ar.nz = plan.d_nz;
+      ArimaArgs ma{};
+      ma.ld_y = ld_y; ma.t_fit = T; ma.d = dd;
+      ArimaSelArgs sel{};
+      sel.n_hold = n_hold; sel.n_cand = n_orders;
+      for (int j = 0; j < n_orders; ++j) sel.cand[j] = orders[j];
+      sel.d_index = k; sel.n_diffs = n_diffs;
+      sel.best = ctx->d_asel_best;
+      sel.choice_p = out_choice_p ? out_choice_p + off : nullptr;
+      sel.choice_d = out_choice_d ? out_choice_d + off : nullptr;
+      sel.mse = out_mse ? out_mse + off : nullptr;
+      sel.cand_mse = out_cand_mse ? out_cand_mse + off * n_diffs * n_orders : nullptr;
+      sel.status = out_status ? out_status + off : nullptr;
+      rc = run_device_slab(ctx, plan, y + off * ld_y, m, ld_y, pred_start, n_pred, out_pred + off * ld_out, ld_out,
+                           nullptr, ctx->d_asel_status, s, &launches, &kernel_used, nullptr, 1, 0, nullptr, nullptr,
+                           &ar, nullptr, &ma, &sel);
+      if (rc != MMF_OK) return rc;
+      if (slab_pending != nullptr) {
+        uint32_t* dst = slab_pending + i * n_diffs + k;
+        if (kernel_used == MMF_KERNEL_TC)
+          CU_TRY(cudaMemcpyAsync(dst, ctx->d_pending + CTR_WORDS * ctx->last_set, sizeof(uint32_t),
+                                 cudaMemcpyDeviceToDevice, s));
+        else
+          CU_TRY(cudaMemsetAsync(dst, 0, sizeof(uint32_t), s));
+      }
+    }
+  }
+  if (stats) {
+    CU_TRY(cudaEventRecord(ctx->ev_k1, s));
+    CU_TRY(cudaEventSynchronize(ctx->ev_k1));
+    CU_TRY(cudaEventElapsedTime(&stats->kernel_ms, ctx->ev_k0, ctx->ev_k1));
+    stats->total_ms = stats->kernel_ms;
+    std::vector<uint32_t> pend((size_t)(n_slabs * n_diffs), 0u);
+    CU_TRY(cudaMemcpy(pend.data(), slab_pending, pend.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    for (uint32_t v : pend) stats->n_pending += v;
+    stats->n_series = n;
+    stats->kernel_launches = launches;
+    stats->kernel_used = kernel_used;
+  }
+  return MMF_OK;
 }
 
 // ---- ragged batches: many calendars, one launch ------------------------------------------------------------------

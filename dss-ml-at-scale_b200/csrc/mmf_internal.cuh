@@ -251,11 +251,37 @@ struct ArimaArgs {
   const float* y;                 // levels [n, ld_y] (row 0 of the slab)
   int64_t ld_y;
   int32_t t_fit;                  // level fit rows; z' has t_fit - d
-  int32_t d;                      // 1 .. MMF_DIFF_MAX
+  int32_t d;                      // 1 .. MMF_DIFF_MAX (selection calls: 0 for the candidates on y itself)
 };
 // z'[i, s] = Delta^d y[i, s + d] for s in [0, t_fit - d) (NaN when any of its d + 1 levels is missing), rows of ld_z floats
 cudaError_t launch_diff(const ArimaArgs& ma, float* z, int64_t ld_z, int64_t n, int sm_count, cudaStream_t s);
 cudaError_t launch_arima(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma, cudaStream_t s);
+
+// per-series (p, d) selection by hold-out MSE on levels (arima.cu, DESIGN.md section 2 item 12): one launch per listed d,
+// in list order, behind that d's fit (on y for d = 0, ArimaArgs::d = 0; on z' otherwise).  Each launch scores its d's
+// candidates and compares its first minimum with the running best the earlier d's left in `best`.
+struct ArimaSelBest {                     // one row's running best over the d's launched so far (16 B)
+  double mse;                             // float64 hold-out MSE of the leader (valid when flags & SCORED)
+  int16_t p, d;                           // the leader
+  int32_t flags;                          // ARIMASEL_SCORED: some eligible candidate scored a point; ARIMASEL_ELIGIBLE
+};
+static_assert(sizeof(ArimaSelBest) == 16, "ArimaSelBest is one 16-B record");
+constexpr int32_t ARIMASEL_SCORED = 1, ARIMASEL_ELIGIBLE = 2;
+struct ArimaSelArgs {
+  int32_t n_hold;                         // held-out level rows [t_fit, t_fit + n_hold)
+  int32_t n_cand;                         // orders: 1 .. MMF_ARSEL_MAX_CAND
+  int32_t cand[MMF_ARSEL_MAX_CAND];       // ascending distinct orders in [0, MMF_AR_MAX], last == ArArgs::p
+  int32_t d_index;                        // position of this d in the call's list; 0 writes every output of every row
+  int32_t n_diffs;
+  ArimaSelBest* best;                     // [n] running best (scratch)
+  int32_t* choice_p;                      // nullable [n]: the chosen order (-1: no eligible candidate)
+  int32_t* choice_d;                      // nullable [n]: the chosen d (-1 likewise)
+  float* mse;                             // nullable [n]: the winner's hold-out MSE
+  float* cand_mse;                        // nullable [n][n_diffs][n_cand]
+  int32_t* status;                        // nullable [n]: the winner's fit status (FitArgs::status is this d's scratch)
+};
+cudaError_t launch_arima_select(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
+                                const ArimaSelArgs& sel, cudaStream_t s);
 
 // integer series -> float32 staging rows, sentinel -> NaN (widen.cu); dtype = MMF_DT_I16 / U16 / I32
 cudaError_t launch_widen(int dtype, const void* src, int64_t ld_src, float* dst, int64_t ld_dst, int64_t n, int32_t t,

@@ -617,6 +617,65 @@ class ForecastEngine:
                                  st.kernel_launches, {N.KERNEL_WARP: "warp", N.KERNEL_TC: "tc"}.get(st.kernel_used, "?"))
         return res
 
+    def fit_select_arima(self, y, n_hold: int, orders=(0, 1, 2, 3, 4), diffs=(0, 1, 2), pred_start: int = 0,
+                         n_pred: int | None = None, want_stats: bool = False):
+        """Regression with ARIMA(p, d, 0) errors, (p, d) chosen per series by hold-out MSE on levels
+        (``mmf_fit_select_arima_f32``, DESIGN.md section 2 item 12).  The candidates are every pair of ``orders``
+        (ascending, distinct, 0 .. MMF_AR_MAX) and ``diffs`` (ascending, distinct, 0 .. MMF_DIFF_MAX), d-major: (p, 0)
+        is ``fit_select_ar``'s candidate p, (p, d >= 1) is ``fit_forecast_arima(p, d)``.  Each is scored by the MSE of
+        its dynamic level forecast from t_fit over the held-out rows [t_fit, t_fit + n_hold); the first minimum wins.
+        A listed d = 0 needs ``plan``'s design, a listed d >= 1 ``plan_arima``'s of the same X (``plan_calendar(...,
+        max_diff=)`` plans both).  ``y`` is a float32 CUDA tensor with at least t_fit + n_hold columns; ``n_pred``
+        defaults to every design row from ``pred_start`` on.  Returns ``{"pred", "choice_p", "choice_d", "mse",
+        "cand_mse", "phi", "order", "sigma", "status"}`` (torch tensors on y's device): ``pred`` the winner's
+        predictions, ``choice_p[i]`` / ``choice_d[i]`` the winner (-1 / -1 when no candidate is eligible), ``mse[i]``
+        its hold-out MSE, ``cand_mse[i, k, j]`` that of ``(orders[j], diffs[k])``, ``phi`` / ``order`` / ``sigma`` /
+        ``status`` the winner's."""
+        import torch
+        orders = [int(m) for m in orders]
+        diffs = [int(d) for d in diffs]
+        if any(d >= 1 for d in diffs):
+            if getattr(self, "_arima", None) is None:
+                raise RuntimeError("plan_arima() (or plan_calendar(..., max_diff=d)) must be called first")
+            t_fit, n_rows = self._arima[0], self._arima[1]
+        else:
+            if self.t_fit is None:
+                raise RuntimeError("plan()/plan_calendar() must be called first")
+            t_fit, n_rows = self.t_fit, self.n_rows
+        yp, n, t_have, ld_y = _describe(y, "y")
+        if not (_is_torch(y) and y.is_cuda and y.dtype == torch.float32) or t_have < t_fit + int(n_hold):
+            raise ValueError(f"y must be a float32 CUDA tensor with at least t_fit + n_hold={t_fit + int(n_hold)} "
+                             "columns")
+        if n_pred is None:
+            n_pred = n_rows - int(pred_start)
+        self.set_stream(torch.cuda.current_stream(y.device).cuda_stream)
+        dev = y.device
+        out = torch.empty((n, n_pred), device=dev, dtype=torch.float32)
+        choice_p = torch.empty(n, device=dev, dtype=torch.int32)
+        choice_d = torch.empty(n, device=dev, dtype=torch.int32)
+        mse = torch.empty(n, device=dev, dtype=torch.float32)
+        cand_mse = torch.empty((n, len(diffs), len(orders)), device=dev, dtype=torch.float32)
+        phi = torch.empty((n, N.AR_MAX), device=dev, dtype=torch.float32)
+        order = torch.empty(n, device=dev, dtype=torch.int32)
+        sigma = torch.empty(n, device=dev, dtype=torch.float32)
+        status = torch.empty(n, device=dev, dtype=torch.int32)
+        cand = (C.c_int32 * max(len(orders), 1))(*orders)
+        dl = (C.c_int32 * max(len(diffs), 1))(*diffs)
+        st = N.MmfStats() if want_stats else None
+        N.check(self._lib.mmf_fit_select_arima_f32(self._h, yp, n, ld_y, int(n_hold), cand, len(orders), dl, len(diffs),
+                                                   int(pred_start), int(n_pred), out.data_ptr(), out.stride(0),
+                                                   choice_p.data_ptr(), choice_d.data_ptr(), mse.data_ptr(),
+                                                   cand_mse.data_ptr(), phi.data_ptr(), order.data_ptr(),
+                                                   sigma.data_ptr(), status.data_ptr(),
+                                                   C.byref(st) if st is not None else None))
+        res = {"pred": out, "choice_p": choice_p, "choice_d": choice_d, "mse": mse, "cand_mse": cand_mse, "phi": phi,
+               "order": order, "sigma": sigma, "status": status}
+        if st is not None:
+            self.launches += st.kernel_launches
+            res["stats"] = Stats(st.kernel_ms, st.total_ms, st.n_series, st.n_pending, st.h2d_bytes, st.d2h_bytes,
+                                 st.kernel_launches, {N.KERNEL_WARP: "warp", N.KERNEL_TC: "tc"}.get(st.kernel_used, "?"))
+        return res
+
     def capture(self, y, pred_start: int, n_pred: int, out=None, status=None):
         """Record one device-resident ``fit_forecast`` call as a CUDA graph.  Small batches are launch-bound (three
         kernel launches plus the Python/ctypes hop cost more than the kernels themselves): ``graph.replay()``

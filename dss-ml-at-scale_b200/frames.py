@@ -343,7 +343,9 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
     ``interval``: prediction standard errors too (``fit_forecast_se``), one call per calendar bucket.
     ``ar``: regression with AR(ar) errors (``fit_forecast_ar``), one call per calendar bucket; a tuple of orders
     chooses the order per series by hold-out MSE over the last ``horizon`` rows (``fit_select_ar``).
-    ``diff``: regression with ARIMA(ar, diff, 0) errors (``fit_forecast_arima``), one call per calendar bucket."""
+    ``diff``: regression with ARIMA(ar, diff, 0) errors (``fit_forecast_arima``), one call per calendar bucket; a tuple
+    of differencing orders (with ``ar`` a tuple of orders) chooses (p, d) per series by hold-out MSE over the last
+    ``horizon`` rows (``fit_select_arima``)."""
     if interval and select is not None:
         raise ValueError("interval= is not offered with select= (model selection returns point forecasts)")
     t_fit_min = min((b.t_len - (horizon if mode == "holdout" else 0)) for b in buckets) if buckets else 0
@@ -352,13 +354,17 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
         yield from _fit_buckets_ragged(buckets, eng, freq, horizon, mode, design, on_device)
         return
     for b in buckets:
-        if diff is None:
+        if diff is None or (isinstance(diff, tuple) and max(diff) == 0):
             out_days, pred_start, n_pred = eng.plan_calendar(b.start, b.t_len, freq, horizon, mode, design)
         else:
             out_days, pred_start, n_pred = eng.plan_calendar(b.start, b.t_len, freq, horizon, mode, design,
-                                                             max_diff=diff)
+                                                             max_diff=max(diff) if isinstance(diff, tuple) else diff)
         se = None
-        if diff is not None:
+        if isinstance(diff, tuple):
+            from .engine import device_packed
+            yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
+            pred = _host(eng.fit_select_arima(yd, horizon, ar, diff, pred_start, n_pred)["pred"])
+        elif diff is not None:
             from .engine import device_packed
             yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
             pred = _host(eng.fit_forecast_arima(yd, ar, diff, pred_start, n_pred)["pred"])
@@ -423,17 +429,44 @@ def _ar_order(ar, select, interval, mode="holdout"):
     return int(ar)
 
 
-def _diff_order(diff, ar, select, interval):
-    """validated differencing order of ``diff=`` (None: no differencing); ``ar`` must then be one order in 0..8"""
+def _diff_order(diff, ar, select, interval, mode="holdout"):
+    """validated differencing order of ``diff=`` (None: no differencing); ``ar`` must then be one order in 0..8.  A
+    sequence of differencing orders gives the tuple of candidate d's; ``ar`` is then one order or a sequence of them"""
     if diff is None:
         return None
     if select is not None or interval is not None:
         raise ValueError("diff= is not offered with select= or interval= (ARIMA forecasts come without either)")
+    if isinstance(diff, (list, tuple, np.ndarray)):
+        diffs = list(diff)
+        if not diffs:
+            raise ValueError("diff= needs at least one candidate differencing order")
+        if any(isinstance(d, bool) or not isinstance(d, (int, np.integer)) or not 0 <= int(d) <= DIFF_MAX for d in diffs):
+            raise ValueError(f"diff= candidate differencing orders must be integers in [0, {DIFF_MAX}], got {diff!r}")
+        diffs = [int(d) for d in diffs]
+        if any(b <= a for a, b in zip(diffs, diffs[1:])):
+            raise ValueError(f"diff= candidate differencing orders must be ascending and distinct, got {diff!r}")
+        if mode != "holdout":
+            raise ValueError("diff= with candidate differencing orders needs mode='holdout' (the last horizon rows score "
+                             "the candidates)")
+        return tuple(diffs)
     if isinstance(diff, bool) or not isinstance(diff, (int, np.integer)) or not 1 <= int(diff) <= DIFF_MAX:
         raise ValueError(f"diff must be a differencing order in [1, {DIFF_MAX}], got {diff!r}")
     if isinstance(ar, bool) or not isinstance(ar, (int, np.integer)) or not 0 <= int(ar) <= AR_MAX:
         raise ValueError(f"diff= needs one integer AR order ar in [0, {AR_MAX}], got ar={ar!r}")
     return int(diff)
+
+
+def _ar_orders_for(diff, ar, select, interval, mode):
+    """``ar=`` validated against ``diff=``: one order in 0..8 for a single d, the tuple of candidate orders for a tuple
+    of d's, and _ar_order's result without differencing"""
+    if diff is None:
+        return _ar_order(ar, select, interval, mode)
+    if not isinstance(diff, tuple):
+        return int(ar)
+    if not isinstance(ar, (list, tuple, np.ndarray)):
+        raise ValueError(f"diff= with candidate differencing orders needs candidate AR orders ar=(...) in [0, {AR_MAX}], "
+                         f"got ar={ar!r}")
+    return _ar_order(ar, select, interval, mode)
 
 
 def _bounds(pred, se, z):
@@ -578,14 +611,18 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     series on the differenced design, integrated back to levels.  ``Demand_Fitted`` holds one-step-ahead level
     predictions on the fit dates (NaN / null on the first d dates of a group) and the integrated dynamic forecast after
     them.  The schema is unchanged; every calendar bucket takes its own call.  ``diff=None`` leaves everything as it
-    was; ``diff`` is not offered with ``select=``, ``interval=`` or a tuple of AR orders.
+    was; an integer ``diff`` is not offered with ``select=``, ``interval=`` or a tuple of AR orders.
+    ``diff=(0, 1, 2)`` (ascending distinct orders in 0..2) with ``ar=(0, 1, 2, 3, 4)`` (a tuple of orders) chooses each
+    series' (p, d) by the MSE of its dynamic level forecast over the last ``horizon`` dates, the held-out rows of
+    ``mode='holdout'`` (``ForecastEngine.fit_select_arima``, DESIGN.md section 2 item 12); ``Demand_Fitted`` comes from
+    each series' winner.  Holdout mode only, one call per calendar bucket, schema unchanged.
     """
     eng = engine or default_engine()
     keys = list(keys)
     fitted_col = value_col + "_Fitted"
     z = _z_of(interval)
-    diff = _diff_order(diff, ar, select, interval)
-    ar = int(ar) if diff is not None else _ar_order(ar, select, interval, mode)
+    diff = _diff_order(diff, ar, select, interval, mode)
+    ar = _ar_orders_for(diff, ar, select, interval, mode)
     if pack == "host" and select is None and z is None and ar is None and isinstance(pdf, pd.DataFrame):
         one = _single_group_fast(pdf, keys, date_col, value_col, freq, horizon, mode, design, eng, null_keys_on_gaps)
         if one is not None:
@@ -698,8 +735,8 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     eng = engine or default_engine()
     keys = list(keys)
     z = _z_of(interval)
-    diff = _diff_order(diff, ar, select, interval)
-    ar = int(ar) if diff is not None else _ar_order(ar, select, interval, mode)
+    diff = _diff_order(diff, ar, select, interval, mode)
+    ar = _ar_orders_for(diff, ar, select, interval, mode)
     schema = tuning_schema(keys, date_col, value_col, interval=z is not None)
     buckets = _buckets_for(table, keys, date_col, value_col, freq, pack, eng)
     parts, lengths = [], []

@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define MMF_VERSION 107          /* 0.1.7 */
+#define MMF_VERSION 108          /* 0.1.8 */
 #define MMF_P 16                 /* design columns (zero-pad narrower designs) */
 #define MMF_PIVOT_TOL 1e-3f      /* per-series relative Cholesky pivot threshold */
 #define MMF_CAL_TOL 1e-10        /* aliasing threshold on the float64 calendar Gram */
@@ -272,6 +272,44 @@ int mmf_fit_forecast_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t 
                                int32_t diff_order, int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out,
                                float* out_phi, int32_t* out_order, float* out_sigma, int32_t* out_status,
                                mmf_stats* stats);
+
+/* ---- (p, d) selection by hold-out MSE on levels (DESIGN.md section 2 item 12) -----------------------------------------
+ * mmf_fit_select_arima_f32: orders [n_orders] (1 .. MMF_ARSEL_MAX_CAND ascending distinct values in [0, MMF_AR_MAX]) and
+ * diffs [n_diffs] (1 .. MMF_DIFF_MAX + 1 ascending distinct values in [0, MMF_DIFF_MAX]) are host arrays; the candidates
+ * are every pair (p, d) in d-major list order (d ascending, then p ascending).  Fit rows [0, t_fit), held-out rows
+ * [t_fit, t_fit + n_hold) of the level design and of y.
+ *   candidate (p, 0) is candidate p of mmf_fit_select_ar_f32 (the plain regression for p = 0, AR(p) on y otherwise, with
+ *   the mmf_plan_design plan); candidate (p, d >= 1) is mmf_fit_forecast_arima_f32(ar_order = p, diff_order = d) with
+ *   the mmf_plan_arima plan;
+ *   score: the MSE on levels of the candidate's dynamic forecast from origin t_fit over the held-out rows (the predictions
+ *   of its single call with pred_start = t_fit, n_pred = n_hold) against y[t_fit, t_fit + n_hold), over the points
+ *   where both are finite, summed in float64, stored as float32, NaN where no point is scored.  Held-out y never enters
+ *   a z-space history or a level chain;
+ *   eligible: the fit the candidate builds on (on y for d = 0, on z' of its d otherwise) is not empty;
+ *   choice: the first minimum of the float64 MSE over the eligible candidates in list order (ties go to the smaller d,
+ *   then the smaller p); the last eligible candidate when none scores a point; (-1, -1) when none is eligible.
+ * out_pred[i, t - pred_start] is the prediction of the chosen candidate, bit-equal to its single call (pred, phi, order,
+ * sigma, status): mmf_fit_select_ar_f32 with orders (p) for d = 0, mmf_fit_forecast_arima_f32(p, d) otherwise (NaN on
+ * the rows t < d).  For d >= 1 the status is that of the fit on z'.  With diffs = (0) the call is mmf_fit_select_ar_f32.
+ * A row with no eligible candidate gets choice (-1, -1), status 1, order 0, phi 0 and NaN sigma, MSEs and predictions.
+ * y is read on [0, t_fit + n_hold) only.  out_choice_p [n], out_choice_d [n], out_mse [n] (the winner's MSE),
+ * out_cand_mse [n][n_diffs][n_orders], out_phi [n][MMF_AR_MAX], out_order [n], out_sigma [n], out_status [n] are
+ * nullable.
+ * Plans: a listed d = 0 needs the mmf_plan_design plan, a listed d >= 1 the mmf_plan_arima plan with max_diff >= max(diffs)
+ * (missing: MMF_E_NOPLAN; max_diff too small: MMF_E_INVALID).  A call that uses both needs them built from the same X (the
+ * same rows, columns, t_fit and bytes; otherwise MMF_E_INVALID).  1 <= n_hold, t_fit + n_hold <= the planned rows,
+ * ld_y >= t_fit + n_hold.  Otherwise the contract of mmf_fit_select_ar_f32: device buffers only, any ld_out >= n_pred and
+ * any base pointer with only columns [0, n_pred) written, enqueue-only unless `stats` is non-NULL (n_pending sums the
+ * fits of every listed d), mmf_config.kernel and assume_finite honoured, refused arguments write nothing.  Scratch: per
+ * slab, z' as mmf_fit_forecast_arima_f32, 20 B per row.
+ * replaces: the reference's per-group tuning loop over p and d (02:435-488, search space 02:461-465) as an exhaustive
+ * search over (p, d) with q = 0, not TPE over (p, d, q). */
+int mmf_fit_select_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
+                             const int32_t* orders, int32_t n_orders, const int32_t* diffs, int32_t n_diffs,
+                             int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out,
+                             int32_t* out_choice_p, int32_t* out_choice_d, float* out_mse,
+                             float* out_cand_mse /* [n][n_diffs][n_orders] */, float* out_phi, int32_t* out_order,
+                             float* out_sigma, int32_t* out_status, mmf_stats* stats);
 
 /* ---- ragged batches: groups on MANY calendars in one launch ---------------------------------------------
  * The reference re-indexes every group on its own calendar (sort_values + asfreq per group, 02:422-423), so one

@@ -518,13 +518,14 @@ int build_multi(MultiPlan& m, const double* X_all, int32_t n_cal, const int32_t*
 // ARIMA calls (arima != nullptr, with ar): y / ld_y are the slab's levels; diff_kernel writes z' into the context's
 // scratch first, and the fit passes and arima_kernel read z' with `plan` = the plan of D_d.  (p, d) selection calls
 // (asel != nullptr) run this once per listed d and end in arima_select_kernel; their d = 0 pass (arima->d == 0) fits y
-// itself with the mmf_plan_design plan.
+// itself with the mmf_plan_design plan.  ARMA calls (arma != nullptr, with ar) run arma_kernel behind ar_kernel (d = 0,
+// arima == nullptr) or arima_kernel.
 int run_device_slab(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, int64_t ld_y, int32_t pred_start,
                     int32_t n_pred, float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s,
                     int* launches, int* kernel_used, float* const* out_more, int n_out, int multimem,
                     const SelectArgs* sel, const SeArgs* se = nullptr, const ArArgs* ar = nullptr,
                     const ArSelArgs* arsel = nullptr, const ArimaArgs* arima = nullptr,
-                    const ArimaSelArgs* asel = nullptr) {
+                    const ArimaSelArgs* asel = nullptr, const ArmaArgs* arma = nullptr) {
   const DesignView d = view_of(plan);
   ArimaArgs ma{};
   if (arima != nullptr) {
@@ -634,6 +635,12 @@ int run_device_slab(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, i
            : arima != nullptr ? launch_arima(d, a, *ar, ma, s)
            : arsel != nullptr ? launch_ar_select(d, a, *ar, *arsel, s) : launch_ar(d, a, *ar, s));
     ++*launches;
+    if (arma != nullptr) {
+      ArimaArgs mh = ma;
+      if (arima == nullptr) { mh.y = a.y; mh.ld_y = a.ld_y; mh.t_fit = d.t_fit; mh.d = 0; }
+      CU_TRY(launch_arma(d, a, *ar, mh, *arma, s));
+      ++*launches;
+    }
   }
   if (many_pred) {
     PredictLaunch pl;
@@ -681,7 +688,8 @@ int run_device(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, int64_
                int32_t n_pred, float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s,
                int* launches, int* kernel_used, float* const* out_more = nullptr, int n_out = 1, int multimem = 0,
                const SelectArgs* sel = nullptr, uint32_t* slab_pending = nullptr, const SeArgs* se = nullptr,
-               const ArArgs* ar = nullptr, const ArSelArgs* arsel = nullptr, const ArimaArgs* arima = nullptr) {
+               const ArArgs* ar = nullptr, const ArSelArgs* arsel = nullptr, const ArimaArgs* arima = nullptr,
+               const ArmaArgs* arma = nullptr) {
   const int64_t slab = slab_rows(plan, n);
   for (int64_t off = 0, i = 0; off < n; off += slab, ++i) {
     const int64_t m = std::min(slab, n - off);
@@ -714,10 +722,17 @@ int run_device(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, int64_
       if (arsel_slab.mse) arsel_slab.mse += off;
       if (arsel_slab.cand_mse) arsel_slab.cand_mse += off * arsel_slab.n_cand;
     }
+    ArmaArgs arma_slab{};
+    if (arma != nullptr) {
+      arma_slab = *arma;
+      if (arma_slab.theta) arma_slab.theta += off * MMF_MA_MAX;
+      if (arma_slab.ma_order) arma_slab.ma_order += off;
+    }
     const int rc = run_device_slab(ctx, plan, y + off * ld_y, m, ld_y, pred_start, n_pred, out + off * ld_out, ld_out,
                                    beta ? beta + off * P : nullptr, status + off, s, launches, kernel_used, more, n_out,
                                    multimem, sel != nullptr ? &sel_slab : nullptr, se != nullptr ? &se_slab : nullptr,
-                                   ar != nullptr ? &ar_slab : nullptr, arsel != nullptr ? &arsel_slab : nullptr, arima);
+                                   ar != nullptr ? &ar_slab : nullptr, arsel != nullptr ? &arsel_slab : nullptr, arima,
+                                   nullptr, arma != nullptr ? &arma_slab : nullptr);
     if (rc != MMF_OK) return rc;
     if (slab_pending != nullptr) {
       if (*kernel_used == MMF_KERNEL_TC)
@@ -1297,7 +1312,8 @@ int mmf_fit_forecast_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
 // the enqueue / stats tail of the AR entry points (arguments already checked, n > 0, device set)
 static int run_ar_call(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, int64_t ld_y, int32_t pred_start,
                        int32_t n_pred, float* out_pred, int64_t ld_out, int32_t* out_status, const ArArgs& ar,
-                       const ArSelArgs* arsel, const ArimaArgs* arima, mmf_stats* stats) {
+                       const ArSelArgs* arsel, const ArimaArgs* arima, mmf_stats* stats,
+                       const ArmaArgs* arma = nullptr) {
   int32_t* status = out_status;
   if (!status) {
     int rc = grow_status_scratch(ctx, n, ctx->stream);
@@ -1318,7 +1334,7 @@ static int run_ar_call(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n
   int launches = 0, kernel_used = 0;
   if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, ctx->stream));
   int rc = run_device(ctx, plan, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, nullptr, status, ctx->stream,
-                      &launches, &kernel_used, nullptr, 1, 0, nullptr, slab_pending, nullptr, &ar, arsel, arima);
+                      &launches, &kernel_used, nullptr, 1, 0, nullptr, slab_pending, nullptr, &ar, arsel, arima, arma);
   if (rc != MMF_OK) return rc;
   if (stats) {
     CU_TRY(cudaEventRecord(ctx->ev_k1, ctx->stream));
@@ -1489,6 +1505,63 @@ int mmf_fit_forecast_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t 
   ArimaArgs ma{};
   ma.y = y; ma.ld_y = ld_y; ma.t_fit = ap.t_fit; ma.d = diff_order;
   return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, &ma, stats);
+}
+
+// ---- regression with ARIMA(p, d, q) errors (DESIGN.md section 2 item 13) -------------------------------------------------
+int mmf_fit_forecast_arma_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
+                              int32_t diff_order, int32_t ma_order, int32_t long_order, int32_t pred_start,
+                              int32_t n_pred, float* out_pred, int64_t ld_out, float* out_phi, float* out_theta,
+                              int32_t* out_order, int32_t* out_ma_order, float* out_sigma, int32_t* out_status,
+                              mmf_stats* stats) {
+  if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
+  GrowScope grow_scope(ctx);
+  if (n < 0) return fail(MMF_E_INVALID, "n < 0");
+  if (n > 0 && (!y || !out_pred)) return fail(MMF_E_INVALID, "y or out_pred is NULL");
+  if (ar_order < 0 || ar_order > MMF_AR_MAX) return fail(MMF_E_INVALID, "ar_order=%d outside [0,%d]", ar_order, MMF_AR_MAX);
+  if (ma_order < 1 || ma_order > MMF_MA_MAX) return fail(MMF_E_INVALID, "ma_order=%d outside [1,%d]", ma_order, MMF_MA_MAX);
+  if (diff_order < 0 || diff_order > MMF_DIFF_MAX)
+    return fail(MMF_E_INVALID, "diff_order=%d outside [0,%d]", diff_order, MMF_DIFF_MAX);
+  // d = 0 models y with the mmf_plan_design plan; d >= 1 models z' with the mmf_plan_arima plan
+  const ArimaPlan& ap = ctx->arima;
+  if (diff_order == 0 && !ctx->plan.valid) return fail(MMF_E_NOPLAN, "mmf_plan_design has not been called");
+  if (diff_order >= 1 && !ap.valid) return fail(MMF_E_NOPLAN, "mmf_plan_arima has not been called");
+  if (diff_order > (diff_order == 0 ? 0 : ap.max_diff))
+    return fail(MMF_E_INVALID, "diff_order=%d above the planned max_diff=%d", diff_order, ap.max_diff);
+  const Plan& pl = diff_order == 0 ? ctx->plan : ap.diff[diff_order - 1];
+  const int32_t T = diff_order == 0 ? pl.t_fit : ap.t_fit;          // level fit rows
+  const int32_t n_rows = diff_order == 0 ? pl.n_rows : ap.n_rows;
+  const int32_t lmin = std::max(ar_order, ma_order);
+  if (long_order != 0 && (long_order < lmin || long_order > MMF_HR_LONG_MAX))
+    return fail(MMF_E_INVALID, "long_order=%d outside {0} and [%d,%d]", long_order, lmin, MMF_HR_LONG_MAX);
+  if (ld_y < T) return fail(MMF_E_INVALID, "ld_y=%lld < t_fit=%d", (long long)ld_y, T);
+  if (n_pred < 1 || pred_start < 0 || (int64_t)pred_start + n_pred > n_rows)
+    return fail(MMF_E_INVALID, "prediction rows [%d,%d) outside the planned design (%d rows)", pred_start,
+                pred_start + n_pred, n_rows);
+  if (ld_out < n_pred) return fail(MMF_E_INVALID, "ld_out=%lld < n_pred=%d", (long long)ld_out, n_pred);
+  if (stats) memset(stats, 0, sizeof(*stats));
+  if (n == 0) return MMF_OK;
+  CU_TRY(cudaSetDevice(ctx->device));
+  if (!is_device_ptr(y) || !is_device_ptr(out_pred) || (out_phi && !is_device_ptr(out_phi)) ||
+      (out_theta && !is_device_ptr(out_theta)) || (out_order && !is_device_ptr(out_order)) ||
+      (out_ma_order && !is_device_ptr(out_ma_order)) || (out_sigma && !is_device_ptr(out_sigma)) ||
+      (out_status && !is_device_ptr(out_status)))
+    return fail(MMF_E_UNSUPPORTED, "mmf_fit_forecast_arma_f32 takes device buffers only");
+  ArArgs ar{};
+  ar.p = ar_order; ar.phi = out_phi; ar.order = out_order; ar.sigma = out_sigma; ar.nz = pl.d_nz;
+  ArmaArgs hr{};
+  hr.q = ma_order;
+  if (long_order == 0) {                   // min(32, max(2 max(p, q), floor(ln(t_fit - d)^2)))
+    const double lt = std::log((double)(T - diff_order));
+    long_order = std::min<int32_t>(MMF_HR_LONG_MAX, std::max<int32_t>(2 * lmin, (int32_t)std::floor(lt * lt)));
+  }
+  hr.m = long_order;
+  hr.theta = out_theta; hr.ma_order = out_ma_order;
+  if (diff_order == 0)
+    return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, nullptr,
+                       stats, &hr);
+  ArimaArgs ma{};
+  ma.y = y; ma.ld_y = ld_y; ma.t_fit = ap.t_fit; ma.d = diff_order;
+  return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, &ma, stats, &hr);
 }
 
 // ---- (p, d) selection by hold-out MSE on levels (DESIGN.md section 2 item 12) -------------------------------------------

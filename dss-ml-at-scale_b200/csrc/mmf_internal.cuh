@@ -283,6 +283,18 @@ struct ArimaSelArgs {
 cudaError_t launch_arima_select(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
                                 const ArimaSelArgs& sel, cudaStream_t s);
 
+// regression with ARIMA(p, d, q) errors (arma.cu, DESIGN.md section 2 item 13): arma_kernel runs behind ar_kernel
+// (d = 0) or arima_kernel (d >= 1) with order p, which write every row's fallback outputs, and overwrites the outputs of
+// the rows whose Hannan-Rissanen estimate passes the gate.  ArimaArgs::d = 0 with ArimaArgs::y = FitArgs::y for d = 0.
+struct ArmaArgs {
+  int32_t q;                              // 1 .. MMF_MA_MAX
+  int32_t m;                              // long AR order, max(p, q) .. MMF_HR_LONG_MAX (resolved: never 0)
+  float* theta;                           // nullable [n][MMF_MA_MAX]
+  int32_t* ma_order;                      // nullable [n]
+};
+cudaError_t launch_arma(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
+                        const ArmaArgs& hr, cudaStream_t s);
+
 // integer series -> float32 staging rows, sentinel -> NaN (widen.cu); dtype = MMF_DT_I16 / U16 / I32
 cudaError_t launch_widen(int dtype, const void* src, int64_t ld_src, float* dst, int64_t ld_dst, int64_t n, int32_t t,
                          int sm_count, cudaStream_t s);

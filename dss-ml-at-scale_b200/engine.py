@@ -571,6 +571,55 @@ class ForecastEngine:
                                  st.kernel_launches, {N.KERNEL_WARP: "warp", N.KERNEL_TC: "tc"}.get(st.kernel_used, "?"))
         return res
 
+    def fit_forecast_arma(self, y, ar_order: int, ma_order: int, diff_order: int = 0, pred_start: int = 0,
+                          n_pred: int | None = None, long_order: int = 0, want_stats: bool = False):
+        """Regression with ARIMA(``ar_order``, ``diff_order``, ``ma_order``) errors (``mmf_fit_forecast_arma_f32``,
+        DESIGN.md section 2 item 13): the plain fit (on the differenced series and design for ``diff_order`` >= 1),
+        then Hannan-Rissanen on its residuals -- a long AR of order ``long_order`` (0: the default) gives innovation
+        estimates, one least-squares solve gives (phi, theta).  Not SARIMAX's Kalman-filter MLE, and beta is not
+        re-estimated.  A series whose estimate fails the gate (too short, collinear, non-stationary AR or non-invertible
+        MA part) gets ``fit_forecast_arima`` / ``fit_forecast_ar`` with ``ar_order`` bit for bit, ``ma_order`` 0 and
+        theta 0.  ``diff_order`` 0 needs ``plan``'s design, >= 1 ``plan_arima``'s.  ``y`` is a float32 CUDA tensor of
+        levels; ``n_pred`` defaults to every design row from ``pred_start`` on.  Returns ``{"pred", "phi", "theta",
+        "order", "ma_order", "sigma", "status"}`` (torch tensors on y's device): ``pred[i, j]`` the level prediction of
+        design row ``pred_start + j`` (one step ahead in sample, the dynamic forecast from t_fit beyond it)."""
+        import torch
+        if int(diff_order) >= 1:
+            if getattr(self, "_arima", None) is None:
+                raise RuntimeError("plan_arima() (or plan_calendar(..., max_diff=d)) must be called first")
+            t_fit, n_rows = self._arima[0], self._arima[1]
+        else:
+            if self.t_fit is None:
+                raise RuntimeError("plan()/plan_calendar() must be called first")
+            t_fit, n_rows = self.t_fit, self.n_rows
+        yp, n, t_have, ld_y = _describe(y, "y")
+        if not (_is_torch(y) and y.is_cuda and y.dtype == torch.float32) or t_have < t_fit:
+            raise ValueError(f"y must be a float32 CUDA tensor with at least t_fit={t_fit} columns")
+        if n_pred is None:
+            n_pred = n_rows - int(pred_start)
+        self.set_stream(torch.cuda.current_stream(y.device).cuda_stream)
+        dev = y.device
+        out = torch.empty((n, n_pred), device=dev, dtype=torch.float32)
+        phi = torch.empty((n, N.AR_MAX), device=dev, dtype=torch.float32)
+        theta = torch.empty((n, N.MA_MAX), device=dev, dtype=torch.float32)
+        order = torch.empty(n, device=dev, dtype=torch.int32)
+        ma = torch.empty(n, device=dev, dtype=torch.int32)
+        sigma = torch.empty(n, device=dev, dtype=torch.float32)
+        status = torch.empty(n, device=dev, dtype=torch.int32)
+        st = N.MmfStats() if want_stats else None
+        N.check(self._lib.mmf_fit_forecast_arma_f32(self._h, yp, n, ld_y, int(ar_order), int(diff_order), int(ma_order),
+                                                    int(long_order), int(pred_start), int(n_pred), out.data_ptr(),
+                                                    out.stride(0), phi.data_ptr(), theta.data_ptr(), order.data_ptr(),
+                                                    ma.data_ptr(), sigma.data_ptr(), status.data_ptr(),
+                                                    C.byref(st) if st is not None else None))
+        res = {"pred": out, "phi": phi, "theta": theta, "order": order, "ma_order": ma, "sigma": sigma,
+               "status": status}
+        if st is not None:
+            self.launches += st.kernel_launches
+            res["stats"] = Stats(st.kernel_ms, st.total_ms, st.n_series, st.n_pending, st.h2d_bytes, st.d2h_bytes,
+                                 st.kernel_launches, {N.KERNEL_WARP: "warp", N.KERNEL_TC: "tc"}.get(st.kernel_used, "?"))
+        return res
+
     def fit_select_ar(self, y, n_hold: int, orders=(0, 1, 2, 3, 4), pred_start: int = 0, n_pred: int | None = None,
                       want_stats: bool = False):
         """Regression with AR(p) errors, p chosen per series by hold-out MSE (``mmf_fit_select_ar_f32``, DESIGN.md

@@ -23,7 +23,7 @@ import pandas as pd
 
 from . import design as D
 from .engine import ForecastEngine, alloc_packed, default_engine
-from ._native import AR_MAX, DIFF_MAX
+from ._native import AR_MAX, DIFF_MAX, MA_MAX
 
 FORECAST_HORIZON = 40                      # 02:341
 DEFAULT_KEYS = ("Product", "SKU")          # 02:526
@@ -338,14 +338,16 @@ def _host(x):
     return x.cpu().numpy() if hasattr(x, "cpu") else np.asarray(x)
 
 
-def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, interval=False, ar=None, diff=None):
+def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, interval=False, ar=None, diff=None,
+                 ma=None):
     """Run the engine over every bucket: yields (bucket, out_days, n_pred, y_host, pred_host, se_host or None).
     ``interval``: prediction standard errors too (``fit_forecast_se``), one call per calendar bucket.
     ``ar``: regression with AR(ar) errors (``fit_forecast_ar``), one call per calendar bucket; a tuple of orders
     chooses the order per series by hold-out MSE over the last ``horizon`` rows (``fit_select_ar``).
     ``diff``: regression with ARIMA(ar, diff, 0) errors (``fit_forecast_arima``), one call per calendar bucket; a tuple
     of differencing orders (with ``ar`` a tuple of orders) chooses (p, d) per series by hold-out MSE over the last
-    ``horizon`` rows (``fit_select_arima``)."""
+    ``horizon`` rows (``fit_select_arima``).
+    ``ma``: regression with ARIMA(ar, diff or 0, ma) errors (``fit_forecast_arma``), one call per calendar bucket."""
     if interval and select is not None:
         raise ValueError("interval= is not offered with select= (model selection returns point forecasts)")
     t_fit_min = min((b.t_len - (horizon if mode == "holdout" else 0)) for b in buckets) if buckets else 0
@@ -360,7 +362,11 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
             out_days, pred_start, n_pred = eng.plan_calendar(b.start, b.t_len, freq, horizon, mode, design,
                                                              max_diff=max(diff) if isinstance(diff, tuple) else diff)
         se = None
-        if isinstance(diff, tuple):
+        if ma is not None:
+            from .engine import device_packed
+            yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
+            pred = _host(eng.fit_forecast_arma(yd, ar, ma, diff or 0, pred_start, n_pred)["pred"])
+        elif isinstance(diff, tuple):
             from .engine import device_packed
             yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
             pred = _host(eng.fit_select_arima(yd, horizon, ar, diff, pred_start, n_pred)["pred"])
@@ -454,6 +460,23 @@ def _diff_order(diff, ar, select, interval, mode="holdout"):
     if isinstance(ar, bool) or not isinstance(ar, (int, np.integer)) or not 0 <= int(ar) <= AR_MAX:
         raise ValueError(f"diff= needs one integer AR order ar in [0, {AR_MAX}], got ar={ar!r}")
     return int(diff)
+
+
+def _arma_orders(ma, ar, diff, select, interval):
+    """validated (ar, diff, ma) of ``ma=``: one MA order in 1..4 with one AR order in 0..8 and ``diff`` None (d = 0) or
+    one differencing order in 1..2.  Choosing q is not built, so a sequence of MA orders is refused."""
+    if select is not None or interval is not None:
+        raise ValueError("ma= is not offered with select= or interval= (ARMA forecasts come without either)")
+    if isinstance(ma, (list, tuple, np.ndarray)):
+        raise ValueError(f"ma= takes one MA order: choosing q per series is not built, got ma={ma!r}")
+    if isinstance(ma, bool) or not isinstance(ma, (int, np.integer)) or not 1 <= int(ma) <= MA_MAX:
+        raise ValueError(f"ma must be an MA order in [1, {MA_MAX}], got {ma!r}")
+    if isinstance(ar, bool) or not isinstance(ar, (int, np.integer)) or not 0 <= int(ar) <= AR_MAX:
+        raise ValueError(f"ma= needs one integer AR order ar in [0, {AR_MAX}], got ar={ar!r}")
+    if diff is not None and (isinstance(diff, bool) or not isinstance(diff, (int, np.integer))
+                             or not 0 <= int(diff) <= DIFF_MAX):
+        raise ValueError(f"ma= takes one differencing order diff in [0, {DIFF_MAX}] (or None), got diff={diff!r}")
+    return int(ar), (int(diff) if diff else None), int(ma)
 
 
 def _ar_orders_for(diff, ar, select, interval, mode):
@@ -572,7 +595,7 @@ def _single_group_fast(pdf, keys, date_col, value_col, freq, horizon, mode, desi
 def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Demand",
                     freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                     engine: ForecastEngine | None = None, pack: str = "host", select=None,
-                    null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None) -> pd.DataFrame:
+                    null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None, ma=None) -> pd.DataFrame:
     """Fit + forecast every group in ``pdf``; returns ``tuning_schema`` rows
     (keys..., Date, Demand, Demand_Fitted), groups in key order, dates ascending.
 
@@ -616,13 +639,22 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     series' (p, d) by the MSE of its dynamic level forecast over the last ``horizon`` dates, the held-out rows of
     ``mode='holdout'`` (``ForecastEngine.fit_select_arima``, DESIGN.md section 2 item 12); ``Demand_Fitted`` comes from
     each series' winner.  Holdout mode only, one call per calendar bucket, schema unchanged.
+
+    ``ma=q`` (1 <= q <= 4) with ``ar=p`` (0 <= p <= 8) and ``diff=d`` (None for d = 0, or 1, 2) fits regression with
+    ARIMA(p, d, q) errors by Hannan-Rissanen (``ForecastEngine.fit_forecast_arma``, DESIGN.md section 2 item 13);
+    ``ar=1, diff=2, ma=1`` is the reference notebook's order.  A series whose estimate fails the gate gets the
+    ARIMA(p, d, 0) forecast.  One call per calendar bucket, schema unchanged; ``ma=None`` leaves everything as it was.
+    Not offered with ``select=`` or ``interval=``, and a sequence of MA orders is refused (choosing q is not built).
     """
     eng = engine or default_engine()
     keys = list(keys)
     fitted_col = value_col + "_Fitted"
     z = _z_of(interval)
-    diff = _diff_order(diff, ar, select, interval, mode)
-    ar = _ar_orders_for(diff, ar, select, interval, mode)
+    if ma is None:
+        diff = _diff_order(diff, ar, select, interval, mode)
+        ar = _ar_orders_for(diff, ar, select, interval, mode)
+    else:
+        ar, diff, ma = _arma_orders(ma, ar, diff, select, interval)
     if pack == "host" and select is None and z is None and ar is None and isinstance(pdf, pd.DataFrame):
         one = _single_group_fast(pdf, keys, date_col, value_col, freq, horizon, mode, design, eng, null_keys_on_gaps)
         if one is not None:
@@ -630,7 +662,7 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     buckets = _buckets_for(pdf, keys, date_col, value_col, freq, pack, eng)
     parts, lengths = [], []
     for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
-                                                              pack == "device", z is not None, ar, diff):
+                                                              pack == "device", z is not None, ar, diff, ma):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n), n_pred)
         # key columns keep the dtype they came in with (no per-row string inference on N x T values)
@@ -721,13 +753,13 @@ def backtest_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
 def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Demand",
                    freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                    engine: ForecastEngine | None = None, pack: str = "host", select=None,
-                   null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None):
+                   null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None, ma=None):
     """Arrow ``Table``/``RecordBatch`` in -> Arrow ``Table`` with ``tuning_schema`` out (the ``mapInArrow``
     flavour of the boundary).  No pandas frame of the rows on either side: keys are dictionary-encoded on the way
     in and expanded from a dictionary on the way out, dates and values are NumPy views of Arrow buffers.
     ``interval=level`` adds the ``{value}_Lower`` / ``{value}_Upper`` columns of ``forecast_groups`` (schema:
     ``tuning_schema(..., interval=True)``).  ``ar=p`` fits regression with AR(p) errors and ``ar=(0, 1, 2, 3, 4)`` chooses the order per series, as in
-    ``forecast_groups``; ``diff=d`` with ``ar=p`` fits ARIMA(p, d, 0) errors as there."""
+    ``forecast_groups``; ``diff=d`` with ``ar=p`` fits ARIMA(p, d, 0) errors as there, and ``ma=q`` ARIMA(p, d, q)."""
     import pyarrow as pa
 
     if isinstance(table, pa.RecordBatch):
@@ -735,13 +767,16 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     eng = engine or default_engine()
     keys = list(keys)
     z = _z_of(interval)
-    diff = _diff_order(diff, ar, select, interval, mode)
-    ar = _ar_orders_for(diff, ar, select, interval, mode)
+    if ma is None:
+        diff = _diff_order(diff, ar, select, interval, mode)
+        ar = _ar_orders_for(diff, ar, select, interval, mode)
+    else:
+        ar, diff, ma = _arma_orders(ma, ar, diff, select, interval)
     schema = tuning_schema(keys, date_col, value_col, interval=z is not None)
     buckets = _buckets_for(table, keys, date_col, value_col, freq, pack, eng)
     parts, lengths = [], []
     for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
-                                                              pack == "device", z is not None, ar, diff):
+                                                              pack == "device", z is not None, ar, diff, ma):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n, dtype=np.int32), n_pred)
         cols = []

@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define MMF_VERSION 108          /* 0.1.8 */
+#define MMF_VERSION 109          /* 0.1.9 */
 #define MMF_P 16                 /* design columns (zero-pad narrower designs) */
 #define MMF_PIVOT_TOL 1e-3f      /* per-series relative Cholesky pivot threshold */
 #define MMF_CAL_TOL 1e-10        /* aliasing threshold on the float64 calendar Gram */
@@ -42,6 +42,9 @@ extern "C" {
 #define MMF_AR_KAPPA_MAX 0.999   /* Levinson-Durbin stops before a partial autocorrelation |kappa| >= this */
 #define MMF_ARSEL_MAX_CAND 9     /* candidate AR orders per mmf_fit_select_ar_f32 call (0 .. MMF_AR_MAX) */
 #define MMF_DIFF_MAX 2           /* largest differencing order of mmf_fit_forecast_arima_f32 */
+#define MMF_MA_MAX 4             /* largest MA order of mmf_fit_forecast_arma_f32 */
+#define MMF_HR_LONG_MAX 32       /* largest long AR order of the Hannan-Rissanen step 1 (one lag per lane of a warp) */
+#define MMF_HR_PIVOT_TOL 1e-5    /* a Hannan-Rissanen Cholesky pivot must exceed this x its Gram diagonal */
 
 /* return codes */
 #define MMF_OK 0
@@ -272,6 +275,47 @@ int mmf_fit_forecast_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t 
                                int32_t diff_order, int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out,
                                float* out_phi, int32_t* out_order, float* out_sigma, int32_t* out_status,
                                mmf_stats* stats);
+
+/* ---- regression with ARIMA(p, d, q) errors (DESIGN.md section 2 item 13) ------------------------------------------------
+ * mmf_fit_forecast_arma_f32: for series i, 0 <= ar_order = p <= MMF_AR_MAX, 1 <= ma_order = q <= MMF_MA_MAX and
+ * 0 <= diff_order = d <= MMF_DIFF_MAX (d = 0 needs the mmf_plan_design plan; d >= 1 the mmf_plan_arima plan with
+ * max_diff >= d; missing: MMF_E_NOPLAN, max_diff too small: MMF_E_INVALID).  The series modelled is y (d = 0) or z' of
+ * mmf_fit_forecast_arima_f32 (d >= 1); e_t is the residual of its plain fit on the observed fit rows t < T = t_fit - d
+ * (0 elsewhere), and the status is that fit's.  Hannan-Rissanen, no likelihood optimisation and no re-estimation of beta
+ * (it is not SARIMAX's Kalman-filter MLE):
+ *   long order m = long_order (max(p, q) <= m <= MMF_HR_LONG_MAX), or for long_order = 0
+ *   min(MMF_HR_LONG_MAX, max(2 max(p, q), floor(ln(T)^2)));
+ *   step 1: mmf_fit_forecast_ar_f32's estimator with order m (r_0..r_m over n_obs, the dof rule, Levinson-Durbin with the
+ *   kappa stop) gives psi and the completed order m_i; the filled long-AR residuals u^L (e on observed fit rows, the AR
+ *   prediction sum_j psi_j u^L_{s-j} elsewhere, 0 before row 0) give eps^_s = e_s - sum_{j<=m_i} psi_j u^L_{s-j} on the
+ *   observed fit rows;
+ *   step 2: the rows R = { t in [m + q, T) : e observed at t, t-1, .., t-max(p, q) } regress e_t on (e_{t-1..t-p},
+ *   eps^_{t-1..t-q}) by float64 normal equations and an in-order Cholesky: (phi_1..phi_p, theta_1..theta_q), with the
+ *   sign convention u_t = sum phi_j u_{t-j} + eps_t + sum theta_j eps_{t-j};
+ *   gate: m_i >= 1, |R| > p + q, every Cholesky pivot > MMF_HR_PIVOT_TOL x its Gram diagonal, and the step-down recursion
+ *   of 1 - sum phi_j z^j and of 1 + sum theta_j z^j gives every |kappa| < MMF_AR_KAPPA_MAX (stationary AR part,
+ *   invertible MA part);
+ *   fallback: a series that fails the gate gets, bit for bit, mmf_fit_forecast_ar_f32(p) (d = 0, p >= 1), the plain
+ *   regression of mmf_fit_select_ar_f32 with orders (0) (d = 0, p = 0) or mmf_fit_forecast_arima_f32(p, d) (d >= 1) in
+ *   out_pred, out_phi, out_order, out_sigma and out_status, with ma_order 0 and theta 0;
+ *   forecast (gated series): from s = 0, with u_s = eps~_s = 0 for s < 0, pr_s = sum phi_j u_{s-j} + sum theta_j eps~_{s-j};
+ *   on an observed fit row u_s = e_s and eps~_s = e_s - pr_s, elsewhere u_s = pr_s and eps~_s = 0.  The prediction is
+ *   c + a_s.gamma + pr_s, for d >= 1 integrated to levels as mmf_fit_forecast_arima_f32 does (NaN for t < d).
+ *   sigma = sqrt(mean of eps~_t^2 over R); order = p, ma_order = q.
+ * out_pred[i, t - pred_start]: one step ahead in sample, the dynamic forecast from t_fit beyond it; y is read on
+ * [0, t_fit) only.  The recursion never restarts: a row's prediction does not depend on the requested window.
+ * out_phi [n][MMF_AR_MAX], out_theta [n][MMF_MA_MAX], out_order [n], out_ma_order [n], out_sigma [n], out_status [n] are
+ * nullable (empty series: status 1, NaN predictions and sigma, orders 0, phi and theta 0).  Otherwise the contract of
+ * mmf_fit_forecast_arima_f32: device buffers only, any ld_out >= n_pred and any base pointer with only columns
+ * [0, n_pred) written, enqueue-only unless `stats` is non-NULL, mmf_config.kernel and assume_finite honoured, refused
+ * arguments write nothing.
+ * replaces: SARIMAX(p, d, q) + exog fit and predict of the reference's per-group model (02:441-450, 472-488 with q > 0),
+ * e.g. its order (1, 2, 1) (02:226-229), for caller-fixed orders. */
+int mmf_fit_forecast_arma_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
+                              int32_t diff_order, int32_t ma_order, int32_t long_order, int32_t pred_start,
+                              int32_t n_pred, float* out_pred, int64_t ld_out, float* out_phi, float* out_theta,
+                              int32_t* out_order, int32_t* out_ma_order, float* out_sigma, int32_t* out_status,
+                              mmf_stats* stats);
 
 /* ---- (p, d) selection by hold-out MSE on levels (DESIGN.md section 2 item 12) -----------------------------------------
  * mmf_fit_select_arima_f32: orders [n_orders] (1 .. MMF_ARSEL_MAX_CAND ascending distinct values in [0, MMF_AR_MAX]) and

@@ -22,6 +22,7 @@ AR_MAX, AR_KAPPA_MAX = 8, 0.999                                            # MMF
 ARSEL_MAX_CAND = 9                                                         # MMF_ARSEL_MAX_CAND
 DIFF_MAX = 2                                                               # MMF_DIFF_MAX
 MA_MAX, HR_LONG_MAX, HR_PIVOT_TOL = 4, 32, 1e-5                            # MMF_MA_MAX, MMF_HR_LONG_MAX, MMF_HR_PIVOT_TOL
+ARMASEL_MAX_PQ = 32                                                        # MMF_ARMASEL_MAX_PQ
 DT_F32, DT_I16, DT_U16, DT_I32 = 0, 1, 2, 3
 INT_DTYPES = {"int16": DT_I16, "uint16": DT_U16, "int32": DT_I32}          # series element types besides float32
 INT_MISSING = {"int16": -32768, "uint16": 65535, "int32": -2147483648}     # the value that means "missing" in each
@@ -32,7 +33,7 @@ EXPORTS = (
     "mmf_set_stream", "mmf_synchronize", "mmf_plan_design", "mmf_pin_scratch", "mmf_get_whitening",
     "mmf_fit_forecast_f32", "mmf_fit_forecast_int", "mmf_fit_forecast_se_f32", "mmf_fit_forecast_ar_f32",
     "mmf_fit_select_ar_f32", "mmf_plan_arima", "mmf_fit_forecast_arima_f32", "mmf_fit_select_arima_f32",
-    "mmf_fit_forecast_arma_f32",
+    "mmf_fit_forecast_arma_f32", "mmf_fit_select_arma_f32",
     "mmf_plan_calendars", "mmf_fit_forecast_ragged_f32",
     "mmf_plan_backtest", "mmf_backtest_f32",
     "mmf_fit_forecast_bcast_f32", "mmf_fit_select_forecast_f32", "mmf_pack_hash_utf8", "mmf_pack_hash_i32",
@@ -135,6 +136,12 @@ def load() -> C.CDLL:
         C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int64,
         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
         C.POINTER(MmfStats),
+    ]
+    lib.mmf_fit_select_arma_f32.argtypes = [
+        C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.POINTER(C.c_int32), C.c_int32,
+        C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+        C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(MmfStats),
     ]
     lib.mmf_plan_calendars.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_int32, C.c_int32]

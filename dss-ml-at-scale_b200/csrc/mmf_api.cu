@@ -218,6 +218,7 @@ struct mmf_ctx {
   float* d_z = nullptr;  size_t z_cap_bytes = 0;           // ARIMA calls: z' of one slab, round4(t_fit - d) per row
   ArimaSelBest* d_asel_best = nullptr;  size_t asel_best_cap = 0;   // (p, d) selection, per slab: running best,
   int32_t* d_asel_status = nullptr;  size_t asel_status_cap = 0;    // and the status of the fit of the current d
+  float* d_hsel_q0 = nullptr;  size_t hsel_q0_cap = 0;     // (p, d, q) selection, per slab: the q = 0 scores
   float* d_bt_mom = nullptr;  size_t bt_mom_cap = 0;   // backtest scratch, per slab: moments at the earlier origins,
   SolveRec* d_bt_recs = nullptr;  size_t bt_recs_cap = 0;   // [K][slab] records, [K][slab] work lists,
   int64_t* d_bt_rows = nullptr;  size_t bt_rows_cap = 0;
@@ -518,14 +519,16 @@ int build_multi(MultiPlan& m, const double* X_all, int32_t n_cal, const int32_t*
 // ARIMA calls (arima != nullptr, with ar): y / ld_y are the slab's levels; diff_kernel writes z' into the context's
 // scratch first, and the fit passes and arima_kernel read z' with `plan` = the plan of D_d.  (p, d) selection calls
 // (asel != nullptr) run this once per listed d and end in arima_select_kernel; their d = 0 pass (arima->d == 0) fits y
-// itself with the mmf_plan_design plan.  ARMA calls (arma != nullptr, with ar) run arma_kernel behind ar_kernel (d = 0,
-// arima == nullptr) or arima_kernel.
+// itself with the mmf_plan_design plan; (p, d, q) selection calls (hsel != nullptr, with asel) add arma_select_kernel
+// behind it.  ARMA calls (arma != nullptr, with ar) run arma_kernel behind ar_kernel (d = 0, arima == nullptr) or
+// arima_kernel.
 int run_device_slab(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, int64_t ld_y, int32_t pred_start,
                     int32_t n_pred, float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s,
                     int* launches, int* kernel_used, float* const* out_more, int n_out, int multimem,
                     const SelectArgs* sel, const SeArgs* se = nullptr, const ArArgs* ar = nullptr,
                     const ArSelArgs* arsel = nullptr, const ArimaArgs* arima = nullptr,
-                    const ArimaSelArgs* asel = nullptr, const ArmaArgs* arma = nullptr) {
+                    const ArimaSelArgs* asel = nullptr, const ArmaArgs* arma = nullptr,
+                    const ArmaSelArgs* hsel = nullptr) {
   const DesignView d = view_of(plan);
   ArimaArgs ma{};
   if (arima != nullptr) {
@@ -635,6 +638,10 @@ int run_device_slab(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, i
            : arima != nullptr ? launch_arima(d, a, *ar, ma, s)
            : arsel != nullptr ? launch_ar_select(d, a, *ar, *arsel, s) : launch_ar(d, a, *ar, s));
     ++*launches;
+    if (hsel != nullptr) {
+      CU_TRY(launch_arma_select(d, a, *ar, ma, *asel, *hsel, s));
+      ++*launches;
+    }
     if (arma != nullptr) {
       ArimaArgs mh = ma;
       if (arima == nullptr) { mh.y = a.y; mh.ld_y = a.ld_y; mh.t_fit = d.t_fit; mh.d = 0; }
@@ -840,7 +847,7 @@ int mmf_destroy(mmf_ctx* ctx) {
   free_bt(ctx->bt);
   free_arima(ctx->arima);
   cudaFree(ctx->d_z);
-  cudaFree(ctx->d_asel_best); cudaFree(ctx->d_asel_status);
+  cudaFree(ctx->d_asel_best); cudaFree(ctx->d_asel_status); cudaFree(ctx->d_hsel_q0);
   cudaFree(ctx->d_bt_mom); cudaFree(ctx->d_bt_recs); cudaFree(ctx->d_bt_rows); cudaFree(ctx->d_bt_ctr); cudaFree(ctx->d_bt_pred);
   for (int i = 0; i < NBUF; ++i) {
     Staging& s = ctx->st[i];
@@ -1564,13 +1571,16 @@ int mmf_fit_forecast_arma_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t l
   return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, &ma, stats, &hr);
 }
 
-// ---- (p, d) selection by hold-out MSE on levels (DESIGN.md section 2 item 12) -------------------------------------------
-int mmf_fit_select_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
-                             const int32_t* orders, int32_t n_orders, const int32_t* diffs, int32_t n_diffs,
-                             int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out,
-                             int32_t* out_choice_p, int32_t* out_choice_d, float* out_mse, float* out_cand_mse,
-                             float* out_phi, int32_t* out_order, float* out_sigma, int32_t* out_status,
-                             mmf_stats* stats) {
+// ---- (p, d) and (p, d, q) selection by hold-out MSE on levels (DESIGN.md section 2 items 12, 14) ------------------------
+// The MA arguments (mas .. out_ma_order) are those of mmf_fit_select_arma_f32 (with_q); mmf_fit_select_arima_f32 passes
+// none and launches no arma_select_kernel.
+static int select_arima_call(mmf_ctx* ctx, const char* name, bool with_q, const float* y, int64_t n, int64_t ld_y,
+                             int32_t n_hold, const int32_t* orders, int32_t n_orders, const int32_t* diffs,
+                             int32_t n_diffs, const int32_t* mas, int32_t n_mas, int32_t long_order, int32_t pred_start,
+                             int32_t n_pred, float* out_pred, int64_t ld_out, int32_t* out_choice_p,
+                             int32_t* out_choice_d, int32_t* out_choice_q, float* out_mse, float* out_cand_mse,
+                             float* out_phi, float* out_theta, int32_t* out_order, int32_t* out_ma_order,
+                             float* out_sigma, int32_t* out_status, mmf_stats* stats) {
   if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
   GrowScope grow_scope(ctx);
   if (n < 0) return fail(MMF_E_INVALID, "n < 0");
@@ -1587,6 +1597,20 @@ int mmf_fit_select_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld
     if (diffs[j] < 0 || diffs[j] > MMF_DIFF_MAX || (j > 0 && diffs[j] <= diffs[j - 1]))
       return fail(MMF_E_INVALID, "diffs must be ascending and distinct in [0,%d] (diffs[%d]=%d)", MMF_DIFF_MAX, j,
                   diffs[j]);
+  if (with_q) {
+    if (!mas || n_mas < 1 || n_mas > MMF_MA_MAX + 1)
+      return fail(MMF_E_INVALID, "n_mas=%d outside [1,%d] (or mas is NULL)", n_mas, MMF_MA_MAX + 1);
+    if (mas[0] != 0) return fail(MMF_E_INVALID, "mas[0]=%d: the MA orders must start with 0", mas[0]);
+    for (int j = 1; j < n_mas; ++j)
+      if (mas[j] > MMF_MA_MAX || mas[j] <= mas[j - 1])
+        return fail(MMF_E_INVALID, "mas must be ascending and distinct in [0,%d] (mas[%d]=%d)", MMF_MA_MAX, j, mas[j]);
+    if (n_orders * (n_mas - 1) > MMF_ARMASEL_MAX_PQ)
+      return fail(MMF_E_INVALID, "%d x %d (p, q >= 1) pairs above MMF_ARMASEL_MAX_PQ=%d", n_orders, n_mas - 1,
+                  MMF_ARMASEL_MAX_PQ);
+    const int32_t lmin = std::max(orders[n_orders - 1], mas[n_mas - 1]);
+    if (long_order != 0 && (long_order < lmin || long_order > MMF_HR_LONG_MAX))
+      return fail(MMF_E_INVALID, "long_order=%d outside {0} and [%d,%d]", long_order, lmin, MMF_HR_LONG_MAX);
+  }
   // a listed d = 0 fits y with the mmf_plan_design plan; a listed d >= 1 fits z' with the mmf_plan_arima plan
   const bool use_plain = diffs[0] == 0, use_arima = diffs[n_diffs - 1] >= 1;
   const Plan& pl = ctx->plan;
@@ -1618,8 +1642,30 @@ int mmf_fit_select_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld
       (out_choice_d && !is_device_ptr(out_choice_d)) || (out_mse && !is_device_ptr(out_mse)) ||
       (out_cand_mse && !is_device_ptr(out_cand_mse)) || (out_phi && !is_device_ptr(out_phi)) ||
       (out_order && !is_device_ptr(out_order)) || (out_sigma && !is_device_ptr(out_sigma)) ||
-      (out_status && !is_device_ptr(out_status)))
-    return fail(MMF_E_UNSUPPORTED, "mmf_fit_select_arima_f32 takes device buffers only");
+      (out_status && !is_device_ptr(out_status)) || (out_choice_q && !is_device_ptr(out_choice_q)) ||
+      (out_theta && !is_device_ptr(out_theta)) || (out_ma_order && !is_device_ptr(out_ma_order)))
+    return fail(MMF_E_UNSUPPORTED, "%s takes device buffers only", name);
+
+  // (p, d, q) selection: the (p, q >= 1) pairs q-major, and their row sets R(q, L = max(p, q)) in order of appearance
+  ArmaSelArgs hs{};
+  if (with_q) {
+    hs.n_mas = n_mas;
+    for (int qi = 1; qi < n_mas; ++qi)
+      for (int j = 0; j < n_orders; ++j) {
+        const int p = orders[j], q = mas[qi], L = std::max(p, q);
+        int r = 0;
+        while (r < hs.n_rs && !(hs.rs_q[r] == q && hs.rs_L[r] == L)) ++r;
+        if (r == hs.n_rs) { hs.rs_q[r] = q; hs.rs_L[r] = L; hs.rs_pmax[r] = 0; ++hs.n_rs; }
+        hs.rs_pmax[r] = std::max(hs.rs_pmax[r], p);
+        const int c = hs.n_pq++;
+        hs.pq_p[c] = p; hs.pq_q[c] = q; hs.pq_j[c] = j; hs.pq_qi[c] = qi; hs.pq_rs[c] = r;
+      }
+    for (int r = 0; r < hs.n_rs; ++r) {
+      const int nd = hs.rs_pmax[r] + hs.rs_q[r] + 1;
+      hs.rs_off[r] = hs.n_ent;
+      hs.n_ent += nd * (nd + 1) / 2 - 1;
+    }
+  }
 
   // slabs as the plain fit of the level rows would cut them; per slab, one fit and one arima_select_kernel per listed d
   const Plan& level_plan = use_plain ? pl : ap.diff[0];
@@ -1627,6 +1673,8 @@ int mmf_fit_select_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld
   const int64_t n_slabs = (n + slab - 1) / slab;
   int rc = grow((void**)&ctx->d_asel_best, &ctx->asel_best_cap, (size_t)slab * sizeof(ArimaSelBest));
   if (rc == MMF_OK) rc = grow((void**)&ctx->d_asel_status, &ctx->asel_status_cap, (size_t)slab * sizeof(int32_t));
+  if (rc == MMF_OK && with_q)
+    rc = grow((void**)&ctx->d_hsel_q0, &ctx->hsel_q0_cap, (size_t)slab * n_diffs * n_orders * sizeof(float));
   if (rc != MMF_OK) return rc;
   uint32_t* slab_pending = nullptr;        // rows each fit handed to the general pass (stats)
   if (stats) {
@@ -1663,9 +1711,25 @@ int mmf_fit_select_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld
       sel.mse = out_mse ? out_mse + off : nullptr;
       sel.cand_mse = out_cand_mse ? out_cand_mse + off * n_diffs * n_orders : nullptr;
       sel.status = out_status ? out_status + off : nullptr;
+      ArmaSelArgs hsd = hs;
+      if (with_q) {
+        // arima_select_kernel's scores go to scratch: arma_select_kernel copies them into the q = 0 slice
+        sel.cand_mse = ctx->d_hsel_q0;
+        hsd.cand_q0 = ctx->d_hsel_q0;
+        hsd.cand_mse = out_cand_mse ? out_cand_mse + off * n_diffs * n_mas * n_orders : nullptr;
+        hsd.choice_q = out_choice_q ? out_choice_q + off : nullptr;
+        hsd.theta = out_theta ? out_theta + off * MMF_MA_MAX : nullptr;
+        hsd.ma_order = out_ma_order ? out_ma_order + off : nullptr;
+        hsd.m = long_order;
+        if (long_order == 0) {             // min(32, max(2 max(orders, mas), floor(ln(t_fit - d)^2)))
+          const double lt = std::log((double)(T - dd));
+          const int32_t lmax = std::max(orders[n_orders - 1], mas[n_mas - 1]);
+          hsd.m = std::min<int32_t>(MMF_HR_LONG_MAX, std::max<int32_t>(2 * lmax, (int32_t)std::floor(lt * lt)));
+        }
+      }
       rc = run_device_slab(ctx, plan, y + off * ld_y, m, ld_y, pred_start, n_pred, out_pred + off * ld_out, ld_out,
                            nullptr, ctx->d_asel_status, s, &launches, &kernel_used, nullptr, 1, 0, nullptr, nullptr,
-                           &ar, nullptr, &ma, &sel);
+                           &ar, nullptr, &ma, &sel, nullptr, with_q ? &hsd : nullptr);
       if (rc != MMF_OK) return rc;
       if (slab_pending != nullptr) {
         uint32_t* dst = slab_pending + i * n_diffs + k;
@@ -1690,6 +1754,30 @@ int mmf_fit_select_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld
     stats->kernel_used = kernel_used;
   }
   return MMF_OK;
+}
+
+int mmf_fit_select_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
+                             const int32_t* orders, int32_t n_orders, const int32_t* diffs, int32_t n_diffs,
+                             int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out,
+                             int32_t* out_choice_p, int32_t* out_choice_d, float* out_mse, float* out_cand_mse,
+                             float* out_phi, int32_t* out_order, float* out_sigma, int32_t* out_status,
+                             mmf_stats* stats) {
+  return select_arima_call(ctx, "mmf_fit_select_arima_f32", false, y, n, ld_y, n_hold, orders, n_orders, diffs, n_diffs,
+                           nullptr, 0, 0, pred_start, n_pred, out_pred, ld_out, out_choice_p, out_choice_d, nullptr,
+                           out_mse, out_cand_mse, out_phi, nullptr, out_order, nullptr, out_sigma, out_status, stats);
+}
+
+int mmf_fit_select_arma_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
+                            const int32_t* orders, int32_t n_orders, const int32_t* diffs, int32_t n_diffs,
+                            const int32_t* mas, int32_t n_mas, int32_t long_order, int32_t pred_start, int32_t n_pred,
+                            float* out_pred, int64_t ld_out, int32_t* out_choice_p, int32_t* out_choice_d,
+                            int32_t* out_choice_q, float* out_mse, float* out_cand_mse, float* out_phi,
+                            float* out_theta, int32_t* out_order, int32_t* out_ma_order, float* out_sigma,
+                            int32_t* out_status, mmf_stats* stats) {
+  return select_arima_call(ctx, "mmf_fit_select_arma_f32", true, y, n, ld_y, n_hold, orders, n_orders, diffs, n_diffs, mas,
+                           n_mas, long_order, pred_start, n_pred, out_pred, ld_out, out_choice_p, out_choice_d,
+                           out_choice_q, out_mse, out_cand_mse, out_phi, out_theta, out_order, out_ma_order, out_sigma,
+                           out_status, stats);
 }
 
 // ---- ragged batches: many calendars, one launch ------------------------------------------------------------------

@@ -295,6 +295,33 @@ struct ArmaArgs {
 cudaError_t launch_arma(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
                         const ArmaArgs& hr, cudaStream_t s);
 
+// per-series (p, d, q) selection by hold-out MSE on levels (arma_select.cu, DESIGN.md section 2 item 14): one launch per
+// listed d, right behind that d's arima_select_kernel (same fit, z', gamma / c and running best), for the q >= 1 blocks.
+// Candidate lane c is the pair (pq_p[c], pq_q[c]), q-major; its normal equations are those of row set pq_rs[c], the rows
+// R(q, L = max(p, q)), shared by every candidate with the same (q, L).
+struct ArmaSelArgs {
+  int32_t m;                                        // long AR order of this d (resolved)
+  int32_t n_mas;                                    // listed MA orders, mas[0] = 0
+  int32_t n_pq;                                     // candidate lanes: the (p, q >= 1) pairs (0: the q outputs only)
+  int32_t n_rs;                                     // distinct row sets
+  int32_t n_ent;                                    // normal-equation entries of all row sets
+  int32_t pq_p[MMF_ARMASEL_MAX_PQ], pq_q[MMF_ARMASEL_MAX_PQ];
+  int32_t pq_j[MMF_ARMASEL_MAX_PQ];                 // index of p in the orders
+  int32_t pq_qi[MMF_ARMASEL_MAX_PQ];                // index of q in the MA orders
+  int32_t pq_rs[MMF_ARMASEL_MAX_PQ];
+  int32_t rs_q[MMF_ARMASEL_MAX_PQ], rs_L[MMF_ARMASEL_MAX_PQ];
+  int32_t rs_pmax[MMF_ARMASEL_MAX_PQ];              // largest p of the row set's candidates: its e lags
+  int32_t rs_off[MMF_ARMASEL_MAX_PQ];               // first entry; (pmax + q + 1)(pmax + q + 2) / 2 - 1 entries
+  const float* cand_q0;                             // [n][n_diffs][n_orders]: arima_select_kernel's scores (scratch)
+  float* cand_mse;                                  // nullable [n][n_diffs][n_mas][n_orders]
+  int32_t* choice_q;                                // nullable [n]: the chosen q (-1: no eligible candidate)
+  float* theta;                                     // nullable [n][MMF_MA_MAX]
+  int32_t* ma_order;                                // nullable [n]
+};
+size_t arma_select_smem_bytes(int n_ent);          // dynamic shared memory of a launch
+cudaError_t launch_arma_select(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
+                               const ArimaSelArgs& sel, const ArmaSelArgs& hs, cudaStream_t s);
+
 // integer series -> float32 staging rows, sentinel -> NaN (widen.cu); dtype = MMF_DT_I16 / U16 / I32
 cudaError_t launch_widen(int dtype, const void* src, int64_t ld_src, float* dst, int64_t ld_dst, int64_t n, int32_t t,
                          int sm_count, cudaStream_t s);

@@ -725,6 +725,69 @@ class ForecastEngine:
                                  st.kernel_launches, {N.KERNEL_WARP: "warp", N.KERNEL_TC: "tc"}.get(st.kernel_used, "?"))
         return res
 
+    def fit_select_arma(self, y, n_hold: int, orders=(0, 1, 2, 3, 4), diffs=(0, 1, 2), mas=(0, 1, 2, 3, 4),
+                        pred_start: int = 0, n_pred: int | None = None, long_order: int = 0, want_stats: bool = False):
+        """Regression with ARIMA(p, d, q) errors, (p, d, q) chosen per series by hold-out MSE on levels
+        (``mmf_fit_select_arma_f32``, DESIGN.md section 2 item 14).  The candidates are every triple of ``orders``,
+        ``diffs`` and ``mas`` (ascending, distinct, 0 .. MMF_MA_MAX, ``mas[0] == 0``), d, then q, then p ascending:
+        (p, d, 0) is ``fit_select_arima``'s candidate (p, d), (p, d, q >= 1) is ``fit_forecast_arma(p, q, d,
+        long_order=m_d)`` with one long order per d (``long_order``, or 0 for min(32, max(2 max(orders, mas),
+        floor(ln(t_fit - d)^2)))).  At most 32 pairs (p, q >= 1).  Scores, eligibility and the first-minimum choice are
+        ``fit_select_arima``'s; a q >= 1 candidate that fails the Hannan-Rissanen gate scores as (p, d, 0) and never
+        wins.  Returns ``fit_select_arima``'s dict plus ``choice_q``, ``theta`` and ``ma_order``; ``cand_mse[i, k, l,
+        j]`` is the score of ``(orders[j], diffs[k], mas[l])``.  With ``mas=(0,)`` the call is ``fit_select_arima``."""
+        import torch
+        orders = [int(m) for m in orders]
+        diffs = [int(d) for d in diffs]
+        mas = [int(q) for q in mas]
+        if any(d >= 1 for d in diffs):
+            if getattr(self, "_arima", None) is None:
+                raise RuntimeError("plan_arima() (or plan_calendar(..., max_diff=d)) must be called first")
+            t_fit, n_rows = self._arima[0], self._arima[1]
+        else:
+            if self.t_fit is None:
+                raise RuntimeError("plan()/plan_calendar() must be called first")
+            t_fit, n_rows = self.t_fit, self.n_rows
+        yp, n, t_have, ld_y = _describe(y, "y")
+        if not (_is_torch(y) and y.is_cuda and y.dtype == torch.float32) or t_have < t_fit + int(n_hold):
+            raise ValueError(f"y must be a float32 CUDA tensor with at least t_fit + n_hold={t_fit + int(n_hold)} "
+                             "columns")
+        if n_pred is None:
+            n_pred = n_rows - int(pred_start)
+        self.set_stream(torch.cuda.current_stream(y.device).cuda_stream)
+        dev = y.device
+        out = torch.empty((n, n_pred), device=dev, dtype=torch.float32)
+        choice_p = torch.empty(n, device=dev, dtype=torch.int32)
+        choice_d = torch.empty(n, device=dev, dtype=torch.int32)
+        choice_q = torch.empty(n, device=dev, dtype=torch.int32)
+        mse = torch.empty(n, device=dev, dtype=torch.float32)
+        cand_mse = torch.empty((n, len(diffs), len(mas), len(orders)), device=dev, dtype=torch.float32)
+        phi = torch.empty((n, N.AR_MAX), device=dev, dtype=torch.float32)
+        theta = torch.empty((n, N.MA_MAX), device=dev, dtype=torch.float32)
+        order = torch.empty(n, device=dev, dtype=torch.int32)
+        ma_order = torch.empty(n, device=dev, dtype=torch.int32)
+        sigma = torch.empty(n, device=dev, dtype=torch.float32)
+        status = torch.empty(n, device=dev, dtype=torch.int32)
+        cand = (C.c_int32 * max(len(orders), 1))(*orders)
+        dl = (C.c_int32 * max(len(diffs), 1))(*diffs)
+        ql = (C.c_int32 * max(len(mas), 1))(*mas)
+        st = N.MmfStats() if want_stats else None
+        N.check(self._lib.mmf_fit_select_arma_f32(self._h, yp, n, ld_y, int(n_hold), cand, len(orders), dl, len(diffs),
+                                                  ql, len(mas), int(long_order), int(pred_start), int(n_pred),
+                                                  out.data_ptr(), out.stride(0), choice_p.data_ptr(),
+                                                  choice_d.data_ptr(), choice_q.data_ptr(), mse.data_ptr(),
+                                                  cand_mse.data_ptr(), phi.data_ptr(), theta.data_ptr(),
+                                                  order.data_ptr(), ma_order.data_ptr(), sigma.data_ptr(),
+                                                  status.data_ptr(), C.byref(st) if st is not None else None))
+        res = {"pred": out, "choice_p": choice_p, "choice_d": choice_d, "choice_q": choice_q, "mse": mse,
+               "cand_mse": cand_mse, "phi": phi, "theta": theta, "order": order, "ma_order": ma_order, "sigma": sigma,
+               "status": status}
+        if st is not None:
+            self.launches += st.kernel_launches
+            res["stats"] = Stats(st.kernel_ms, st.total_ms, st.n_series, st.n_pending, st.h2d_bytes, st.d2h_bytes,
+                                 st.kernel_launches, {N.KERNEL_WARP: "warp", N.KERNEL_TC: "tc"}.get(st.kernel_used, "?"))
+        return res
+
     def capture(self, y, pred_start: int, n_pred: int, out=None, status=None):
         """Record one device-resident ``fit_forecast`` call as a CUDA graph.  Small batches are launch-bound (three
         kernel launches plus the Python/ctypes hop cost more than the kernels themselves): ``graph.replay()``

@@ -23,7 +23,7 @@ import pandas as pd
 
 from . import design as D
 from .engine import ForecastEngine, alloc_packed, default_engine
-from ._native import AR_MAX, DIFF_MAX, MA_MAX
+from ._native import AR_MAX, ARMASEL_MAX_PQ, DIFF_MAX, MA_MAX
 
 FORECAST_HORIZON = 40                      # 02:341
 DEFAULT_KEYS = ("Product", "SKU")          # 02:526
@@ -347,7 +347,9 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
     ``diff``: regression with ARIMA(ar, diff, 0) errors (``fit_forecast_arima``), one call per calendar bucket; a tuple
     of differencing orders (with ``ar`` a tuple of orders) chooses (p, d) per series by hold-out MSE over the last
     ``horizon`` rows (``fit_select_arima``).
-    ``ma``: regression with ARIMA(ar, diff or 0, ma) errors (``fit_forecast_arma``), one call per calendar bucket."""
+    ``ma``: regression with ARIMA(ar, diff or 0, ma) errors (``fit_forecast_arma``), one call per calendar bucket; a
+    tuple of MA orders (with ``ar`` and ``diff`` tuples) chooses (p, d, q) per series by hold-out MSE over the last
+    ``horizon`` rows (``fit_select_arma``)."""
     if interval and select is not None:
         raise ValueError("interval= is not offered with select= (model selection returns point forecasts)")
     t_fit_min = min((b.t_len - (horizon if mode == "holdout" else 0)) for b in buckets) if buckets else 0
@@ -362,7 +364,11 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
             out_days, pred_start, n_pred = eng.plan_calendar(b.start, b.t_len, freq, horizon, mode, design,
                                                              max_diff=max(diff) if isinstance(diff, tuple) else diff)
         se = None
-        if ma is not None:
+        if isinstance(ma, tuple):
+            from .engine import device_packed
+            yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
+            pred = _host(eng.fit_select_arma(yd, horizon, ar, diff, ma, pred_start, n_pred)["pred"])
+        elif ma is not None:
             from .engine import device_packed
             yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
             pred = _host(eng.fit_forecast_arma(yd, ar, ma, diff or 0, pred_start, n_pred)["pred"])
@@ -462,13 +468,33 @@ def _diff_order(diff, ar, select, interval, mode="holdout"):
     return int(diff)
 
 
-def _arma_orders(ma, ar, diff, select, interval):
+def _arma_orders(ma, ar, diff, select, interval, mode="holdout"):
     """validated (ar, diff, ma) of ``ma=``: one MA order in 1..4 with one AR order in 0..8 and ``diff`` None (d = 0) or
-    one differencing order in 1..2.  Choosing q is not built, so a sequence of MA orders is refused."""
+    one differencing order in 1..2.  A sequence of MA orders (ascending, distinct, in 0..4, starting with 0) chooses
+    (p, d, q) per series: it needs a sequence of AR orders, ``diff`` None (d = 0) or a sequence of differencing orders,
+    and ``mode='holdout'``; the result is then three tuples."""
     if select is not None or interval is not None:
         raise ValueError("ma= is not offered with select= or interval= (ARMA forecasts come without either)")
     if isinstance(ma, (list, tuple, np.ndarray)):
-        raise ValueError(f"ma= takes one MA order: choosing q per series is not built, got ma={ma!r}")
+        mas = list(ma)
+        if (not mas or any(isinstance(q, bool) or not isinstance(q, (int, np.integer)) or not 0 <= int(q) <= MA_MAX
+                           for q in mas)):
+            raise ValueError(f"ma= candidate MA orders must be integers in [0, {MA_MAX}], got ma={ma!r}")
+        mas = [int(q) for q in mas]
+        if mas[0] != 0 or any(b <= a for a, b in zip(mas, mas[1:])):
+            raise ValueError(f"ma= candidate MA orders must be ascending and distinct and start with 0, got ma={ma!r}")
+        if not isinstance(ar, (list, tuple, np.ndarray)):
+            raise ValueError(f"ma= with candidate MA orders needs candidate AR orders ar=(...) in [0, {AR_MAX}], "
+                             f"got ar={ar!r}")
+        if diff is not None and not isinstance(diff, (list, tuple, np.ndarray)):
+            raise ValueError(f"ma= with candidate MA orders needs diff=None or candidate differencing orders, "
+                             f"got diff={diff!r}")
+        diffs = _diff_order((0,) if diff is None else diff, ar, select, interval, mode)
+        orders = _ar_orders_for(diffs, ar, select, interval, mode)
+        if len(orders) * (len(mas) - 1) > ARMASEL_MAX_PQ:
+            raise ValueError(f"ar= and ma= give {len(orders) * (len(mas) - 1)} (p, q >= 1) pairs, more than "
+                             f"{ARMASEL_MAX_PQ}")
+        return tuple(orders), diffs, tuple(mas)
     if isinstance(ma, bool) or not isinstance(ma, (int, np.integer)) or not 1 <= int(ma) <= MA_MAX:
         raise ValueError(f"ma must be an MA order in [1, {MA_MAX}], got {ma!r}")
     if isinstance(ar, bool) or not isinstance(ar, (int, np.integer)) or not 0 <= int(ar) <= AR_MAX:
@@ -644,7 +670,12 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     ARIMA(p, d, q) errors by Hannan-Rissanen (``ForecastEngine.fit_forecast_arma``, DESIGN.md section 2 item 13);
     ``ar=1, diff=2, ma=1`` is the reference notebook's order.  A series whose estimate fails the gate gets the
     ARIMA(p, d, 0) forecast.  One call per calendar bucket, schema unchanged; ``ma=None`` leaves everything as it was.
-    Not offered with ``select=`` or ``interval=``, and a sequence of MA orders is refused (choosing q is not built).
+    Not offered with ``select=`` or ``interval=``.
+    ``ma=(0, 1, 2, 3, 4)`` (ascending distinct orders in 0..4 starting with 0) with ``ar=(0, 1, 2, 3, 4)`` and
+    ``diff=(0, 1, 2)`` (or None for d = 0) chooses each series' (p, d, q) by the MSE of its dynamic level forecast over
+    the last ``horizon`` dates (``ForecastEngine.fit_select_arma``, DESIGN.md section 2 item 14): the reference's search
+    space, searched exhaustively.  At most 32 pairs (p, q >= 1).  Holdout mode only, one call per calendar bucket,
+    schema unchanged.
     """
     eng = engine or default_engine()
     keys = list(keys)
@@ -654,7 +685,7 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
         diff = _diff_order(diff, ar, select, interval, mode)
         ar = _ar_orders_for(diff, ar, select, interval, mode)
     else:
-        ar, diff, ma = _arma_orders(ma, ar, diff, select, interval)
+        ar, diff, ma = _arma_orders(ma, ar, diff, select, interval, mode)
     if pack == "host" and select is None and z is None and ar is None and isinstance(pdf, pd.DataFrame):
         one = _single_group_fast(pdf, keys, date_col, value_col, freq, horizon, mode, design, eng, null_keys_on_gaps)
         if one is not None:
@@ -759,7 +790,8 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     in and expanded from a dictionary on the way out, dates and values are NumPy views of Arrow buffers.
     ``interval=level`` adds the ``{value}_Lower`` / ``{value}_Upper`` columns of ``forecast_groups`` (schema:
     ``tuning_schema(..., interval=True)``).  ``ar=p`` fits regression with AR(p) errors and ``ar=(0, 1, 2, 3, 4)`` chooses the order per series, as in
-    ``forecast_groups``; ``diff=d`` with ``ar=p`` fits ARIMA(p, d, 0) errors as there, and ``ma=q`` ARIMA(p, d, q)."""
+    ``forecast_groups``; ``diff=d`` with ``ar=p`` fits ARIMA(p, d, 0) errors as there, and ``ma=q`` ARIMA(p, d, q); tuples of ``ar``, ``diff`` and
+    ``ma`` choose (p, d, q) per series."""
     import pyarrow as pa
 
     if isinstance(table, pa.RecordBatch):
@@ -771,7 +803,7 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
         diff = _diff_order(diff, ar, select, interval, mode)
         ar = _ar_orders_for(diff, ar, select, interval, mode)
     else:
-        ar, diff, ma = _arma_orders(ma, ar, diff, select, interval)
+        ar, diff, ma = _arma_orders(ma, ar, diff, select, interval, mode)
     schema = tuning_schema(keys, date_col, value_col, interval=z is not None)
     buckets = _buckets_for(table, keys, date_col, value_col, freq, pack, eng)
     parts, lengths = [], []

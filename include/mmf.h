@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define MMF_VERSION 109          /* 0.1.9 */
+#define MMF_VERSION 110          /* 0.1.10 */
 #define MMF_P 16                 /* design columns (zero-pad narrower designs) */
 #define MMF_PIVOT_TOL 1e-3f      /* per-series relative Cholesky pivot threshold */
 #define MMF_CAL_TOL 1e-10        /* aliasing threshold on the float64 calendar Gram */
@@ -45,6 +45,7 @@ extern "C" {
 #define MMF_MA_MAX 4             /* largest MA order of mmf_fit_forecast_arma_f32 */
 #define MMF_HR_LONG_MAX 32       /* largest long AR order of the Hannan-Rissanen step 1 (one lag per lane of a warp) */
 #define MMF_HR_PIVOT_TOL 1e-5    /* a Hannan-Rissanen Cholesky pivot must exceed this x its Gram diagonal */
+#define MMF_ARMASEL_MAX_PQ 32    /* (p, q >= 1) candidate pairs per mmf_fit_select_arma_f32 call (one per lane of a warp) */
 
 /* return codes */
 #define MMF_OK 0
@@ -347,13 +348,47 @@ int mmf_fit_forecast_arma_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t l
  * fits of every listed d), mmf_config.kernel and assume_finite honoured, refused arguments write nothing.  Scratch: per
  * slab, z' as mmf_fit_forecast_arima_f32, 20 B per row.
  * replaces: the reference's per-group tuning loop over p and d (02:435-488, search space 02:461-465) as an exhaustive
- * search over (p, d) with q = 0, not TPE over (p, d, q). */
+ * search over (p, d) with q = 0; mmf_fit_select_arma_f32 adds q. */
 int mmf_fit_select_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
                              const int32_t* orders, int32_t n_orders, const int32_t* diffs, int32_t n_diffs,
                              int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out,
                              int32_t* out_choice_p, int32_t* out_choice_d, float* out_mse,
                              float* out_cand_mse /* [n][n_diffs][n_orders] */, float* out_phi, int32_t* out_order,
                              float* out_sigma, int32_t* out_status, mmf_stats* stats);
+
+/* ---- (p, d, q) selection by hold-out MSE on levels (DESIGN.md section 2 item 14) -----------------------------------------
+ * mmf_fit_select_arma_f32: the arguments of mmf_fit_select_arima_f32, and mas [n_mas] (a host array of 1 .. MMF_MA_MAX + 1
+ * ascending distinct values in [0, MMF_MA_MAX], mas[0] = 0) and long_order.  The candidates are every triple (p, d, q),
+ * in list order d ascending, then q ascending, then p ascending: for each d the q = 0 block comes first and is
+ * mmf_fit_select_arima_f32's candidates.  At most MMF_ARMASEL_MAX_PQ pairs (p, q >= 1), n_orders x (n_mas - 1).
+ *   candidate (p, d, 0) is mmf_fit_select_arima_f32's candidate (p, d), its score bit-equal to that call's cand_mse;
+ *   candidate (p, d, q >= 1) is mmf_fit_forecast_arma_f32(p, d, q, long_order = m_d), with one long order per d and call:
+ *   m_d = long_order (max(orders, mas) <= long_order <= MMF_HR_LONG_MAX), or for long_order = 0
+ *   min(MMF_HR_LONG_MAX, max(2 max(orders, mas), floor(ln(t_fit - d)^2))).  This is the single call's default whenever
+ *   t_fit - d >= 55 (floor(ln(t_fit - d)^2) >= 16 >= 2 max(p, q) then); below that it may be a larger m.  A candidate that
+ *   fails the Hannan-Rissanen gate forecasts as (p, d, 0), so its score is (p, d, 0)'s bit for bit and, (p, d, 0) coming
+ *   first, it never wins;
+ *   score, eligibility and choice are mmf_fit_select_arima_f32's: the MSE on levels of the dynamic forecast from t_fit over
+ *   the held-out rows, summed in float64; eligible when the fit the candidate builds on is not empty; the first minimum
+ *   over the eligible candidates in list order.  A q >= 1 candidate wins only with a scored point: with none anywhere the
+ *   choice is mmf_fit_select_arima_f32's (the last eligible q = 0 candidate); (-1, -1, -1) when none is eligible.
+ * Outputs: a winner with q >= 1 gets its single call's pred, phi, theta, order, ma_order, sigma and status bit for bit; a
+ * winner with q = 0 gets mmf_fit_select_arima_f32's outputs bit for bit, with theta 0, ma_order 0 and choice_q 0.  With
+ * mas = (0) the call is mmf_fit_select_arima_f32 in every shared output.  y is read on [0, t_fit + n_hold) only, and
+ * held-out y enters no recursion and no level chain.  out_choice_q [n], out_theta [n][MMF_MA_MAX], out_ma_order [n] and
+ * out_cand_mse [n][n_diffs][n_mas][n_orders] are nullable, as is every output of mmf_fit_select_arima_f32 but out_pred.
+ * Otherwise the contract of mmf_fit_select_arima_f32 (plans, device buffers, ld_out, enqueue-only unless `stats`, refused
+ * arguments write nothing).  Scratch: per slab, that of mmf_fit_select_arima_f32 and 4 B per row and candidate (p, d, 0).
+ * replaces: the reference's per-group tuning loop over p, d and q (02:435-488, search space 02:461-465), exhaustively
+ * rather than by TPE. */
+int mmf_fit_select_arma_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
+                            const int32_t* orders, int32_t n_orders, const int32_t* diffs, int32_t n_diffs,
+                            const int32_t* mas, int32_t n_mas, int32_t long_order, int32_t pred_start, int32_t n_pred,
+                            float* out_pred, int64_t ld_out, int32_t* out_choice_p, int32_t* out_choice_d,
+                            int32_t* out_choice_q, float* out_mse,
+                            float* out_cand_mse /* [n][n_diffs][n_mas][n_orders] */, float* out_phi, float* out_theta,
+                            int32_t* out_order, int32_t* out_ma_order, float* out_sigma, int32_t* out_status,
+                            mmf_stats* stats);
 
 /* ---- ragged batches: groups on MANY calendars in one launch ---------------------------------------------
  * The reference re-indexes every group on its own calendar (sort_values + asfreq per group, 02:422-423), so one

@@ -1571,6 +1571,51 @@ int mmf_fit_forecast_arma_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t l
   return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, &ma, stats, &hr);
 }
 
+// ---- standard errors of the ARIMA-family forecasts (DESIGN.md section 2 item 15) ---------------------------------------
+int mmf_arima_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t t_fit, int32_t diff_order,
+                     const int32_t* diffs, const float* phi, const int32_t* order, const float* theta,
+                     const int32_t* ma_order, const float* sigma, int32_t pred_start, int32_t n_pred, float* out_se,
+                     int64_t ld_se, mmf_stats* stats) {
+  if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
+  GrowScope grow_scope(ctx);
+  if (n < 0) return fail(MMF_E_INVALID, "n < 0");
+  if (n > 0 && (!y || !phi || !order || !sigma || !out_se))
+    return fail(MMF_E_INVALID, "y, phi, order, sigma or out_se is NULL");
+  if ((theta == nullptr) != (ma_order == nullptr))
+    return fail(MMF_E_INVALID, "theta and ma_order must both be given or both be NULL");
+  if (!diffs && (diff_order < 0 || diff_order > MMF_DIFF_MAX))
+    return fail(MMF_E_INVALID, "diff_order=%d outside [0,%d]", diff_order, MMF_DIFF_MAX);
+  if (t_fit < 1) return fail(MMF_E_INVALID, "t_fit=%d < 1", t_fit);
+  if (ld_y < t_fit) return fail(MMF_E_INVALID, "ld_y=%lld < t_fit=%d", (long long)ld_y, t_fit);
+  if (n_pred < 1 || pred_start < 0 || (int64_t)pred_start + n_pred > INT32_MAX)
+    return fail(MMF_E_INVALID, "prediction rows [%d,%lld) outside [0,%d]", pred_start,
+                (long long)pred_start + n_pred, INT32_MAX);
+  if (ld_se < n_pred) return fail(MMF_E_INVALID, "ld_se=%lld < n_pred=%d", (long long)ld_se, n_pred);
+  if (stats) memset(stats, 0, sizeof(*stats));
+  if (n == 0) return MMF_OK;
+  CU_TRY(cudaSetDevice(ctx->device));
+  if (!is_device_ptr(y) || !is_device_ptr(phi) || !is_device_ptr(order) || !is_device_ptr(sigma) ||
+      !is_device_ptr(out_se) || (diffs && !is_device_ptr(diffs)) || (theta && !is_device_ptr(theta)) ||
+      (ma_order && !is_device_ptr(ma_order)))
+    return fail(MMF_E_UNSUPPORTED, "mmf_arima_se_f32 takes device buffers only");
+  ArimaSeArgs a{};
+  a.y = y; a.ld_y = ld_y; a.t_fit = t_fit; a.diff_order = diff_order; a.diffs = diffs;
+  a.phi = phi; a.order = order; a.theta = theta; a.ma_order = ma_order; a.sigma = sigma;
+  a.pred_start = pred_start; a.n_pred = n_pred; a.out = out_se; a.ld_se = ld_se; a.n = n;
+  if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, ctx->stream));
+  CU_TRY(launch_arima_se(a, ctx->sm_count, ctx->stream));
+  if (stats) {
+    CU_TRY(cudaEventRecord(ctx->ev_k1, ctx->stream));
+    CU_TRY(cudaEventSynchronize(ctx->ev_k1));
+    CU_TRY(cudaEventElapsedTime(&stats->kernel_ms, ctx->ev_k0, ctx->ev_k1));
+    stats->total_ms = stats->kernel_ms;
+    stats->n_series = n;
+    stats->kernel_launches = 1;
+    stats->kernel_used = MMF_KERNEL_WARP;
+  }
+  return MMF_OK;
+}
+
 // ---- (p, d) and (p, d, q) selection by hold-out MSE on levels (DESIGN.md section 2 items 12, 14) ------------------------
 // The MA arguments (mas .. out_ma_order) are those of mmf_fit_select_arma_f32 (with_q); mmf_fit_select_arima_f32 passes
 // none and launches no arma_select_kernel.

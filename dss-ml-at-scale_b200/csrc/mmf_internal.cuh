@@ -322,6 +322,25 @@ size_t arma_select_smem_bytes(int n_ent);          // dynamic shared memory of a
 cudaError_t launch_arma_select(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
                                const ArimaSelArgs& sel, const ArmaSelArgs& hs, cudaStream_t s);
 
+// standard errors of the ARIMA-family forecasts (arima_se.cu, DESIGN.md section 2 item 15): one warp per series, no plan
+struct ArimaSeArgs {
+  const float* y;                 // [n, ld_y] levels, read on [0, t_fit) for finiteness only
+  int64_t ld_y;
+  int32_t t_fit;
+  int32_t diff_order;             // d of every row when diffs is null
+  const int32_t* diffs;           // nullable [n]: per-row d
+  const float* phi;               // [n][MMF_AR_MAX]
+  const int32_t* order;           // [n]
+  const float* theta;             // nullable [n][MMF_MA_MAX] (with ma_order)
+  const int32_t* ma_order;        // nullable [n]: q = 0 when null
+  const float* sigma;             // [n]
+  int32_t pred_start, n_pred;
+  float* out;                     // [n, ld_se]
+  int64_t ld_se;
+  int64_t n;
+};
+cudaError_t launch_arima_se(const ArimaSeArgs& a, int sm_count, cudaStream_t s);
+
 // integer series -> float32 staging rows, sentinel -> NaN (widen.cu); dtype = MMF_DT_I16 / U16 / I32
 cudaError_t launch_widen(int dtype, const void* src, int64_t ld_src, float* dst, int64_t ld_dst, int64_t n, int32_t t,
                          int sm_count, cudaStream_t s);

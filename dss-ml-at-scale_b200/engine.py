@@ -498,7 +498,8 @@ class ForecastEngine:
                                  st.kernel_launches, {N.KERNEL_WARP: "warp", N.KERNEL_TC: "tc"}.get(st.kernel_used, "?"))
         return res
 
-    def fit_forecast_ar(self, y, ar_order: int, pred_start: int, n_pred: int, want_stats: bool = False):
+    def fit_forecast_ar(self, y, ar_order: int, pred_start: int, n_pred: int, want_stats: bool = False,
+                        want_se: bool = False):
         """Regression with AR(``ar_order``) errors (``mmf_fit_forecast_ar_f32``, DESIGN.md section 2 item 9): the plain
         fit, then Yule-Walker AR coefficients of each series' residuals.  ``y`` is a float32 CUDA tensor.  Returns
         ``{"pred", "phi", "order", "sigma", "status"}`` (torch tensors on y's device): ``pred[i, j]`` the one-step-ahead
@@ -523,6 +524,8 @@ class ForecastEngine:
                                                   sigma.data_ptr(), status.data_ptr(),
                                                   C.byref(st) if st is not None else None))
         res = {"pred": out, "phi": phi, "order": order, "sigma": sigma, "status": status}
+        if want_se:
+            self._add_se(res, y, self.t_fit, pred_start, n_pred, 0)
         if st is not None:
             self.launches += st.kernel_launches
             res["stats"] = Stats(st.kernel_ms, st.total_ms, st.n_series, st.n_pending, st.h2d_bytes, st.d2h_bytes,
@@ -539,7 +542,7 @@ class ForecastEngine:
         self._arima = (int(t_fit), int(X.shape[0]), int(max_diff))
 
     def fit_forecast_arima(self, y, ar_order: int, diff_order: int, pred_start: int, n_pred: int,
-                           want_stats: bool = False):
+                           want_stats: bool = False, want_se: bool = False):
         """Regression with ARIMA(``ar_order``, ``diff_order``, 0) errors (``mmf_fit_forecast_arima_f32``, DESIGN.md
         section 2 item 11): ``fit_forecast_ar`` on the differenced series and design, integrated back to levels.
         ``y`` is a float32 CUDA tensor of levels.  Returns ``{"pred", "phi", "order", "sigma", "status"}`` (torch tensors
@@ -565,6 +568,8 @@ class ForecastEngine:
                                                      phi.data_ptr(), order.data_ptr(), sigma.data_ptr(),
                                                      status.data_ptr(), C.byref(st) if st is not None else None))
         res = {"pred": out, "phi": phi, "order": order, "sigma": sigma, "status": status}
+        if want_se:
+            self._add_se(res, y, t_fit, pred_start, n_pred, int(diff_order))
         if st is not None:
             self.launches += st.kernel_launches
             res["stats"] = Stats(st.kernel_ms, st.total_ms, st.n_series, st.n_pending, st.h2d_bytes, st.d2h_bytes,
@@ -572,7 +577,8 @@ class ForecastEngine:
         return res
 
     def fit_forecast_arma(self, y, ar_order: int, ma_order: int, diff_order: int = 0, pred_start: int = 0,
-                          n_pred: int | None = None, long_order: int = 0, want_stats: bool = False):
+                          n_pred: int | None = None, long_order: int = 0, want_stats: bool = False,
+                          want_se: bool = False):
         """Regression with ARIMA(``ar_order``, ``diff_order``, ``ma_order``) errors (``mmf_fit_forecast_arma_f32``,
         DESIGN.md section 2 item 13): the plain fit (on the differenced series and design for ``diff_order`` >= 1),
         then Hannan-Rissanen on its residuals -- a long AR of order ``long_order`` (0: the default) gives innovation
@@ -614,6 +620,8 @@ class ForecastEngine:
                                                     C.byref(st) if st is not None else None))
         res = {"pred": out, "phi": phi, "theta": theta, "order": order, "ma_order": ma, "sigma": sigma,
                "status": status}
+        if want_se:
+            self._add_se(res, y, t_fit, pred_start, n_pred, int(diff_order))
         if st is not None:
             self.launches += st.kernel_launches
             res["stats"] = Stats(st.kernel_ms, st.total_ms, st.n_series, st.n_pending, st.h2d_bytes, st.d2h_bytes,
@@ -621,7 +629,7 @@ class ForecastEngine:
         return res
 
     def fit_select_ar(self, y, n_hold: int, orders=(0, 1, 2, 3, 4), pred_start: int = 0, n_pred: int | None = None,
-                      want_stats: bool = False):
+                      want_stats: bool = False, want_se: bool = False):
         """Regression with AR(p) errors, p chosen per series by hold-out MSE (``mmf_fit_select_ar_f32``, DESIGN.md
         section 2 item 10).  Candidate m of ``orders`` (ascending, distinct, 0 .. MMF_AR_MAX) is ``fit_forecast_ar``
         with ``ar_order = m`` (m = 0: the plain regression); it is scored by the MSE of its dynamic forecast from t_fit
@@ -660,6 +668,8 @@ class ForecastEngine:
                                                 C.byref(st) if st is not None else None))
         res = {"pred": out, "choice": choice, "mse": mse, "cand_mse": cand_mse, "phi": phi, "order": order,
                "sigma": sigma, "status": status}
+        if want_se:
+            self._add_se(res, y, self.t_fit, pred_start, n_pred, 0)
         if st is not None:
             self.launches += st.kernel_launches
             res["stats"] = Stats(st.kernel_ms, st.total_ms, st.n_series, st.n_pending, st.h2d_bytes, st.d2h_bytes,
@@ -667,7 +677,7 @@ class ForecastEngine:
         return res
 
     def fit_select_arima(self, y, n_hold: int, orders=(0, 1, 2, 3, 4), diffs=(0, 1, 2), pred_start: int = 0,
-                         n_pred: int | None = None, want_stats: bool = False):
+                         n_pred: int | None = None, want_stats: bool = False, want_se: bool = False):
         """Regression with ARIMA(p, d, 0) errors, (p, d) chosen per series by hold-out MSE on levels
         (``mmf_fit_select_arima_f32``, DESIGN.md section 2 item 12).  The candidates are every pair of ``orders``
         (ascending, distinct, 0 .. MMF_AR_MAX) and ``diffs`` (ascending, distinct, 0 .. MMF_DIFF_MAX), d-major: (p, 0)
@@ -719,6 +729,8 @@ class ForecastEngine:
                                                    C.byref(st) if st is not None else None))
         res = {"pred": out, "choice_p": choice_p, "choice_d": choice_d, "mse": mse, "cand_mse": cand_mse, "phi": phi,
                "order": order, "sigma": sigma, "status": status}
+        if want_se:
+            self._add_se(res, y, t_fit, pred_start, n_pred, 0, diffs=choice_d)
         if st is not None:
             self.launches += st.kernel_launches
             res["stats"] = Stats(st.kernel_ms, st.total_ms, st.n_series, st.n_pending, st.h2d_bytes, st.d2h_bytes,
@@ -726,7 +738,8 @@ class ForecastEngine:
         return res
 
     def fit_select_arma(self, y, n_hold: int, orders=(0, 1, 2, 3, 4), diffs=(0, 1, 2), mas=(0, 1, 2, 3, 4),
-                        pred_start: int = 0, n_pred: int | None = None, long_order: int = 0, want_stats: bool = False):
+                        pred_start: int = 0, n_pred: int | None = None, long_order: int = 0, want_stats: bool = False,
+                        want_se: bool = False):
         """Regression with ARIMA(p, d, q) errors, (p, d, q) chosen per series by hold-out MSE on levels
         (``mmf_fit_select_arma_f32``, DESIGN.md section 2 item 14).  The candidates are every triple of ``orders``,
         ``diffs`` and ``mas`` (ascending, distinct, 0 .. MMF_MA_MAX, ``mas[0] == 0``), d, then q, then p ascending:
@@ -782,11 +795,28 @@ class ForecastEngine:
         res = {"pred": out, "choice_p": choice_p, "choice_d": choice_d, "choice_q": choice_q, "mse": mse,
                "cand_mse": cand_mse, "phi": phi, "theta": theta, "order": order, "ma_order": ma_order, "sigma": sigma,
                "status": status}
+        if want_se:
+            self._add_se(res, y, t_fit, pred_start, n_pred, 0, diffs=choice_d)
         if st is not None:
             self.launches += st.kernel_launches
             res["stats"] = Stats(st.kernel_ms, st.total_ms, st.n_series, st.n_pending, st.h2d_bytes, st.d2h_bytes,
                                  st.kernel_launches, {N.KERNEL_WARP: "warp", N.KERNEL_TC: "tc"}.get(st.kernel_used, "?"))
         return res
+
+    def _add_se(self, res, y, t_fit: int, pred_start: int, n_pred: int, diff_order: int, diffs=None) -> None:
+        """``want_se=True`` of the ARIMA-family calls: ``res["se"]`` [n, n_pred] float32, the standard error of every
+        prediction in ``res["pred"]`` (``mmf_arima_se_f32``, DESIGN.md section 2 item 15), from the call's own phi,
+        theta, orders, sigma and d (``diffs``: the per-series d of a selection), enqueued on the same stream."""
+        import torch
+        yp, n, _, ld_y = _describe(y, "y")
+        se = torch.empty((n, n_pred), device=y.device, dtype=torch.float32)
+        theta, ma = res.get("theta"), res.get("ma_order")
+        N.check(self._lib.mmf_arima_se_f32(self._h, yp, n, ld_y, int(t_fit), int(diff_order),
+                                           diffs.data_ptr() if diffs is not None else None, res["phi"].data_ptr(),
+                                           res["order"].data_ptr(), theta.data_ptr() if theta is not None else None,
+                                           ma.data_ptr() if ma is not None else None, res["sigma"].data_ptr(),
+                                           int(pred_start), int(n_pred), se.data_ptr(), se.stride(0), None))
+        res["se"] = se
 
     def capture(self, y, pred_start: int, n_pred: int, out=None, status=None):
         """Record one device-resident ``fit_forecast`` call as a CUDA graph.  Small batches are launch-bound (three

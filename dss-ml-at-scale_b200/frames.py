@@ -339,7 +339,7 @@ def _host(x):
 
 
 def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, interval=False, ar=None, diff=None,
-                 ma=None):
+                 ma=None, want_se=False):
     """Run the engine over every bucket: yields (bucket, out_days, n_pred, y_host, pred_host, se_host or None).
     ``interval``: prediction standard errors too (``fit_forecast_se``), one call per calendar bucket.
     ``ar``: regression with AR(ar) errors (``fit_forecast_ar``), one call per calendar bucket; a tuple of orders
@@ -349,7 +349,9 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
     ``horizon`` rows (``fit_select_arima``).
     ``ma``: regression with ARIMA(ar, diff or 0, ma) errors (``fit_forecast_arma``), one call per calendar bucket; a
     tuple of MA orders (with ``ar`` and ``diff`` tuples) chooses (p, d, q) per series by hold-out MSE over the last
-    ``horizon`` rows (``fit_select_arma``)."""
+    ``horizon`` rows (``fit_select_arma``).
+    ``want_se``: the ARIMA-family call's forecast standard errors too (``want_se=True``, DESIGN.md section 2 item 15)."""
+    se_kw = {"want_se": True} if want_se else {}
     if interval and select is not None:
         raise ValueError("interval= is not offered with select= (model selection returns point forecasts)")
     t_fit_min = min((b.t_len - (horizon if mode == "holdout" else 0)) for b in buckets) if buckets else 0
@@ -367,27 +369,33 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
         if isinstance(ma, tuple):
             from .engine import device_packed
             yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
-            pred = _host(eng.fit_select_arma(yd, horizon, ar, diff, ma, pred_start, n_pred)["pred"])
+            res = eng.fit_select_arma(yd, horizon, ar, diff, ma, pred_start, n_pred, **se_kw)
+            pred, se = _host(res["pred"]), (_host(res["se"]) if want_se else None)
         elif ma is not None:
             from .engine import device_packed
             yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
-            pred = _host(eng.fit_forecast_arma(yd, ar, ma, diff or 0, pred_start, n_pred)["pred"])
+            res = eng.fit_forecast_arma(yd, ar, ma, diff or 0, pred_start, n_pred, **se_kw)
+            pred, se = _host(res["pred"]), (_host(res["se"]) if want_se else None)
         elif isinstance(diff, tuple):
             from .engine import device_packed
             yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
-            pred = _host(eng.fit_select_arima(yd, horizon, ar, diff, pred_start, n_pred)["pred"])
+            res = eng.fit_select_arima(yd, horizon, ar, diff, pred_start, n_pred, **se_kw)
+            pred, se = _host(res["pred"]), (_host(res["se"]) if want_se else None)
         elif diff is not None:
             from .engine import device_packed
             yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
-            pred = _host(eng.fit_forecast_arima(yd, ar, diff, pred_start, n_pred)["pred"])
+            res = eng.fit_forecast_arima(yd, ar, diff, pred_start, n_pred, **se_kw)
+            pred, se = _host(res["pred"]), (_host(res["se"]) if want_se else None)
         elif isinstance(ar, tuple):
             from .engine import device_packed
             yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
-            pred = _host(eng.fit_select_ar(yd, horizon, ar, pred_start, n_pred)["pred"])
+            res = eng.fit_select_ar(yd, horizon, ar, pred_start, n_pred, **se_kw)
+            pred, se = _host(res["pred"]), (_host(res["se"]) if want_se else None)
         elif ar is not None:
             from .engine import device_packed
             yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
-            pred = _host(eng.fit_forecast_ar(yd, ar, pred_start, n_pred)["pred"])
+            res = eng.fit_forecast_ar(yd, ar, pred_start, n_pred, **se_kw)
+            pred, se = _host(res["pred"]), (_host(res["se"]) if want_se else None)
         elif interval:
             from .engine import device_packed
             yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
@@ -416,6 +424,24 @@ def _z_of(interval):
     if not 0.0 < level < 1.0:
         raise ValueError(f"interval must be a level in (0, 1), got {interval!r}")
     return NormalDist().inv_cdf(0.5 + level / 2.0)
+
+
+def _conf_z(conf_int, ar, select, interval):
+    """normal quantile of ``conf_int=`` (None: no band).  It is the band of the ARIMA-family forecasts (DESIGN.md
+    section 2 item 15), so it needs ``ar=``; ``interval=`` is the plain regression's band, a different quantity"""
+    if conf_int is None:
+        return None
+    if ar is None:
+        raise ValueError("conf_int= needs ar= (it is the band of the AR / ARIMA forecasts; the plain regression's band "
+                         "is interval=)")
+    if interval is not None:
+        raise ValueError("conf_int= and interval= are different bands: pass one of them")
+    if select is not None:
+        raise ValueError("conf_int= is not offered with select=")
+    level = float(conf_int)
+    if not 0.0 < level < 1.0:
+        raise ValueError(f"conf_int must be a level in (0, 1), got {conf_int!r}")
+    return _z_of(level)
 
 
 def _ar_order(ar, select, interval, mode="holdout"):
@@ -621,7 +647,8 @@ def _single_group_fast(pdf, keys, date_col, value_col, freq, horizon, mode, desi
 def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Demand",
                     freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                     engine: ForecastEngine | None = None, pack: str = "host", select=None,
-                    null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None, ma=None) -> pd.DataFrame:
+                    null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None, ma=None,
+                    conf_int=None) -> pd.DataFrame:
     """Fit + forecast every group in ``pdf``; returns ``tuning_schema`` rows
     (keys..., Date, Demand, Demand_Fitted), groups in key order, dates ascending.
 
@@ -676,16 +703,25 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     the last ``horizon`` dates (``ForecastEngine.fit_select_arma``, DESIGN.md section 2 item 14): the reference's search
     space, searched exhaustively.  At most 32 pairs (p, q >= 1).  Holdout mode only, one call per calendar bucket,
     schema unchanged.
+
+    ``conf_int=0.9`` with any accepted ``ar=`` / ``diff=`` / ``ma=`` (fixed or tuples) appends float32 ``Demand_Lower``
+    / ``Demand_Upper`` = ``Demand_Fitted -+ z * se``, ``z`` as for ``interval=`` and ``se`` the standard error of the
+    ARIMA-family forecast (``want_se=True``, DESIGN.md section 2 item 15: the fitted model taken as true, no estimation
+    uncertainty; NaN where ``Demand_Fitted`` is NaN).  Schema ``tuning_schema(interval=True)``.  Refused without
+    ``ar=``, with ``interval=`` (the plain regression's band, a different quantity) or ``select=``, and for a level
+    outside (0, 1).
     """
     eng = engine or default_engine()
     keys = list(keys)
     fitted_col = value_col + "_Fitted"
     z = _z_of(interval)
+    cz = _conf_z(conf_int, ar, select, interval)
     if ma is None:
         diff = _diff_order(diff, ar, select, interval, mode)
         ar = _ar_orders_for(diff, ar, select, interval, mode)
     else:
         ar, diff, ma = _arma_orders(ma, ar, diff, select, interval, mode)
+    zb = z if z is not None else cz               # the band's quantile, whichever of the two asked for it
     if pack == "host" and select is None and z is None and ar is None and isinstance(pdf, pd.DataFrame):
         one = _single_group_fast(pdf, keys, date_col, value_col, freq, horizon, mode, design, eng, null_keys_on_gaps)
         if one is not None:
@@ -693,7 +729,8 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     buckets = _buckets_for(pdf, keys, date_col, value_col, freq, pack, eng)
     parts, lengths = [], []
     for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
-                                                              pack == "device", z is not None, ar, diff, ma):
+                                                              pack == "device", z is not None, ar, diff, ma,
+                                                              cz is not None):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n), n_pred)
         # key columns keep the dtype they came in with (no per-row string inference on N x T values)
@@ -704,8 +741,8 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
         else:
             frame[value_col] = np.full(n * n_pred, np.nan, dtype=np.float32)
         frame[fitted_col] = pred.reshape(-1)
-        if z is not None:
-            frame[value_col + "_Lower"], frame[value_col + "_Upper"] = _bounds(pred, se, z)
+        if zb is not None:
+            frame[value_col + "_Lower"], frame[value_col + "_Upper"] = _bounds(pred, se, zb)
         if null_keys_on_gaps and mode == "holdout":
             gap = np.isnan(frame[value_col])
             if gap.any():
@@ -715,7 +752,7 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
         lengths.append(n_pred)
     if not parts:
         bounds = ({value_col + "_Lower": pd.Series(dtype=np.float32), value_col + "_Upper": pd.Series(dtype=np.float32)}
-                  if z is not None else {})
+                  if zb is not None else {})
         return pd.DataFrame({**{k: pd.Series(dtype=object) for k in keys},
                              date_col: pd.Series(dtype="datetime64[ns]"),
                              value_col: pd.Series(dtype=np.float32), fitted_col: pd.Series(dtype=np.float32), **bounds})
@@ -784,14 +821,16 @@ def backtest_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
 def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Demand",
                    freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                    engine: ForecastEngine | None = None, pack: str = "host", select=None,
-                   null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None, ma=None):
+                   null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None, ma=None,
+                   conf_int=None):
     """Arrow ``Table``/``RecordBatch`` in -> Arrow ``Table`` with ``tuning_schema`` out (the ``mapInArrow``
     flavour of the boundary).  No pandas frame of the rows on either side: keys are dictionary-encoded on the way
     in and expanded from a dictionary on the way out, dates and values are NumPy views of Arrow buffers.
     ``interval=level`` adds the ``{value}_Lower`` / ``{value}_Upper`` columns of ``forecast_groups`` (schema:
     ``tuning_schema(..., interval=True)``).  ``ar=p`` fits regression with AR(p) errors and ``ar=(0, 1, 2, 3, 4)`` chooses the order per series, as in
     ``forecast_groups``; ``diff=d`` with ``ar=p`` fits ARIMA(p, d, 0) errors as there, and ``ma=q`` ARIMA(p, d, q); tuples of ``ar``, ``diff`` and
-    ``ma`` choose (p, d, q) per series."""
+    ``ma`` choose (p, d, q) per series.  ``conf_int=level`` adds the same two columns for those forecasts, as in
+    ``forecast_groups``."""
     import pyarrow as pa
 
     if isinstance(table, pa.RecordBatch):
@@ -799,16 +838,19 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     eng = engine or default_engine()
     keys = list(keys)
     z = _z_of(interval)
+    cz = _conf_z(conf_int, ar, select, interval)
     if ma is None:
         diff = _diff_order(diff, ar, select, interval, mode)
         ar = _ar_orders_for(diff, ar, select, interval, mode)
     else:
         ar, diff, ma = _arma_orders(ma, ar, diff, select, interval, mode)
-    schema = tuning_schema(keys, date_col, value_col, interval=z is not None)
+    zb = z if z is not None else cz
+    schema = tuning_schema(keys, date_col, value_col, interval=zb is not None)
     buckets = _buckets_for(table, keys, date_col, value_col, freq, pack, eng)
     parts, lengths = [], []
     for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
-                                                              pack == "device", z is not None, ar, diff, ma):
+                                                              pack == "device", z is not None, ar, diff, ma,
+                                                              cz is not None):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n, dtype=np.int32), n_pred)
         cols = []
@@ -826,8 +868,8 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
         cols.append(pa.array(np.tile(day32, n)).cast(pa.date32()))
         cols.append(pa.array(demand, from_pandas=True))               # NaN -> null, like the pandas route
         cols.append(pa.array(np.ascontiguousarray(pred).reshape(-1), from_pandas=True))
-        if z is not None:
-            cols.extend(pa.array(v, from_pandas=True) for v in _bounds(pred, se, z))
+        if zb is not None:
+            cols.extend(pa.array(v, from_pandas=True) for v in _bounds(pred, se, zb))
         parts.append(pa.Table.from_arrays(cols, schema=schema))
         lengths.append(n_pred)
     if not parts:

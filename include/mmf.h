@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define MMF_VERSION 110          /* 0.1.10 */
+#define MMF_VERSION 111          /* 0.1.11 */
 #define MMF_P 16                 /* design columns (zero-pad narrower designs) */
 #define MMF_PIVOT_TOL 1e-3f      /* per-series relative Cholesky pivot threshold */
 #define MMF_CAL_TOL 1e-10        /* aliasing threshold on the float64 calendar Gram */
@@ -389,6 +389,32 @@ int mmf_fit_select_arma_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
                             float* out_cand_mse /* [n][n_diffs][n_mas][n_orders] */, float* out_phi, float* out_theta,
                             int32_t* out_order, int32_t* out_ma_order, float* out_sigma, int32_t* out_status,
                             mmf_stats* stats);
+
+/* ---- standard errors of the ARIMA-family forecasts (DESIGN.md section 2 item 15) ----------------------------------------
+ * mmf_arima_se_f32: a post-pass over the outputs of any ARIMA-family call (mmf_fit_forecast_ar_f32, _arima_f32, _arma_f32,
+ * mmf_fit_select_ar_f32, _select_arima_f32, _select_arma_f32): se[i, j] = sqrt(Var(y_t - yhat_t)), t = pred_start + j,
+ * for the predictor those calls ship (one step ahead in sample, the dynamic forecast from t_fit beyond it, missing values
+ * filled with predictions), taking the fitted model as true: u_s = sum phi_j u_{s-j} + eps_s + sum theta_j eps_{s-j} on
+ * y (d = 0) or z' (d >= 1), eps iid with variance sigma^2, u_s = eps_s = 0 for s < 0, and beta, phi, theta, sigma known
+ * (no estimation uncertainty).  The covariance of the predictor's error state is propagated in float64 over rows
+ * [0, pred_start + n_pred); rows whose z' value (t < t_fit and y_{t-d} .. y_t finite) and level (t < t_fit and y_t
+ * finite) are observed reset their error components.  On a gap-free fit window se = sigma in sample and
+ * sigma sqrt(sum_{j<h} psi*_j^2) beyond (h = t - t_fit + 1, psi* the psi-weights of (phi, theta) summed d times).
+ *   y [n, ld_y]: levels, read on [0, t_fit) only, and only for whether each value is finite (1 <= t_fit <= ld_y);
+ *   diffs [n] (nullable): per-row d, e.g. out_choice_d of a selection; NULL: diff_order (0 .. MMF_DIFF_MAX) for every row;
+ *   phi [n][MMF_AR_MAX], order [n], sigma [n]: the call's outputs (phi read up to the row's order);
+ *   theta [n][MMF_MA_MAX], ma_order [n]: both given or both NULL (NULL: q = 0);
+ *   out_se [n, ld_se] (ld_se >= n_pred, any base pointer): only columns [0, n_pred) of a row are written, float32 of
+ *   sigma sqrt(1 + c'Pc).  NaN for rows t < d, rows whose level chain is NaN in the predictor (a missing level before
+ *   the first observed one), and every row of a series whose sigma is not finite (status 1, choice -1) or whose order,
+ *   ma_order or d is out of range; +Inf where the float64 variance overflows (explosive parameters).
+ * No plan is needed and none is changed.  Device buffers only (host pointers: MMF_E_UNSUPPORTED); enqueue-only unless
+ * `stats` is non-NULL; refused arguments write nothing.
+ * replaces: SARIMAX's get_forecast().se_mean / conf_int() beside the reference's forecast (02:453-457, 484-488). */
+int mmf_arima_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t t_fit,
+                     int32_t diff_order, const int32_t* diffs, const float* phi, const int32_t* order,
+                     const float* theta, const int32_t* ma_order, const float* sigma, int32_t pred_start,
+                     int32_t n_pred, float* out_se, int64_t ld_se, mmf_stats* stats);
 
 /* ---- ragged batches: groups on MANY calendars in one launch ---------------------------------------------
  * The reference re-indexes every group on its own calendar (sort_values + asfreq per group, 02:422-423), so one

@@ -27,20 +27,8 @@ ar_kernel(const DesignView d, const FitArgs a, const ArArgs ar) {
   const int S = min(a.pred_start, t_fit);
   if (threadIdx.x == 0) s_lo = INT32_MAX;
 
-  int st = MMF_STATUS_EMPTY;
-  float g[P], c = 0.f;
-#pragma unroll
-  for (int q = 0; q < P; ++q) g[q] = 0.f;
-  if (live) {
-    st = a.status[row];
-    const float4* gp = reinterpret_cast<const float4*>(a.out_gamma + row * P);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const float4 v = gp[q];
-      g[4 * q] = v.x; g[4 * q + 1] = v.y; g[4 * q + 2] = v.z; g[4 * q + 3] = v.w;
-    }
-    c = a.out_c[row];
-  }
+  float g[P], c;
+  const int st = load_fit(a, row, live, g, c);
   const bool work = live && st != MMF_STATUS_EMPTY;
   const float* __restrict__ yr = a.y + (live ? row : 0) * a.ld_y;
 
@@ -112,18 +100,12 @@ ar_kernel(const DesignView d, const FitArgs a, const ArArgs ar) {
   // used columns k of the dof rule (section 2 item 7): the calendar's kept columns that are non-zero on an observed fit
   // row (a column that is zero there has a zero pivot and is skipped, as in the fit kernels), less those the pivoted
   // solve dropped for the series' mask (status 2 only; a dropped column's gamma is pinned to exactly 0)
-  colmask = __reduce_or_sync(0xffffffffu, colmask);
-  uint32_t used = d.kept_mask & colmask;
-  if (st == MMF_STATUS_RANKDEF) {
-#pragma unroll
-    for (int q = 0; q < P; ++q) used &= g[q] != 0.f ? ~0u : ~(1u << q);
-  }
-  const int k_used = __popc(used);
+  const int k_used = used_columns(d, colmask, st, g);
   double phi[AR_MAX];
 #pragma unroll
   for (int j = 0; j < AR_MAX; ++j) phi[j] = 0.0;
   int order = 0;
-  double var = __longlong_as_double(0x7ff8000000000000ll);
+  double var = dnan();
   if (work) {
     const double inv = 1.0 / (double)max(n_obs, 1);
     double r[AR_MAX + 1];
@@ -157,12 +139,7 @@ ar_kernel(const DesignView d, const FitArgs a, const ArArgs ar) {
 #pragma unroll
   for (int j = 0; j < AR_MAX; ++j) f[j] = (float)phi[j];
   if (live) {
-    if (ar.phi != nullptr && lane < AR_MAX) {
-      float v = 0.f;
-#pragma unroll
-      for (int j = 0; j < AR_MAX; ++j) v = lane == j ? f[j] : v;
-      ar.phi[row * AR_MAX + lane] = v;
-    }
+    store_row(ar.phi, row, lane, f);
     if (lane == 0) {
       if (ar.order != nullptr) ar.order[row] = order;
       if (ar.sigma != nullptr) ar.sigma[row] = (float)sqrt(var);
@@ -250,20 +227,8 @@ ar_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const ArS
   const int S = min(a.pred_start, t_fit);
   if (threadIdx.x == 0) s_lo = INT32_MAX;
 
-  int st = MMF_STATUS_EMPTY;
-  float g[P], c = 0.f;
-#pragma unroll
-  for (int q = 0; q < P; ++q) g[q] = 0.f;
-  if (live) {
-    st = a.status[row];
-    const float4* gp = reinterpret_cast<const float4*>(a.out_gamma + row * P);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const float4 v = gp[q];
-      g[4 * q] = v.x; g[4 * q + 1] = v.y; g[4 * q + 2] = v.z; g[4 * q + 3] = v.w;
-    }
-    c = a.out_c[row];
-  }
+  float g[P], c;
+  const int st = load_fit(a, row, live, g, c);
   const bool work = live && st != MMF_STATUS_EMPTY;
   const float* __restrict__ yr = a.y + (live ? row : 0) * a.ld_y;
 
@@ -347,13 +312,7 @@ ar_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const ArS
   // used columns k of the dof rule (section 2 item 7): the calendar's kept columns that are non-zero on an observed fit
   // row (a column that is zero there has a zero pivot and is skipped, as in the fit kernels), less those the pivoted
   // solve dropped for the series' mask (status 2 only; a dropped column's gamma is pinned to exactly 0)
-  colmask = __reduce_or_sync(0xffffffffu, colmask);
-  uint32_t used = d.kept_mask & colmask;
-  if (st == MMF_STATUS_RANKDEF) {
-#pragma unroll
-    for (int q = 0; q < P; ++q) used &= g[q] != 0.f ? ~0u : ~(1u << q);
-  }
-  const int k_used = __popc(used);
+  const int k_used = used_columns(d, colmask, st, g);
   // Levinson-Durbin bound of lane j: candidate j; lanes >= n_cand repeat the last candidate
   int pl = sel.cand[0];
 #pragma unroll
@@ -363,7 +322,7 @@ ar_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const ArS
 #pragma unroll
   for (int j = 0; j < AR_MAX; ++j) phi[j] = 0.0;
   int order = 0;
-  double var = __longlong_as_double(0x7ff8000000000000ll);
+  double var = dnan();
   if (work) {
     const double inv = 1.0 / (double)max(n_obs, 1);
     double r[AR_MAX + 1];
@@ -458,7 +417,7 @@ ar_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const ArS
       }
       __syncthreads();
     }
-    const double mse = cnt > 0 ? sse / (double)cnt : __longlong_as_double(0x7ff8000000000000ll);
+    const double mse = cnt > 0 ? sse / (double)cnt : dnan();
     // ---- choice: the first minimum in list order; no scored point: the last candidate
     int win = -1;
     double best = 0.0;
@@ -482,12 +441,7 @@ ar_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const ArS
     }
   }
   if (live) {
-    if (ar.phi != nullptr && lane < AR_MAX) {
-      float v = 0.f;
-#pragma unroll
-      for (int j = 0; j < AR_MAX; ++j) v = lane == j ? f[j] : v;
-      ar.phi[row * AR_MAX + lane] = v;
-    }
+    store_row(ar.phi, row, lane, f);
     if (lane == 0) {
       if (ar.order != nullptr) ar.order[row] = order;
       if (ar.sigma != nullptr) ar.sigma[row] = (float)sqrt(var);

@@ -15,8 +15,6 @@
 namespace mmf {
 namespace {
 
-__device__ __forceinline__ float qnan() { return __int_as_float(0x7fc00000); }
-
 // one warp per row, lanes over s: z' in the stated fp32 order; any non-finite level gives a non-finite z
 __global__ void __launch_bounds__(THREADS)
 diff_kernel(const ArimaArgs ma, float* __restrict__ z, int64_t ld_z, int64_t n) {
@@ -34,11 +32,6 @@ diff_kernel(const ArimaArgs ma, float* __restrict__ z, int64_t ld_z, int64_t n) 
       zr[s] = __fsub_rn(__fsub_rn(y2, y1), __fsub_rn(y1, y0));
     }
   }
-}
-
-// yhat_t from zhat_t and the filled levels ytilde_{t-1} (l1), ytilde_{t-2} (l2), in the order include/mmf.h states
-__device__ __forceinline__ float integrate(float zh, float l1, float l2, int d) {
-  return d == 1 ? __fadd_rn(zh, l1) : __fsub_rn(__fadd_rn(zh, __fmul_rn(2.f, l1)), l2);
 }
 
 // d.t_fit, d.n_rows: the differenced plan (t_fit - dd, n_rows - dd); a.y / a.ld_y: z'; a.pred_start / n_pred / out /
@@ -61,20 +54,8 @@ arima_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const ArimaAr
   const int S = min(a.pred_start, T) - dd; // the latest restart: no later than the first requested level's z' row
   if (threadIdx.x == 0) s_lo = INT32_MAX;
 
-  int st = MMF_STATUS_EMPTY;
-  float g[P], c = 0.f;
-#pragma unroll
-  for (int q = 0; q < P; ++q) g[q] = 0.f;
-  if (live) {
-    st = a.status[row];
-    const float4* gp = reinterpret_cast<const float4*>(a.out_gamma + row * P);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const float4 v = gp[q];
-      g[4 * q] = v.x; g[4 * q + 1] = v.y; g[4 * q + 2] = v.z; g[4 * q + 3] = v.w;
-    }
-    c = a.out_c[row];
-  }
+  float g[P], c;
+  const int st = load_fit(a, row, live, g, c);
   const bool work = live && st != MMF_STATUS_EMPTY;
   const float* __restrict__ zr = a.y + (live ? row : 0) * a.ld_y;
   const float* __restrict__ yr = ma.y + (live ? row : 0) * ma.ld_y;
@@ -144,18 +125,12 @@ arima_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const ArimaAr
     if (k <= p)
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], o);
-  colmask = __reduce_or_sync(0xffffffffu, colmask);
-  uint32_t used = d.kept_mask & colmask;
-  if (st == MMF_STATUS_RANKDEF) {
-#pragma unroll
-    for (int q = 0; q < P; ++q) used &= g[q] != 0.f ? ~0u : ~(1u << q);
-  }
-  const int k_used = __popc(used);
+  const int k_used = used_columns(d, colmask, st, g);
   double phi[AR_MAX];
 #pragma unroll
   for (int j = 0; j < AR_MAX; ++j) phi[j] = 0.0;
   int order = 0;
-  double var = __longlong_as_double(0x7ff8000000000000ll);
+  double var = dnan();
   if (work) {
     const double inv = 1.0 / (double)max(n_obs, 1);
     double r[AR_MAX + 1];
@@ -189,12 +164,7 @@ arima_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const ArimaAr
 #pragma unroll
   for (int j = 0; j < AR_MAX; ++j) f[j] = (float)phi[j];
   if (live) {
-    if (ar.phi != nullptr && lane < AR_MAX) {
-      float v = 0.f;
-#pragma unroll
-      for (int j = 0; j < AR_MAX; ++j) v = lane == j ? f[j] : v;
-      ar.phi[row * AR_MAX + lane] = v;
-    }
+    store_row(ar.phi, row, lane, f);
     if (lane == 0) {
       if (ar.order != nullptr) ar.order[row] = order;
       if (ar.sigma != nullptr) ar.sigma[row] = (float)sqrt(var);
@@ -328,20 +298,8 @@ arima_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const 
   const bool first = sel.d_index == 0;
   if (threadIdx.x == 0) s_lo = INT32_MAX;
 
-  int st = MMF_STATUS_EMPTY;
-  float g[P], c = 0.f;
-#pragma unroll
-  for (int q = 0; q < P; ++q) g[q] = 0.f;
-  if (live) {
-    st = a.status[row];
-    const float4* gp = reinterpret_cast<const float4*>(a.out_gamma + row * P);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const float4 v = gp[q];
-      g[4 * q] = v.x; g[4 * q + 1] = v.y; g[4 * q + 2] = v.z; g[4 * q + 3] = v.w;
-    }
-    c = a.out_c[row];
-  }
+  float g[P], c;
+  const int st = load_fit(a, row, live, g, c);
   const bool work = live && st != MMF_STATUS_EMPTY;     // eligible: the fit this d builds on is not empty
   const float* __restrict__ zr = a.y + (live ? row : 0) * a.ld_y;
   const float* __restrict__ yr = ma.y + (live ? row : 0) * ma.ld_y;
@@ -417,13 +375,7 @@ arima_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const 
     if (k <= p)
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], o);
-  colmask = __reduce_or_sync(0xffffffffu, colmask);
-  uint32_t used = d.kept_mask & colmask;
-  if (st == MMF_STATUS_RANKDEF) {
-#pragma unroll
-    for (int q = 0; q < P; ++q) used &= g[q] != 0.f ? ~0u : ~(1u << q);
-  }
-  const int k_used = __popc(used);
+  const int k_used = used_columns(d, colmask, st, g);
   int pl = sel.cand[0];                    // lanes >= n_cand repeat the last candidate
 #pragma unroll
   for (int j = 1; j < MMF_ARSEL_MAX_CAND; ++j)
@@ -432,7 +384,7 @@ arima_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const 
 #pragma unroll
   for (int j = 0; j < AR_MAX; ++j) phi[j] = 0.0;
   int order = 0;
-  double var = __longlong_as_double(0x7ff8000000000000ll);
+  double var = dnan();
   if (work) {
     const double inv = 1.0 / (double)max(n_obs, 1);
     double r[AR_MAX + 1];
@@ -545,7 +497,7 @@ arima_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const 
       }
       __syncthreads();
     }
-    const double mse = cnt > 0 ? sse / (double)cnt : __longlong_as_double(0x7ff8000000000000ll);
+    const double mse = cnt > 0 ? sse / (double)cnt : dnan();
     // ---- this d's first minimum in list order (no scored point: its last candidate), then the running best
     int win = -1;
     double best = 0.0;
@@ -585,12 +537,7 @@ arima_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const 
     }
   }
   if (live && (first || lead)) {
-    if (ar.phi != nullptr && lane < AR_MAX) {
-      float v = 0.f;
-#pragma unroll
-      for (int j = 0; j < AR_MAX; ++j) v = lane == j ? f[j] : v;
-      ar.phi[row * AR_MAX + lane] = v;
-    }
+    store_row(ar.phi, row, lane, f);
     if (lane == 0) {
       if (ar.order != nullptr) ar.order[row] = order;
       if (ar.sigma != nullptr) ar.sigma[row] = (float)sqrt(var);

@@ -10,7 +10,9 @@
 //              fallback outputs;
 //     pass B   the ARMA recursion from s = 0 (never restarted: MA terms have infinite memory), integrated to levels as
 //              arima_kernel does for d >= 1, for the gated series only.
-// A kernel of its own rather than a template of ar_kernel / arima_kernel: wrapping moved ar_kernel's registers (4.14).
+// The fit hand-off load, the ring shift, the theta store and the small helpers come from ar_common.cuh.  The other blocks
+// it shares with arma_select_kernel (pass A, step 1, the pass-A2 rings, the solve, pass B) stay written out here: as
+// shared functions they changed this kernel's code, and the ARMA calls were measured about 1 % slower (DESIGN.md 4.17).
 #include "ar_common.cuh"
 
 // timing builds only (scripts/bench_arma.py --split): 1 ends the kernel after pass A and step 1, 2 after the solve
@@ -21,35 +23,7 @@
 namespace mmf {
 namespace {
 
-constexpr int MA_MAX = MMF_MA_MAX;
 constexpr int NC = AR_MAX + MA_MAX + 1;    // regressors + target: columns of the staged normal equations
-
-__device__ __forceinline__ float arma_qnan() { return __int_as_float(0x7fc00000); }
-
-// yhat_t from zhat_t and the filled levels ytilde_{t-1} (l1), ytilde_{t-2} (l2), in the order include/mmf.h states
-__device__ __forceinline__ float arma_integrate(float zh, float l1, float l2, int d) {
-  return d == 1 ? __fadd_rn(zh, l1) : __fsub_rn(__fadd_rn(zh, __fmul_rn(2.f, l1)), l2);
-}
-
-__device__ __forceinline__ double warp_sum(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-// step-down (reverse Levinson) of 1 - sum_j a_j z^j, a[0 .. k): true when every |kappa| < MMF_AR_KAPPA_MAX
-template <int N>
-__device__ bool step_down_ok(double (&a)[N], int k) {
-  for (int j = k; j >= 1; --j) {
-    const double kap = a[j - 1];
-    if (!(fabs(kap) < (double)MMF_AR_KAPPA_MAX)) return false;
-    const double den = 1.0 - kap * kap;
-    double nxt[N];
-    for (int i = 1; i < j; ++i) nxt[i - 1] = (a[i - 1] + kap * a[j - i - 1]) / den;
-    for (int i = 1; i < j; ++i) a[i - 1] = nxt[i - 1];
-  }
-  return true;
-}
 
 // d.t_fit: fit rows of a.y (z' for d >= 1); ma: the levels (ma.d = 0: ma.y is a.y); ar.p / hr.q / hr.m: the orders
 __global__ void __launch_bounds__(THREADS, 3)
@@ -78,20 +52,8 @@ arma_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const ArimaArg
   double* __restrict__ sU = s_u[warp];
   double* __restrict__ sV = s_v[warp];
 
-  int st = MMF_STATUS_EMPTY;
-  float g[P], c = 0.f;
-#pragma unroll
-  for (int k = 0; k < P; ++k) g[k] = 0.f;
-  if (live) {
-    st = a.status[row];
-    const float4* gp = reinterpret_cast<const float4*>(a.out_gamma + row * P);
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float4 v = gp[k];
-      g[4 * k] = v.x; g[4 * k + 1] = v.y; g[4 * k + 2] = v.z; g[4 * k + 3] = v.w;
-    }
-    c = a.out_c[row];
-  }
+  float g[P], c;
+  const int st = load_fit(a, row, live, g, c);
   const bool work = live && st != MMF_STATUS_EMPTY;
   const float* __restrict__ zr = a.y + (live ? row : 0) * a.ld_y;
   const float* __restrict__ yr = ma.y + (live ? row : 0) * ma.ld_y;
@@ -244,9 +206,7 @@ arma_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const ArimaArg
             gacc[s] = acc;
           }
           __syncwarp();
-          sE[lane] = ed;
-          sU[lane] = sU[32 + lane];
-          sV[lane] = sV[32 + lane];
+          hr_rings_shift(sE, sU, sV, ed);
           bprev = bal;
           __syncwarp();
         }
@@ -304,12 +264,7 @@ arma_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const ArimaArg
 #pragma unroll
   for (int k = 0; k < MA_MAX; ++k) th[k] = hr_ok && k < q ? s_beta[warp][p + k] : 0.f;
   if (live) {
-    if (hr.theta != nullptr && lane < MA_MAX) {
-      float v = 0.f;
-#pragma unroll
-      for (int k = 0; k < MA_MAX; ++k) v = lane == k ? th[k] : v;
-      hr.theta[row * MA_MAX + lane] = v;
-    }
+    store_row(hr.theta, row, lane, th);
     if (lane == 0 && hr.ma_order != nullptr) hr.ma_order[row] = hr_ok ? q : 0;
     if (hr_ok) {
       if (ar.phi != nullptr && lane < AR_MAX) {
@@ -335,13 +290,13 @@ arma_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const ArimaArg
   for (int k = 0; k < MA_MAX; ++k) he[k] = 0.f;
   double sse = 0.0;
   bprev = 0u;
-  float l1 = arma_qnan(), l2 = arma_qnan();
+  float l1 = qnan(), l2 = qnan();
   if (hr_ok && dd > 0) {
     const int i1 = dd - 1, i2 = dd - 2;
     const float v1 = __ldg(yr + i1);
-    const float v2 = i2 >= 0 ? __ldg(yr + i2) : arma_qnan();
-    l1 = finite_f(v1) ? v1 : arma_qnan();
-    l2 = finite_f(v2) ? v2 : arma_qnan();
+    const float v2 = i2 >= 0 ? __ldg(yr + i2) : qnan();
+    l1 = finite_f(v1) ? v1 : qnan();
+    l2 = finite_f(v2) ? v2 : qnan();
   }
   for (int c0 = 0; c0 < endB; c0 += TC) {
     stage(s_a, s_nz, d, ar, c0);
@@ -425,7 +380,7 @@ arma_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const ArimaArg
           const uint32_t lbal = __ballot_sync(0xffffffffu, lobs);
           if (lbal == 0xffffffffu) {
             const float p1 = __shfl_up_sync(0xffffffffu, lv, 1), p2 = __shfl_up_sync(0xffffffffu, lv, 2);
-            yh = arma_integrate(zh, lane >= 1 ? p1 : l1, lane >= 2 ? p2 : (lane == 1 ? l1 : l2), dd);
+            yh = integrate(zh, lane >= 1 ? p1 : l1, lane >= 2 ? p2 : (lane == 1 ? l1 : l2), dd);
             l1 = __shfl_sync(0xffffffffu, lv, 31);
             l2 = __shfl_sync(0xffffffffu, lv, 30);
           } else {
@@ -433,7 +388,7 @@ arma_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const ArimaArg
             const int jn = min(32, endB - t0);
 #pragma unroll 1
             for (int j = 0; j < jn; ++j) {
-              const float hj = arma_integrate(__shfl_sync(0xffffffffu, zh, j), l1, l2, dd);
+              const float hj = integrate(__shfl_sync(0xffffffffu, zh, j), l1, l2, dd);
               const float yj = __shfl_sync(0xffffffffu, lv, j);
               const float nl = (lbal >> j) & 1u ? yj : hj;
               if (lane == j) yh = hj;

@@ -12,7 +12,8 @@
 //              scores the dynamic forecast of the held-out levels;
 //     choice   the first minimum over the lanes, compared strictly with the running best;
 //     pass B   arma_kernel's, with the winner, only for the rows this launch leads.
-// A kernel of its own rather than a template of arma_kernel: wrapping moved the wrapped kernel's registers (4.14).
+// The ring shift and the small helpers come from ar_common.cuh; the blocks it has in common with arma_kernel stay written
+// out in each kernel, for the reason arma.cu gives.
 #include "ar_common.cuh"
 
 // timing builds only (scripts/bench_arma_select.py --split): 1 ends the kernel after pass A and step 1, 2 after pass A2
@@ -24,43 +25,15 @@
 namespace mmf {
 namespace {
 
-constexpr int MA_MAX = MMF_MA_MAX;
 constexpr int NR = AR_MAX + MA_MAX;        // regressors of a candidate, at most
-
-__device__ __forceinline__ float hs_qnan() { return __int_as_float(0x7fc00000); }
-
-// yhat_t from zhat_t and the filled levels ytilde_{t-1} (l1), ytilde_{t-2} (l2), in the order include/mmf.h states
-__device__ __forceinline__ float hs_integrate(float zh, float l1, float l2, int d) {
-  return d == 1 ? __fadd_rn(zh, l1) : __fsub_rn(__fadd_rn(zh, __fmul_rn(2.f, l1)), l2);
-}
-
-__device__ __forceinline__ double hs_warp_sum(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-// step-down (reverse Levinson) of 1 - sum_j a_j z^j, a[0 .. k): true when every |kappa| < MMF_AR_KAPPA_MAX
-template <int N>
-__device__ bool hs_step_down_ok(double (&a)[N], int k) {
-  for (int j = k; j >= 1; --j) {
-    const double kap = a[j - 1];
-    if (!(fabs(kap) < (double)MMF_AR_KAPPA_MAX)) return false;
-    const double den = 1.0 - kap * kap;
-    double nxt[N];
-    for (int i = 1; i < j; ++i) nxt[i - 1] = (a[i - 1] + kap * a[j - i - 1]) / den;
-    for (int i = 1; i < j; ++i) a[i - 1] = nxt[i - 1];
-  }
-  return true;
-}
 
 // A row set with pmax e lags and q eps^ lags orders its regressors e_{t-1..t-pmax}, eps^_{t-1..t-q}, then the
 // target e_t.  Its normal equations are the upper triangle, column-major, without the target's own square.  Source
 // code of a regressor: k for e_{t-k} (0: the target), 16 + k for eps^_{t-k}.
-__device__ __forceinline__ uint32_t hs_src(int x, int pmax, int q) {
+__device__ __forceinline__ uint32_t reg_src(int x, int pmax, int q) {
   return x < pmax ? (uint32_t)(x + 1) : (x < pmax + q ? 16u + (uint32_t)(x - pmax + 1) : 0u);
 }
-__device__ __forceinline__ const double* hs_base(const double* sE, const double* sV, uint32_t code) {
+__device__ __forceinline__ const double* src_base(const double* sE, const double* sV, uint32_t code) {
   return (code & 16u ? sV : sE) + 32 - (int)(code & 15u);
 }
 
@@ -124,7 +97,7 @@ arma_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const A
     while ((j + 1) * (j + 2) / 2 <= idx) ++j;
     const int i = idx - j * (j + 1) / 2;
     const int pm = hs.rs_pmax[r], qq = hs.rs_q[r];
-    s_code[e] = (uint32_t)r | hs_src(i, pm, qq) << 8 | hs_src(j, pm, qq) << 16;
+    s_code[e] = (uint32_t)r | reg_src(i, pm, qq) << 8 | reg_src(j, pm, qq) << 16;
   }
 
   // this lane's candidate (lanes >= n_pq repeat the last one and never take part)
@@ -170,7 +143,7 @@ arma_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const A
   }
 
   // ---- step 1: Levinson-Durbin to order m with the kappa stop; lane i holds psi_{i+1} and r_{i+1}
-  acc0 = hs_warp_sum(acc0);
+  acc0 = warp_sum(acc0);
   colmask = __reduce_or_sync(0xffffffffu, colmask);
   uint32_t used = d.kept_mask & colmask;
   if (st == MMF_STATUS_RANKDEF) {
@@ -187,7 +160,7 @@ arma_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const A
     bool go = n_obs - k_used > m && r0 > 0.0;
     for (int j = 1; j <= m && go; ++j) {
       const double rr = __shfl_sync(0xffffffffu, rl, (j - lane - 2) & 31);     // r_{j - (lane + 1)}
-      const double num = __shfl_sync(0xffffffffu, rl, j - 1) - hs_warp_sum(lane + 1 < j ? psi * rr : 0.0);
+      const double num = __shfl_sync(0xffffffffu, rl, j - 1) - warp_sum(lane + 1 < j ? psi * rr : 0.0);
       const double kap = num / var;
       if (fabs(kap) >= (double)MMF_AR_KAPPA_MAX) {
         go = false;
@@ -236,7 +209,7 @@ arma_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const A
           while (miss) {
             const int j = __ffs(miss) - 1;
             miss &= miss - 1u;
-            const double v = hs_warp_sum(lane < m_i ? psi * sU[31 + j - lane] : 0.0);
+            const double v = warp_sum(lane < m_i ? psi * sU[31 + j - lane] : 0.0);
             if (lane == 0) sU[32 + j] = v;
             __syncwarp();
           }
@@ -262,8 +235,8 @@ arma_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const A
             const uint32_t code = s_code[e];
             uint32_t rm = s_rm[warp][code & 0xffu];
             if (rm == 0u) continue;
-            const double* bi = hs_base(sE, sV, (code >> 8) & 0xffu);
-            const double* bj = hs_base(sE, sV, code >> 16);
+            const double* bi = src_base(sE, sV, (code >> 8) & 0xffu);
+            const double* bj = src_base(sE, sV, code >> 16);
             double acc = sG[e];
             while (rm) {
               const int j = __ffs(rm) - 1;
@@ -273,9 +246,7 @@ arma_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const A
             sG[e] = acc;
           }
           __syncwarp();
-          sE[lane] = ed;
-          sU[lane] = sU[32 + lane];
-          sV[lane] = sV[32 + lane];
+          hr_rings_shift(sE, sU, sV, ed);
           bprev = bal;
           __syncwarp();
         }
@@ -321,7 +292,7 @@ arma_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const A
       double fa[AR_MAX], fm[MA_MAX];
       for (int i = 0; i < p; ++i) fa[i] = w[i];
       for (int i = 0; i < q; ++i) fm[i] = -w[p + i];
-      ok = hs_step_down_ok(fa, p) && hs_step_down_ok(fm, q);
+      ok = step_down_ok(fa, p) && step_down_ok(fm, q);
     }
 #pragma unroll
     for (int k = 0; k < AR_MAX; ++k) f[k] = ok && k < p ? (float)w[k] : 0.f;
@@ -348,12 +319,12 @@ arma_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const A
     for (int k = 0; k < AR_MAX; ++k) hu[k] = 0.f;
 #pragma unroll
     for (int k = 0; k < MA_MAX; ++k) he[k] = 0.f;
-    float l1 = hs_qnan(), l2 = hs_qnan();  // this lane's filled levels ytilde_{t-1}, ytilde_{t-2}
+    float l1 = qnan(), l2 = qnan();  // this lane's filled levels ytilde_{t-1}, ytilde_{t-2}
     if (walk && dd > 0) {
       const float v1 = __ldg(yr + dd - 1);
-      const float v2 = dd >= 2 ? __ldg(yr + dd - 2) : hs_qnan();
-      l1 = finite_f(v1) ? v1 : hs_qnan();
-      l2 = finite_f(v2) ? v2 : hs_qnan();
+      const float v2 = dd >= 2 ? __ldg(yr + dd - 2) : qnan();
+      l1 = finite_f(v1) ? v1 : qnan();
+      l2 = finite_f(v2) ? v2 : qnan();
     }
     for (int c0 = 0; c0 < hendz; c0 += TC) {
       stage(s_a, s_nz, d, ar, c0);
@@ -400,7 +371,7 @@ arma_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const A
               xj = oj ? ej - pj : 0.f;
             }
             const float zh = fj + pr;
-            const float hj = dd == 0 ? zh : hs_integrate(zh, l1, l2, dd);
+            const float hj = dd == 0 ? zh : integrate(zh, l1, l2, dd);
             const int tj = t0 + j + dd;                          // level row
             if (tj >= TL && finite_f(yj) && finite_f(hj)) {      // held-out row: score the dynamic forecast
               const double df = (double)yj - (double)hj;
@@ -430,7 +401,7 @@ arma_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const A
       __syncthreads();
     }
   }
-  const double mse = ok && cnt > 0 ? sse / (double)cnt : __longlong_as_double(0x7ff8000000000000ll);
+  const double mse = ok && cnt > 0 ? sse / (double)cnt : dnan();
 
   // ---- this launch's first minimum in list order (q, then p), then strictly below the running best.  A candidate that
   // fails the gate forecasts as (p, d, 0), whose score the running best already holds: it never leads
@@ -486,7 +457,7 @@ arma_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const A
       }
       // the requested levels t < d, which have no prediction
       const int n_nan = min(a.n_pred, dd - a.pred_start);
-      for (int k = lane; k < n_nan; k += 32) a.out[row * a.ld_out + k] = hs_qnan();
+      for (int k = lane; k < n_nan; k += 32) a.out[row * a.ld_out + k] = qnan();
     } else if (q0_lead || first) {
       // the leader has q = 0 (arima_select_kernel of this d wrote its other outputs), or no candidate is eligible yet
       if (lane == 0) {
@@ -511,12 +482,12 @@ arma_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const A
   for (int k = 0; k < MA_MAX; ++k) he[k] = 0.f;
   double sseB = 0.0;
   bprev = 0u;
-  float l1 = hs_qnan(), l2 = hs_qnan();
+  float l1 = qnan(), l2 = qnan();
   if (lead && dd > 0) {
     const float v1 = __ldg(yr + dd - 1);
-    const float v2 = dd >= 2 ? __ldg(yr + dd - 2) : hs_qnan();
-    l1 = finite_f(v1) ? v1 : hs_qnan();
-    l2 = finite_f(v2) ? v2 : hs_qnan();
+    const float v2 = dd >= 2 ? __ldg(yr + dd - 2) : qnan();
+    l1 = finite_f(v1) ? v1 : qnan();
+    l2 = finite_f(v2) ? v2 : qnan();
   }
   for (int c0 = 0; c0 < endB; c0 += TC) {
     stage(s_a, s_nz, d, ar, c0);
@@ -598,7 +569,7 @@ arma_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const A
           const uint32_t lbal = __ballot_sync(0xffffffffu, lobs);
           if (lbal == 0xffffffffu) {
             const float p1 = __shfl_up_sync(0xffffffffu, lv, 1), p2 = __shfl_up_sync(0xffffffffu, lv, 2);
-            yh = hs_integrate(zh, lane >= 1 ? p1 : l1, lane >= 2 ? p2 : (lane == 1 ? l1 : l2), dd);
+            yh = integrate(zh, lane >= 1 ? p1 : l1, lane >= 2 ? p2 : (lane == 1 ? l1 : l2), dd);
             l1 = __shfl_sync(0xffffffffu, lv, 31);
             l2 = __shfl_sync(0xffffffffu, lv, 30);
           } else {
@@ -606,7 +577,7 @@ arma_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const A
             const int jn = min(32, endB - t0);
 #pragma unroll 1
             for (int j = 0; j < jn; ++j) {
-              const float hj = hs_integrate(__shfl_sync(0xffffffffu, zh, j), l1, l2, dd);
+              const float hj = integrate(__shfl_sync(0xffffffffu, zh, j), l1, l2, dd);
               const float yj = __shfl_sync(0xffffffffu, lv, j);
               const float nl = (lbal >> j) & 1u ? yj : hj;
               if (lane == j) yh = hj;
@@ -620,7 +591,7 @@ arma_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const A
     }
     __syncthreads();
   }
-  sseB = hs_warp_sum(sseB);
+  sseB = warp_sum(sseB);
   if (lead && lane == 0 && ar.sigma != nullptr) ar.sigma[row] = (float)sqrt(sseB / (double)nRw);
 }
 

@@ -14,6 +14,14 @@ Workloads (synthetic daily demand, 1,095 days, 28-day horizon):
   ragged64         64 calendars of 400 to 1,095 days in one ragged launch
   se               the standard-error call
   backtest4        a backtest at K = 4 origins
+and the ARIMA-family calls, each on the gap-free series (.clean), missing2 (.missing2) and gaps10 (.gaps10):
+  ar3, ar3h        AR(3) errors in future mode, and in holdout mode (every date) on the first n / 8 series
+  arsel            AR order selection over (0 .. 4), 28 held-out days
+  arima210, arima120  ARIMA(2, 1, 0) and ARIMA(1, 2, 0) errors
+  arimasel         (p, d) selection over (0 .. 4) x (0, 1, 2)
+  arma111, arma102    ARIMA(1, 1, 1) and ARMA(1, 0, 2) errors
+  armasel          (p, d, q) selection over (0, 1, 2) x (0, 1) x (0, 1, 2)
+  arimase          the standard errors of ARIMA(2, 1, 0)
 """
 import argparse
 import os
@@ -85,6 +93,26 @@ def produce(path, n):
     r = engb.backtest(yg)
     keep("backtest4", **r)
     engb.close()
+
+    # ARIMA family: future mode on the whole history; selection and holdout mode with the last H days held out
+    engf = mmf.ForecastEngine(device=0)
+    _, ps, npred = engf.plan_calendar(start, T, "D", H, "future", max_diff=2)
+    engh = mmf.ForecastEngine(device=0)
+    _, psh, nph = engh.plan_calendar(start, T, "D", H, "holdout", max_diff=2)
+    tf = T - H
+    for tag, ys in (("clean", y), ("missing2", ym), ("gaps10", yg)):
+        keep(f"ar3.{tag}", **engf.fit_forecast_ar(ys, 3, ps, npred))
+        keep(f"ar3h.{tag}", **engh.fit_forecast_ar(ys[: n // 8], 3, psh, nph))
+        keep(f"arsel.{tag}", **engh.fit_select_ar(ys, H, (0, 1, 2, 3, 4), tf, H))
+        keep(f"arima210.{tag}", **engf.fit_forecast_arima(ys, 2, 1, ps, npred))
+        keep(f"arima120.{tag}", **engf.fit_forecast_arima(ys, 1, 2, ps, npred))
+        keep(f"arimasel.{tag}", **engh.fit_select_arima(ys, H, (0, 1, 2, 3, 4), (0, 1, 2), tf, H))
+        keep(f"arma111.{tag}", **engf.fit_forecast_arma(ys, 1, 1, 1, ps, npred))
+        keep(f"arma102.{tag}", **engf.fit_forecast_arma(ys, 1, 2, 0, ps, npred))
+        keep(f"armasel.{tag}", **engh.fit_select_arma(ys, H, (0, 1, 2), (0, 1), (0, 1, 2), tf, H))
+        keep(f"arimase.{tag}", **engf.fit_forecast_arima(ys, 2, 1, ps, npred, want_se=True))
+    engf.close()
+    engh.close()
     torch.cuda.synchronize()
     np.savez(path, **out)
 
@@ -120,7 +148,7 @@ def main():
     for k in sorted(set(a.files) | set(b.files)):
         if k not in a.files or k not in b.files or not same_bits(a[k], b[k]):
             bad.append(k)
-        print(f"{k:24s} {'DIFFERS' if k in bad else 'bit-identical'}", flush=True)
+        print(f"{k:32s} {'DIFFERS' if k in bad else 'bit-identical'}", flush=True)
     if bad:
         sys.exit(f"{len(bad)} outputs differ between {args.lib_a} and {args.lib_b}: {', '.join(bad)}")
     print(f"all {len(a.files)} outputs bit-identical")

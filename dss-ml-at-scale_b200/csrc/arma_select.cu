@@ -595,6 +595,44 @@ arma_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const A
   if (lead && lane == 0 && ar.sigma != nullptr) ar.sigma[row] = (float)sqrt(sseB / (double)nRw);
 }
 
+// Normal-equation entries of the list orders = {p : bit p of order_bits}, mas = {0} and {q : bit q - 1 of ma_bits}, by
+// select_arima_call's rule: every (p, q >= 1) pair joins row set R(q, L = max(p, q)), whose p_max is the largest p
+// in it, and a row set keeps (p_max + q + 1)(p_max + q + 2) / 2 - 1 entries.
+constexpr int armasel_entries(int order_bits, int ma_bits) {
+  int pmax[MMF_MA_MAX + 1][MMF_AR_MAX + 1] = {};   // p_max + 1 of R(q, L); 0: no such row set
+  for (int q = 1; q <= MMF_MA_MAX; ++q)
+    for (int p = 0; p <= MMF_AR_MAX; ++p)
+      if ((ma_bits >> (q - 1) & 1) && (order_bits >> p & 1)) {
+        int& r = pmax[q][p > q ? p : q];
+        r = r > p + 1 ? r : p + 1;
+      }
+  int n = 0;
+  for (int q = 1; q <= MMF_MA_MAX; ++q)
+    for (int L = 0; L <= MMF_AR_MAX; ++L)
+      if (pmax[q][L] > 0) n += (pmax[q][L] + q) * (pmax[q][L] + q + 1) / 2 - 1;
+  return n;
+}
+
+constexpr int popcount_c(int v) { return v ? (v & 1) + popcount_c(v >> 1) : 0; }
+
+// the most entries of any list the ABI accepts: orders a nonempty subset of 0..MMF_AR_MAX, mas {0} plus a nonempty
+// subset of 1..MMF_MA_MAX, at most MMF_ARMASEL_MAX_PQ pairs (p, q >= 1)
+constexpr int armasel_max_entries() {
+  int best = 0;
+  for (int o = 1; o < 1 << (MMF_AR_MAX + 1); ++o)
+    for (int m = 1; m < 1 << MMF_MA_MAX; ++m)
+      if (popcount_c(o) * popcount_c(m) <= MMF_ARMASEL_MAX_PQ) {
+        const int e = armasel_entries(o, m);
+        best = best > e ? best : e;
+      }
+  return best;
+}
+
+constexpr int ARMASEL_MAX_ENT = armasel_max_entries();
+// (1..8) x (0..4): 26 row sets; (0..8) x (0..3) (769 entries) and the reference grid (215) stay below 48 KB
+static_assert(ARMASEL_MAX_ENT == 1099, "the largest accepted (orders, mas) list has 1,099 entries (74,732 B)");
+static_assert(armasel_entries(0x1f, 0xf) == 215 && armasel_entries(0x1ff, 0x7) == 769, "DESIGN.md section 4.18");
+
 }  // namespace
 
 size_t arma_select_smem_bytes(int n_ent) { return (size_t)n_ent * (WARPS * sizeof(double) + sizeof(uint32_t)); }
@@ -602,10 +640,13 @@ size_t arma_select_smem_bytes(int n_ent) { return (size_t)n_ent * (WARPS * sizeo
 cudaError_t launch_arma_select(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
                                const ArimaSelArgs& sel, const ArmaSelArgs& hs, cudaStream_t s) {
   if (a.n <= 0) return cudaSuccess;
+  if (hs.n_ent > ARMASEL_MAX_ENT) return cudaErrorInvalidValue;
   const size_t smem = arma_select_smem_bytes(hs.n_ent);
   if (smem > 48 * 1024) {
-    const cudaError_t e =
-        cudaFuncSetAttribute(arma_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    // the attribute is per function and process-wide: always the same value, the largest any call needs, so that a
+    // context on another host thread cannot lower it between this call's set and its launch
+    const cudaError_t e = cudaFuncSetAttribute(arma_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               (int)arma_select_smem_bytes(ARMASEL_MAX_ENT));
     if (e != cudaSuccess) return e;
   }
   const int64_t grid = (a.n + WARPS - 1) / WARPS;

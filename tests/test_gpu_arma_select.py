@@ -32,8 +32,9 @@ from test_gpu_edges import _le, _same_bits
 pytestmark = pytest.mark.gpu
 
 REF = ((0, 1, 2, 3, 4), (0, 1, 2), (0, 1, 2, 3, 4))
+# the last grid is the largest the ABI accepts: 32 (p, q >= 1) pairs, every lane a candidate, 26 row sets, 74,732 B
 GRIDS = (REF, (tuple(range(9)), (0, 1, 2), (0, 1, 2, 3)), ((1,), (1,), (0, 1)), ((0,), (2,), (0, 4)),
-         ((0, 1, 2, 3, 4), (0, 1, 2), (0,)))
+         ((0, 1, 2, 3, 4), (0, 1, 2), (0,)), (tuple(range(1, 9)), (0, 1, 2), (0, 1, 2, 3, 4)))
 SENT_F, SENT_I = float(np.float32(PATTERN)), -7
 
 

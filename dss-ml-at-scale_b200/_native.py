@@ -23,6 +23,8 @@ ARSEL_MAX_CAND = 9                                                         # MMF
 DIFF_MAX = 2                                                               # MMF_DIFF_MAX
 MA_MAX, HR_LONG_MAX, HR_PIVOT_TOL = 4, 32, 1e-5                            # MMF_MA_MAX, MMF_HR_LONG_MAX, MMF_HR_PIVOT_TOL
 ARMASEL_MAX_PQ = 32                                                        # MMF_ARMASEL_MAX_PQ
+CSS_LAMBDA0, CSS_LAMBDA_MAX, CSS_RTOL = 1e-3, 1e10, 1e-6                   # MMF_CSS_LAMBDA0, _LAMBDA_MAX, _RTOL
+CSS_ITER_DEFAULT, CSS_ITER_MAX = 20, 64                                    # MMF_CSS_ITER_DEFAULT, MMF_CSS_ITER_MAX
 DT_F32, DT_I16, DT_U16, DT_I32 = 0, 1, 2, 3
 INT_DTYPES = {"int16": DT_I16, "uint16": DT_U16, "int32": DT_I32}          # series element types besides float32
 INT_MISSING = {"int16": -32768, "uint16": 65535, "int32": -2147483648}     # the value that means "missing" in each
@@ -33,7 +35,7 @@ EXPORTS = (
     "mmf_set_stream", "mmf_synchronize", "mmf_plan_design", "mmf_pin_scratch", "mmf_get_whitening",
     "mmf_fit_forecast_f32", "mmf_fit_forecast_int", "mmf_fit_forecast_se_f32", "mmf_fit_forecast_ar_f32",
     "mmf_fit_select_ar_f32", "mmf_plan_arima", "mmf_fit_forecast_arima_f32", "mmf_fit_select_arima_f32",
-    "mmf_fit_forecast_arma_f32", "mmf_fit_select_arma_f32", "mmf_arima_se_f32",
+    "mmf_fit_forecast_arma_f32", "mmf_fit_forecast_arma_css_f32", "mmf_fit_select_arma_f32", "mmf_arima_se_f32",
     "mmf_plan_calendars", "mmf_fit_forecast_ragged_f32",
     "mmf_plan_backtest", "mmf_backtest_f32",
     "mmf_fit_forecast_bcast_f32", "mmf_fit_select_forecast_f32", "mmf_pack_hash_utf8", "mmf_pack_hash_i32",
@@ -130,6 +132,11 @@ def load() -> C.CDLL:
         C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
         C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
         C.POINTER(MmfStats),
+    ]
+    lib.mmf_fit_forecast_arma_css_f32.argtypes = [
+        C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+        C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(MmfStats),
     ]
     lib.mmf_fit_select_arima_f32.argtypes = [
         C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.POINTER(C.c_int32), C.c_int32,

@@ -219,6 +219,8 @@ struct mmf_ctx {
   ArimaSelBest* d_asel_best = nullptr;  size_t asel_best_cap = 0;   // (p, d) selection, per slab: running best,
   int32_t* d_asel_status = nullptr;  size_t asel_status_cap = 0;    // and the status of the fit of the current d
   float* d_hsel_q0 = nullptr;  size_t hsel_q0_cap = 0;     // (p, d, q) selection, per slab: the q = 0 scores
+  float* d_css_hr = nullptr;  size_t css_hr_cap = 0;       // CSS calls, per slab: the HR phi / theta / ma_order the
+                                                           // caller did not ask for
   float* d_bt_mom = nullptr;  size_t bt_mom_cap = 0;   // backtest scratch, per slab: moments at the earlier origins,
   SolveRec* d_bt_recs = nullptr;  size_t bt_recs_cap = 0;   // [K][slab] records, [K][slab] work lists,
   int64_t* d_bt_rows = nullptr;  size_t bt_rows_cap = 0;
@@ -521,14 +523,14 @@ int build_multi(MultiPlan& m, const double* X_all, int32_t n_cal, const int32_t*
 // (asel != nullptr) run this once per listed d and end in arima_select_kernel; their d = 0 pass (arima->d == 0) fits y
 // itself with the mmf_plan_design plan; (p, d, q) selection calls (hsel != nullptr, with asel) add arma_select_kernel
 // behind it.  ARMA calls (arma != nullptr, with ar) run arma_kernel behind ar_kernel (d = 0, arima == nullptr) or
-// arima_kernel.
+// arima_kernel; CSS calls (css != nullptr, with arma) add arma_css_kernel behind arma_kernel.
 int run_device_slab(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, int64_t ld_y, int32_t pred_start,
                     int32_t n_pred, float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s,
                     int* launches, int* kernel_used, float* const* out_more, int n_out, int multimem,
                     const SelectArgs* sel, const SeArgs* se = nullptr, const ArArgs* ar = nullptr,
                     const ArSelArgs* arsel = nullptr, const ArimaArgs* arima = nullptr,
                     const ArimaSelArgs* asel = nullptr, const ArmaArgs* arma = nullptr,
-                    const ArmaSelArgs* hsel = nullptr) {
+                    const ArmaSelArgs* hsel = nullptr, const CssArgs* css = nullptr) {
   const DesignView d = view_of(plan);
   ArimaArgs ma{};
   if (arima != nullptr) {
@@ -647,6 +649,10 @@ int run_device_slab(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, i
       if (arima == nullptr) { mh.y = a.y; mh.ld_y = a.ld_y; mh.t_fit = d.t_fit; mh.d = 0; }
       CU_TRY(launch_arma(d, a, *ar, mh, *arma, s));
       ++*launches;
+      if (css != nullptr) {
+        CU_TRY(launch_arma_css(d, a, *ar, mh, *arma, *css, s));
+        ++*launches;
+      }
     }
   }
   if (many_pred) {
@@ -696,8 +702,20 @@ int run_device(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, int64_
                int* launches, int* kernel_used, float* const* out_more = nullptr, int n_out = 1, int multimem = 0,
                const SelectArgs* sel = nullptr, uint32_t* slab_pending = nullptr, const SeArgs* se = nullptr,
                const ArArgs* ar = nullptr, const ArSelArgs* arsel = nullptr, const ArimaArgs* arima = nullptr,
-               const ArmaArgs* arma = nullptr) {
+               const ArmaArgs* arma = nullptr, const CssArgs* css = nullptr) {
   const int64_t slab = slab_rows(plan, n);
+  // CSS calls read the HR (phi, theta, ma_order) back: what the caller did not ask for goes to per-slab scratch
+  float* hr_phi = nullptr;
+  float* hr_theta = nullptr;
+  int32_t* hr_ma = nullptr;
+  if (css != nullptr && (ar->phi == nullptr || arma->theta == nullptr || arma->ma_order == nullptr)) {
+    const size_t per_row = (MMF_AR_MAX + MMF_MA_MAX + 1) * sizeof(float);
+    int rc = grow((void**)&ctx->d_css_hr, &ctx->css_hr_cap, (size_t)slab * per_row);
+    if (rc != MMF_OK) return rc;
+    hr_phi = ctx->d_css_hr;
+    hr_theta = hr_phi + (size_t)slab * MMF_AR_MAX;
+    hr_ma = reinterpret_cast<int32_t*>(hr_theta + (size_t)slab * MMF_MA_MAX);
+  }
   for (int64_t off = 0, i = 0; off < n; off += slab, ++i) {
     const int64_t m = std::min(slab, n - off);
     float* more[MAX_OUT - 1] = {};
@@ -719,6 +737,7 @@ int run_device(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, int64_
     if (ar != nullptr) {
       ar_slab = *ar;
       if (ar_slab.phi) ar_slab.phi += off * MMF_AR_MAX;
+      else if (css != nullptr) ar_slab.phi = hr_phi;
       if (ar_slab.order) ar_slab.order += off;
       if (ar_slab.sigma) ar_slab.sigma += off;
     }
@@ -733,13 +752,24 @@ int run_device(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, int64_
     if (arma != nullptr) {
       arma_slab = *arma;
       if (arma_slab.theta) arma_slab.theta += off * MMF_MA_MAX;
+      else if (css != nullptr) arma_slab.theta = hr_theta;
       if (arma_slab.ma_order) arma_slab.ma_order += off;
+      else if (css != nullptr) arma_slab.ma_order = hr_ma;
+    }
+    CssArgs css_slab{};
+    if (css != nullptr) {
+      css_slab = *css;
+      if (css_slab.css_start) css_slab.css_start += off;
+      if (css_slab.css) css_slab.css += off;
+      if (css_slab.css_stop) css_slab.css_stop += off;
+      if (css_slab.iters) css_slab.iters += off;
     }
     const int rc = run_device_slab(ctx, plan, y + off * ld_y, m, ld_y, pred_start, n_pred, out + off * ld_out, ld_out,
                                    beta ? beta + off * P : nullptr, status + off, s, launches, kernel_used, more, n_out,
                                    multimem, sel != nullptr ? &sel_slab : nullptr, se != nullptr ? &se_slab : nullptr,
                                    ar != nullptr ? &ar_slab : nullptr, arsel != nullptr ? &arsel_slab : nullptr, arima,
-                                   nullptr, arma != nullptr ? &arma_slab : nullptr);
+                                   nullptr, arma != nullptr ? &arma_slab : nullptr, nullptr,
+                                   css != nullptr ? &css_slab : nullptr);
     if (rc != MMF_OK) return rc;
     if (slab_pending != nullptr) {
       if (*kernel_used == MMF_KERNEL_TC)
@@ -847,7 +877,7 @@ int mmf_destroy(mmf_ctx* ctx) {
   free_bt(ctx->bt);
   free_arima(ctx->arima);
   cudaFree(ctx->d_z);
-  cudaFree(ctx->d_asel_best); cudaFree(ctx->d_asel_status); cudaFree(ctx->d_hsel_q0);
+  cudaFree(ctx->d_asel_best); cudaFree(ctx->d_asel_status); cudaFree(ctx->d_hsel_q0); cudaFree(ctx->d_css_hr);
   cudaFree(ctx->d_bt_mom); cudaFree(ctx->d_bt_recs); cudaFree(ctx->d_bt_rows); cudaFree(ctx->d_bt_ctr); cudaFree(ctx->d_bt_pred);
   for (int i = 0; i < NBUF; ++i) {
     Staging& s = ctx->st[i];
@@ -1320,7 +1350,7 @@ int mmf_fit_forecast_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
 static int run_ar_call(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, int64_t ld_y, int32_t pred_start,
                        int32_t n_pred, float* out_pred, int64_t ld_out, int32_t* out_status, const ArArgs& ar,
                        const ArSelArgs* arsel, const ArimaArgs* arima, mmf_stats* stats,
-                       const ArmaArgs* arma = nullptr) {
+                       const ArmaArgs* arma = nullptr, const CssArgs* css = nullptr) {
   int32_t* status = out_status;
   if (!status) {
     int rc = grow_status_scratch(ctx, n, ctx->stream);
@@ -1341,7 +1371,8 @@ static int run_ar_call(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n
   int launches = 0, kernel_used = 0;
   if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, ctx->stream));
   int rc = run_device(ctx, plan, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, nullptr, status, ctx->stream,
-                      &launches, &kernel_used, nullptr, 1, 0, nullptr, slab_pending, nullptr, &ar, arsel, arima, arma);
+                      &launches, &kernel_used, nullptr, 1, 0, nullptr, slab_pending, nullptr, &ar, arsel, arima, arma,
+                      css);
   if (rc != MMF_OK) return rc;
   if (stats) {
     CU_TRY(cudaEventRecord(ctx->ev_k1, ctx->stream));
@@ -1514,12 +1545,14 @@ int mmf_fit_forecast_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t 
   return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, &ma, stats);
 }
 
-// ---- regression with ARIMA(p, d, q) errors (DESIGN.md section 2 item 13) -------------------------------------------------
-int mmf_fit_forecast_arma_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
-                              int32_t diff_order, int32_t ma_order, int32_t long_order, int32_t pred_start,
-                              int32_t n_pred, float* out_pred, int64_t ld_out, float* out_phi, float* out_theta,
-                              int32_t* out_order, int32_t* out_ma_order, float* out_sigma, int32_t* out_status,
-                              mmf_stats* stats) {
+// ---- regression with ARIMA(p, d, q) errors (DESIGN.md section 2 items 13, 16) --------------------------------------------
+// The HR call (css == nullptr) and the CSS call: the same checks, plans and launches; the CSS call adds arma_css_kernel
+// behind arma_kernel in every slab.
+static int arma_call(mmf_ctx* ctx, const char* name, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
+                     int32_t diff_order, int32_t ma_order, int32_t long_order, int32_t pred_start, int32_t n_pred,
+                     float* out_pred, int64_t ld_out, float* out_phi, float* out_theta, int32_t* out_order,
+                     int32_t* out_ma_order, float* out_sigma, int32_t* out_status, mmf_stats* stats,
+                     const CssArgs* css) {
   if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
   GrowScope grow_scope(ctx);
   if (n < 0) return fail(MMF_E_INVALID, "n < 0");
@@ -1551,8 +1584,10 @@ int mmf_fit_forecast_arma_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t l
   if (!is_device_ptr(y) || !is_device_ptr(out_pred) || (out_phi && !is_device_ptr(out_phi)) ||
       (out_theta && !is_device_ptr(out_theta)) || (out_order && !is_device_ptr(out_order)) ||
       (out_ma_order && !is_device_ptr(out_ma_order)) || (out_sigma && !is_device_ptr(out_sigma)) ||
-      (out_status && !is_device_ptr(out_status)))
-    return fail(MMF_E_UNSUPPORTED, "mmf_fit_forecast_arma_f32 takes device buffers only");
+      (out_status && !is_device_ptr(out_status)) ||
+      (css && ((css->css_start && !is_device_ptr(css->css_start)) || (css->css && !is_device_ptr(css->css)) ||
+               (css->css_stop && !is_device_ptr(css->css_stop)) || (css->iters && !is_device_ptr(css->iters)))))
+    return fail(MMF_E_UNSUPPORTED, "%s takes device buffers only", name);
   ArArgs ar{};
   ar.p = ar_order; ar.phi = out_phi; ar.order = out_order; ar.sigma = out_sigma; ar.nz = pl.d_nz;
   ArmaArgs hr{};
@@ -1565,10 +1600,38 @@ int mmf_fit_forecast_arma_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t l
   hr.theta = out_theta; hr.ma_order = out_ma_order;
   if (diff_order == 0)
     return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, nullptr,
-                       stats, &hr);
+                       stats, &hr, css);
   ArimaArgs ma{};
   ma.y = y; ma.ld_y = ld_y; ma.t_fit = ap.t_fit; ma.d = diff_order;
-  return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, &ma, stats, &hr);
+  return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, &ma, stats, &hr,
+                     css);
+}
+
+int mmf_fit_forecast_arma_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
+                              int32_t diff_order, int32_t ma_order, int32_t long_order, int32_t pred_start,
+                              int32_t n_pred, float* out_pred, int64_t ld_out, float* out_phi, float* out_theta,
+                              int32_t* out_order, int32_t* out_ma_order, float* out_sigma, int32_t* out_status,
+                              mmf_stats* stats) {
+  return arma_call(ctx, "mmf_fit_forecast_arma_f32", y, n, ld_y, ar_order, diff_order, ma_order, long_order, pred_start,
+                   n_pred, out_pred, ld_out, out_phi, out_theta, out_order, out_ma_order, out_sigma, out_status, stats,
+                   nullptr);
+}
+
+int mmf_fit_forecast_arma_css_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
+                                  int32_t diff_order, int32_t ma_order, int32_t long_order, int32_t max_iter,
+                                  int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out, float* out_phi,
+                                  float* out_theta, int32_t* out_order, int32_t* out_ma_order, float* out_sigma,
+                                  int32_t* out_status, float* out_css_start, float* out_css, int32_t* out_css_stop,
+                                  int32_t* out_iters, mmf_stats* stats) {
+  if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
+  if (max_iter < 0 || max_iter > MMF_CSS_ITER_MAX)
+    return fail(MMF_E_INVALID, "max_iter=%d outside [0,%d]", max_iter, MMF_CSS_ITER_MAX);
+  CssArgs css{};
+  css.max_iter = max_iter == 0 ? MMF_CSS_ITER_DEFAULT : max_iter;
+  css.css_start = out_css_start; css.css = out_css; css.css_stop = out_css_stop; css.iters = out_iters;
+  return arma_call(ctx, "mmf_fit_forecast_arma_css_f32", y, n, ld_y, ar_order, diff_order, ma_order, long_order,
+                   pred_start, n_pred, out_pred, ld_out, out_phi, out_theta, out_order, out_ma_order, out_sigma,
+                   out_status, stats, &css);
 }
 
 // ---- standard errors of the ARIMA-family forecasts (DESIGN.md section 2 item 15) ---------------------------------------

@@ -295,6 +295,20 @@ struct ArmaArgs {
 cudaError_t launch_arma(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
                         const ArmaArgs& hr, cudaStream_t s);
 
+// ARIMA(p, d, q) errors by conditional least squares (arma_css.cu, DESIGN.md section 2 item 16): arma_css_kernel runs
+// behind arma_kernel in the same slab (same fit hand-off, z'), reads the HR (phi, theta) from ArArgs::phi /
+// ArmaArgs::theta and the gated rows from ArmaArgs::ma_order (caller buffers or scratch: never null for this kernel), and
+// overwrites the outputs of the rows that accepted a step
+struct CssArgs {
+  int32_t max_iter;                       // passes per series, 1 .. MMF_CSS_ITER_MAX (resolved: never 0)
+  float* css_start;                       // nullable [n]: S at the HR estimate
+  float* css;                             // nullable [n]: S at the shipped estimate
+  int32_t* css_stop;                      // nullable [n]: 1 converged, 2 stalled, 3 budget, 0 not refined
+  int32_t* iters;                         // nullable [n]: passes run
+};
+cudaError_t launch_arma_css(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
+                            const ArmaArgs& hr, const CssArgs& cs, cudaStream_t s);
+
 // per-series (p, d, q) selection by hold-out MSE on levels (arma_select.cu, DESIGN.md section 2 item 14): one launch per
 // listed d, right behind that d's arima_select_kernel (same fit, z', gamma / c and running best), for the q >= 1 blocks.
 // Candidate lane c is the pair (pq_p[c], pq_q[c]), q-major; its normal equations are those of row set pq_rs[c], the rows

@@ -339,7 +339,7 @@ def _host(x):
 
 
 def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, interval=False, ar=None, diff=None,
-                 ma=None, want_se=False):
+                 ma=None, want_se=False, estimator=None):
     """Run the engine over every bucket: yields (bucket, out_days, n_pred, y_host, pred_host, se_host or None).
     ``interval``: prediction standard errors too (``fit_forecast_se``), one call per calendar bucket.
     ``ar``: regression with AR(ar) errors (``fit_forecast_ar``), one call per calendar bucket; a tuple of orders
@@ -350,7 +350,8 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
     ``ma``: regression with ARIMA(ar, diff or 0, ma) errors (``fit_forecast_arma``), one call per calendar bucket; a
     tuple of MA orders (with ``ar`` and ``diff`` tuples) chooses (p, d, q) per series by hold-out MSE over the last
     ``horizon`` rows (``fit_select_arma``).
-    ``want_se``: the ARIMA-family call's forecast standard errors too (``want_se=True``, DESIGN.md section 2 item 15)."""
+    ``want_se``: the ARIMA-family call's forecast standard errors too (``want_se=True``, DESIGN.md section 2 item 15).
+    ``estimator``: the fixed-order ARIMA(p, d, q) call's estimator (None: the engine's default, Hannan-Rissanen)."""
     se_kw = {"want_se": True} if want_se else {}
     if interval and select is not None:
         raise ValueError("interval= is not offered with select= (model selection returns point forecasts)")
@@ -374,7 +375,8 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
         elif ma is not None:
             from .engine import device_packed
             yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
-            res = eng.fit_forecast_arma(yd, ar, ma, diff or 0, pred_start, n_pred, **se_kw)
+            est_kw = {"estimator": estimator} if estimator is not None else {}
+            res = eng.fit_forecast_arma(yd, ar, ma, diff or 0, pred_start, n_pred, **se_kw, **est_kw)
             pred, se = _host(res["pred"]), (_host(res["se"]) if want_se else None)
         elif isinstance(diff, tuple):
             from .engine import device_packed
@@ -531,6 +533,23 @@ def _arma_orders(ma, ar, diff, select, interval, mode="holdout"):
     return int(ar), (int(diff) if diff else None), int(ma)
 
 
+def _estimator(estimator, ma, select, interval):
+    """validated ``estimator=`` of the fixed-order ARIMA(p, d, q) forecasts: None (Hannan-Rissanen, as before), "hr" or
+    "css" (DESIGN.md section 2 item 16).  It needs one MA order ``ma=q``."""
+    if estimator is None:
+        return None
+    if estimator not in ("hr", "css"):
+        raise ValueError(f"estimator must be 'hr' or 'css', got {estimator!r}")
+    if select is not None or interval is not None:
+        raise ValueError("estimator= is not offered with select= or interval= (ARMA forecasts come without either)")
+    if ma is None:
+        raise ValueError("estimator= needs one MA order ma=q in [1, 4] (it chooses how ARIMA(p, d, q) is estimated)")
+    if isinstance(ma, (list, tuple, np.ndarray)):
+        raise ValueError(f"estimator= is not offered with candidate MA orders (order selection scores Hannan-Rissanen "
+                         f"fits), got ma={ma!r}")
+    return estimator
+
+
 def _ar_orders_for(diff, ar, select, interval, mode):
     """``ar=`` validated against ``diff=``: one order in 0..8 for a single d, the tuple of candidate orders for a tuple
     of d's, and _ar_order's result without differencing"""
@@ -648,7 +667,7 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
                     freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                     engine: ForecastEngine | None = None, pack: str = "host", select=None,
                     null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None, ma=None,
-                    conf_int=None) -> pd.DataFrame:
+                    conf_int=None, estimator=None) -> pd.DataFrame:
     """Fit + forecast every group in ``pdf``; returns ``tuning_schema`` rows
     (keys..., Date, Demand, Demand_Fitted), groups in key order, dates ascending.
 
@@ -710,12 +729,18 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     uncertainty; NaN where ``Demand_Fitted`` is NaN).  Schema ``tuning_schema(interval=True)``.  Refused without
     ``ar=``, with ``interval=`` (the plain regression's band, a different quantity) or ``select=``, and for a level
     outside (0, 1).
+
+    ``estimator="css"`` with a fixed ``ma=q`` refines every gated series' Hannan-Rissanen (phi, theta) by conditional
+    least squares (``ForecastEngine.fit_forecast_arma(..., estimator="css")``, DESIGN.md section 2 item 16); schema
+    unchanged, ``conf_int=`` works as above.  ``estimator=None`` (or ``"hr"``) leaves everything as it was.  Refused
+    without ``ma=``, with candidate MA orders, ``select=`` or ``interval=``.
     """
     eng = engine or default_engine()
     keys = list(keys)
     fitted_col = value_col + "_Fitted"
     z = _z_of(interval)
     cz = _conf_z(conf_int, ar, select, interval)
+    est = _estimator(estimator, ma, select, interval)
     if ma is None:
         diff = _diff_order(diff, ar, select, interval, mode)
         ar = _ar_orders_for(diff, ar, select, interval, mode)
@@ -730,7 +755,7 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     parts, lengths = [], []
     for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
                                                               pack == "device", z is not None, ar, diff, ma,
-                                                              cz is not None):
+                                                              cz is not None, est):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n), n_pred)
         # key columns keep the dtype they came in with (no per-row string inference on N x T values)
@@ -822,15 +847,15 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
                    freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                    engine: ForecastEngine | None = None, pack: str = "host", select=None,
                    null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None, ma=None,
-                   conf_int=None):
+                   conf_int=None, estimator=None):
     """Arrow ``Table``/``RecordBatch`` in -> Arrow ``Table`` with ``tuning_schema`` out (the ``mapInArrow``
     flavour of the boundary).  No pandas frame of the rows on either side: keys are dictionary-encoded on the way
     in and expanded from a dictionary on the way out, dates and values are NumPy views of Arrow buffers.
     ``interval=level`` adds the ``{value}_Lower`` / ``{value}_Upper`` columns of ``forecast_groups`` (schema:
     ``tuning_schema(..., interval=True)``).  ``ar=p`` fits regression with AR(p) errors and ``ar=(0, 1, 2, 3, 4)`` chooses the order per series, as in
     ``forecast_groups``; ``diff=d`` with ``ar=p`` fits ARIMA(p, d, 0) errors as there, and ``ma=q`` ARIMA(p, d, q); tuples of ``ar``, ``diff`` and
-    ``ma`` choose (p, d, q) per series.  ``conf_int=level`` adds the same two columns for those forecasts, as in
-    ``forecast_groups``."""
+    ``ma`` choose (p, d, q) per series.  ``conf_int=level`` adds the same two columns for those forecasts, and
+    ``estimator="css"`` refines a fixed ``ma=q``'s estimate, as in ``forecast_groups``."""
     import pyarrow as pa
 
     if isinstance(table, pa.RecordBatch):
@@ -839,6 +864,7 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     keys = list(keys)
     z = _z_of(interval)
     cz = _conf_z(conf_int, ar, select, interval)
+    est = _estimator(estimator, ma, select, interval)
     if ma is None:
         diff = _diff_order(diff, ar, select, interval, mode)
         ar = _ar_orders_for(diff, ar, select, interval, mode)
@@ -850,7 +876,7 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     parts, lengths = [], []
     for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
                                                               pack == "device", z is not None, ar, diff, ma,
-                                                              cz is not None):
+                                                              cz is not None, est):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n, dtype=np.int32), n_pred)
         cols = []

@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define MMF_VERSION 111          /* 0.1.11 */
+#define MMF_VERSION 112          /* 0.1.12 */
 #define MMF_P 16                 /* design columns (zero-pad narrower designs) */
 #define MMF_PIVOT_TOL 1e-3f      /* per-series relative Cholesky pivot threshold */
 #define MMF_CAL_TOL 1e-10        /* aliasing threshold on the float64 calendar Gram */
@@ -46,6 +46,11 @@ extern "C" {
 #define MMF_HR_LONG_MAX 32       /* largest long AR order of the Hannan-Rissanen step 1 (one lag per lane of a warp) */
 #define MMF_HR_PIVOT_TOL 1e-5    /* a Hannan-Rissanen Cholesky pivot must exceed this x its Gram diagonal */
 #define MMF_ARMASEL_MAX_PQ 32    /* (p, q >= 1) candidate pairs per mmf_fit_select_arma_f32 call (one per lane of a warp) */
+#define MMF_CSS_LAMBDA0 1e-3     /* mmf_fit_forecast_arma_css_f32: the Levenberg-Marquardt damping of the first step */
+#define MMF_CSS_LAMBDA_MAX 1e10  /* ... a series stops (stalled) once its damping exceeds this */
+#define MMF_CSS_RTOL 1e-6        /* ... and (converged) when an accepted pass lowers S by at most this x S */
+#define MMF_CSS_ITER_DEFAULT 20  /* ... passes per series for max_iter = 0 */
+#define MMF_CSS_ITER_MAX 64      /* ... the largest max_iter accepted */
 
 /* return codes */
 #define MMF_OK 0
@@ -317,6 +322,40 @@ int mmf_fit_forecast_arma_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t l
                               int32_t n_pred, float* out_pred, int64_t ld_out, float* out_phi, float* out_theta,
                               int32_t* out_order, int32_t* out_ma_order, float* out_sigma, int32_t* out_status,
                               mmf_stats* stats);
+
+/* ---- ARIMA(p, d, q) errors by conditional least squares (DESIGN.md section 2 item 16) ---------------------------------
+ * mmf_fit_forecast_arma_css_f32: mmf_fit_forecast_arma_f32, then Levenberg-Marquardt refinement of every gated series'
+ * (phi, theta) on the conditional sum of squares (R's arima(method = "CSS") conditioning, with the gap rule above):
+ *   S(x) = sum over C = { s in [p, T) : e observed at s } of eps~_s(x)^2, eps~ the forecast recursion of
+ *   mmf_fit_forecast_arma_f32 from s = 0 (zero pre-sample, missing rows filled), evaluated in float64 from the fp32
+ *   residuals e; the Jacobian d eps~ / dx is exact, gaps included (a filled value depends on x);
+ *   start: x0 = the (phi, theta) the HR call ships (fp32).  One pass over the fit window evaluates S, g = J' eps~ and
+ *   H = J'J at an fp32 point (float64 sums); the first pass is at x0;
+ *   step: (H + lambda diag H) delta = -g by an in-order float64 Cholesky, lambda starting at MMF_CSS_LAMBDA0; the trial
+ *   point is x' = fp32(x + delta).  A pivot <= MMF_HR_PIVOT_TOL x its diagonal, or an x' whose 1 - sum phi_j z^j or
+ *   1 + sum theta_j z^j fails the HR gate's step-down test, sets lambda <- 10 lambda and solves again (no pass);
+ *   accept: the next pass evaluates S(x'); S(x') < S(x) accepts x' (lambda <- lambda / 10, H and g of x'), otherwise
+ *   lambda <- 10 lambda with H and g kept;
+ *   stop (out_css_stop): 1 converged (an accepted pass lowered S by <= MMF_CSS_RTOL x S), 2 stalled (lambda >
+ *   MMF_CSS_LAMBDA_MAX), 3 budget (max_iter passes run; max_iter = 0: MMF_CSS_ITER_DEFAULT, at most MMF_CSS_ITER_MAX).
+ *   So S(shipped) <= S(x0) for every gated series.
+ * Outputs: a series that accepted no step keeps the HR call's pred, phi, theta, order, ma_order and status bit for bit;
+ * one that did gets the recursion and level integration of the HR call with the shipped (phi, theta).  For every gated
+ * series sigma = sqrt(S / |C|) at the shipped point (the conditional MLE).  Series that fail the HR gate and empty
+ * series get the HR call's outputs bit for bit.  out_css_start [n] (S(x0)), out_css [n] (S shipped), out_css_stop [n]
+ * and out_iters [n] (passes run) are nullable; NaN, NaN, 0, 0 for fallback and empty series.  beta is not re-estimated;
+ * this is not the exact (Kalman) likelihood.  Otherwise the contract of mmf_fit_forecast_arma_f32 (plans, device buffers
+ * only, any ld_out, enqueue-only unless `stats` is non-NULL, mmf_config.kernel and assume_finite honoured, refused
+ * arguments write nothing); max_iter outside [0, MMF_CSS_ITER_MAX] is MMF_E_INVALID.  Scratch: per slab, 52 B per row
+ * when out_phi, out_theta or out_ma_order is NULL.
+ * replaces: SARIMAX(p, d, q) + exog fit of the reference's per-group model (02:441-450, 472-481) by likelihood
+ * optimisation, with the conditional likelihood in place of the exact one. */
+int mmf_fit_forecast_arma_css_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
+                                  int32_t diff_order, int32_t ma_order, int32_t long_order, int32_t max_iter,
+                                  int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out, float* out_phi,
+                                  float* out_theta, int32_t* out_order, int32_t* out_ma_order, float* out_sigma,
+                                  int32_t* out_status, float* out_css_start, float* out_css, int32_t* out_css_stop,
+                                  int32_t* out_iters, mmf_stats* stats);
 
 /* ---- (p, d) selection by hold-out MSE on levels (DESIGN.md section 2 item 12) -----------------------------------------
  * mmf_fit_select_arima_f32: orders [n_orders] (1 .. MMF_ARSEL_MAX_CAND ascending distinct values in [0, MMF_AR_MAX]) and

@@ -44,7 +44,11 @@ __device__ bool css_step(const double* __restrict__ hg, const float* __restrict_
       if (!(dj > (double)MMF_HR_PIVOT_TOL * ajj)) { ok = false; break; }
       diag[j] = sqrt(dj);
       for (int i = j + 1; i < nreg; ++i) {
+#ifdef MMF_ARMACSS_DIAG_STEP
+        double v = 0.0;                    // control build: diag(H) only, the off-diagonal entries ignored
+#else
         double v = hg[ent(j, i)];
+#endif
         for (int k = 0; k < j; ++k) v -= W[i * NPAR + k] * W[j * NPAR + k];
         W[i * NPAR + j] = v / diag[j];
       }

@@ -12,6 +12,8 @@ For a gated series (``arma_oracle.hannan_rissanen`` passed its gate): x = (phi, 
              S by <= RTOL x S), 2 stalled (lam > LAMBDA_MAX), 3 budget (max_iter passes, the first at x0).
 Outputs as the library's: the HR row when no step was accepted, otherwise the recursion with the shipped x; sigma =
 sqrt(S / |C|) for every gated row.
+``lm_replay`` is ``lm`` vectorised over series, with the margin of every discrete decision in units of its float64
+noise; the exact-input GPU test replays the kernel with it pass by pass.
 """
 from __future__ import annotations
 
@@ -108,13 +110,13 @@ def _step(H, g, x, p: int, q: int, lam: float):
 
 def lm(e, obs, T: int, p: int, q: int, x0, max_iter: int = 0, gap_jacobian: bool = True):
     """LM of section 2 item 16 from the fp32 point x0 -> dict(x (fp32), S0, S, stop, iters, n_acc, path (S after every
-    pass), n_C)"""
+    pass), acc (whether every pass after the first accepted its point), n_C)"""
     max_iter = max_iter or ITER_DEFAULT
     x = np.asarray(x0, dtype=np.float32).copy()
     xt = x
     lam, S, S0, passes, n_acc, stop = LAMBDA0, 0.0, np.nan, 0, 0, 0
     H = g = None
-    path = []
+    path, acc = [], []
     n_C = 0
     while True:
         Sn, J, eps, C = css_eval(e, obs, T, p, q, xt, gap_jacobian)
@@ -126,6 +128,7 @@ def lm(e, obs, T: int, p: int, q: int, x0, max_iter: int = 0, gap_jacobian: bool
         else:
             take = Sn < S
             conv = take and S - Sn <= RTOL * S
+            acc.append(bool(take))
         if take:
             if passes > 1:
                 n_acc += 1
@@ -147,7 +150,7 @@ def lm(e, obs, T: int, p: int, q: int, x0, max_iter: int = 0, gap_jacobian: bool
             if xt is None:
                 stop = 2
         if stop:
-            return dict(x=x, S0=S0, S=S, stop=stop, iters=passes, n_acc=n_acc, path=path, n_C=n_C)
+            return dict(x=x, S0=S0, S=S, stop=stop, iters=passes, n_acc=n_acc, path=path, acc=acc, n_C=n_C)
 
 
 def css_bound(e, obs, T: int, p: int, q: int, x, tau):
@@ -173,6 +176,220 @@ def css_bound(e, obs, T: int, p: int, q: int, x, tau):
     C[:p] = False
     S = float(eps[C] @ eps[C])
     return 2.0 * float(np.sum(2.0 * np.abs(eps[C]) * be[C] + be[C] ** 2)) + 64 * 2.0 ** -52 * T * S
+
+
+U52 = 2.0 ** -52
+MARGINS = ("accept", "conv", "pivot", "kappa", "round")
+
+
+def s_noise(T: int, S):
+    """float64 noise of one evaluation of S over T rows: 64 T 2^-52 S (css_bound's rounding term)"""
+    return 64.0 * T * U52 * np.asarray(S, dtype=np.float64)
+
+
+def h_noise(T: int, k: int) -> float:
+    """float64 noise of an entry of H = J'J (of g = J' eps~) relative to sqrt(H_ii H_jj) (to sqrt(H_ii S)), sums in
+    another order and the derivative recursion included: 8 (k + sqrt(T)) 2^-52"""
+    return 8.0 * (k + np.sqrt(T)) * U52
+
+
+def rounding_margin(v, err):
+    """distance of each float64 v to the nearest fp32 rounding midpoint, in units of err (inf where err is 0)"""
+    v = np.asarray(v, dtype=np.float64)
+    f = v.astype(np.float32)
+    up = f.astype(np.float64) <= v
+    nb = np.where(up, np.nextafter(f, np.float32(np.inf)), np.nextafter(f, np.float32(-np.inf)))
+    dist = np.abs(v - 0.5 * (f.astype(np.float64) + nb.astype(np.float64)))
+    err = np.broadcast_to(np.asarray(err, dtype=np.float64), dist.shape)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return np.where(err > 0, dist / np.where(err > 0, err, 1.0), np.inf)
+
+
+def _step_down_batch(a):
+    """ar_oracle's step-down test of 1 - sum_j a_j z^j on every row of a [m, k] -> (ok [m], kappa margin [m]): the
+    distance of each |kappa| reached to KAPPA_MAX over 64 k 2^-52 / prod (1 - kappa^2) of the stages before it"""
+    a = np.array(a, dtype=np.float64)
+    m, k = a.shape
+    ok, mg, amp = np.ones(m, dtype=bool), np.full(m, np.inf), np.ones(m)
+    with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
+        for j in range(k, 0, -1):
+            kap = a[:, j - 1]
+            mg = np.where(ok, np.minimum(mg, np.abs(KAPPA_MAX - np.abs(kap)) / (64.0 * k * U52 * amp)), mg)
+            ok &= np.abs(kap) < KAPPA_MAX
+            den = np.where(ok, 1.0 - kap * kap, 1.0)
+            amp = amp / den
+            if j > 1:
+                a = (a[:, :j - 1] + kap[:, None] * a[:, j - 2::-1]) / den[:, None]
+    return ok, mg
+
+
+def _css_pass(E, OBS, T: int, p: int, q: int, X, gap_jacobian: bool = True):
+    """``css_eval`` on every row at once, with [H g; g' S] summed over the rows of C in row order (as the kernel does)
+    -> (S [n], g [n, k], H [n, k, k], |C| [n]); X [n, k] the points"""
+    n, k = X.shape[0], p + q
+    phi, th = X[:, :p], X[:, p:]
+    P0 = AR_MAX + 1                                  # history padding: the lag slices never reach index -1
+    U, EP = np.zeros((n, T + P0)), np.zeros((n, T + P0))
+    DU, DE = np.zeros((n, T + P0, k)), np.zeros((n, T + P0, k))
+    S, g, H, nC = np.zeros(n), np.zeros((n, k)), np.zeros((n, k, k)), np.zeros(n, dtype=np.int64)
+    for s in range(T):
+        i = P0 + s
+        ul, el = U[:, i - 1:i - 1 - p:-1], EP[:, i - 1:i - 1 - q:-1]
+        pr = np.einsum("nj,nj->n", phi, ul) + np.einsum("nj,nj->n", th, el)
+        dpr = np.concatenate([ul, el], axis=1)
+        if p:
+            dpr = dpr + np.einsum("nj,njk->nk", phi, DU[:, i - 1:i - 1 - p:-1])
+        if q:
+            dpr = dpr + np.einsum("nj,njk->nk", th, DE[:, i - 1:i - 1 - q:-1])
+        o, e = OBS[:, s], E[:, s]
+        U[:, i] = np.where(o, e, pr)
+        eps = np.where(o, e - pr, 0.0)
+        EP[:, i] = eps
+        if gap_jacobian:
+            DU[:, i] = np.where(o[:, None], 0.0, dpr)
+            DE[:, i] = np.where(o[:, None], -dpr, 0.0)
+        else:
+            DE[:, i] = -dpr
+        if s >= p and o.any():
+            J = DE[:, i] * o[:, None]
+            ec = eps * o
+            S += ec * ec
+            g += J * ec[:, None]
+            H += J[:, :, None] * J[:, None, :]
+            nC += o
+    return S, g, H, nC
+
+
+def _step_batch(H, g, S, x, p: int, q: int, lam, T: int):
+    """``_step`` on every row at once -> (trial points [m, k] fp32, lam [m], found [m], margins {pivot, kappa, round})
+
+    Margins (in units of the float64 noise of the quantity; below 1 the kernel's float64 may decide otherwise):
+      pivot  |d_j - PIVOT_TOL a_jj| over h_noise a_jj max(1, a_jj / |d_j|) (the Schur complement's sensitivity);
+      kappa  ``_step_down_batch``;
+      round  the distance of x + delta to the nearest fp32 midpoint over the first-order bound on delta's float64
+             error, h_noise (|A^-1| w + |delta|) componentwise, w_i = sqrt(a_ii) (sum_k sqrt(a_kk) |delta_k| + sqrt(S)):
+             delta' - delta = -A^-1 (dA delta + dg) with |dA_ij| <= h_noise sqrt(a_ii a_jj) (H's entries, Cauchy-Schwarz
+             on the row sums, a_ii >= H_ii) and |dg_i| <= h_noise sqrt(a_ii S), plus the rounding of x + delta itself.
+             It depends on the row's own system only, so a row is classified the same alone or in any batch."""
+    m, k = g.shape
+    hn = h_noise(T, k)
+    lam = np.array(lam, dtype=np.float64)
+    xt = np.zeros((m, k), dtype=np.float32)
+    found = np.zeros(m, dtype=bool)
+    mg = {key: np.full(m, np.inf) for key in ("pivot", "kappa", "round")}
+    eye = np.eye(k)
+    while True:
+        live = np.flatnonzero(~found & (lam <= LAMBDA_MAX))
+        if live.size == 0:
+            return xt, lam, found, mg
+        Hl = H[live]
+        dH = np.diagonal(Hl, axis1=1, axis2=2)
+        A = Hl + lam[live, None, None] * (eye * dH[:, None, :])
+        L = np.zeros_like(A)
+        ok = np.ones(live.size, dtype=bool)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            for j in range(k):
+                ajj = A[:, j, j]
+                dj = ajj - np.einsum("nk,nk->n", L[:, j, :j], L[:, j, :j])
+                noise = hn * ajj * np.maximum(1.0, ajj / np.abs(dj))
+                mp = np.abs(dj - PIVOT_TOL * ajj) / noise
+                mg["pivot"][live] = np.minimum(mg["pivot"][live], np.where(ok, mp, np.inf))
+                ok &= dj > PIVOT_TOL * ajj
+                Ljj = np.sqrt(np.where(ok, dj, 1.0))
+                L[:, j, j] = Ljj
+                L[:, j + 1:, j] = (A[:, j + 1:, j] - np.einsum("nik,nk->ni", L[:, j + 1:, :j], L[:, j, :j])) / Ljj[:, None]
+        good = np.zeros(live.size, dtype=bool)
+        if ok.any():
+            r = np.flatnonzero(ok)
+            Lr = L[r]
+            y = np.linalg.solve(Lr, -g[live[r]][:, :, None])
+            delta = np.linalg.solve(np.transpose(Lr, (0, 2, 1)), y)[:, :, 0]
+            v = x[live[r]].astype(np.float64) + delta
+            Ar = A[r]
+            Dd = np.sqrt(np.diagonal(Ar, axis1=1, axis2=2))
+            # first-order bound: |A^-1| (|dA| |delta| + |dg|), |dA_ij| <= hn sqrt(a_ii a_jj), |dg_i| <= hn sqrt(a_ii S)
+            w = Dd * ((Dd * np.abs(delta)).sum(axis=1) + np.sqrt(S[live[r]]))[:, None]
+            err = hn * (np.einsum("nij,nj->ni", np.abs(np.linalg.inv(Ar)), w) + np.abs(delta))
+            rm = rounding_margin(v, err).min(axis=1)
+            mg["round"][live[r]] = np.minimum(mg["round"][live[r]], rm)
+            cand = v.astype(np.float32)
+            ok_ar, m_ar = _step_down_batch(cand[:, :p].astype(np.float64))
+            ok_ma, m_ma = _step_down_batch(-cand[:, p:].astype(np.float64))
+            mg["kappa"][live[r]] = np.minimum(mg["kappa"][live[r]], np.minimum(m_ar, m_ma))
+            pass_ = ok_ar & ok_ma
+            good[r] = pass_
+            xt[live[r[pass_]]] = cand[pass_]
+        found[live[good]] = True
+        lam[live[~good]] *= 10.0
+
+
+def lm_replay(E, OBS, T: int, p: int, q: int, X0, max_iter: int = 0, gap_jacobian: bool = True, rtol: float = RTOL):
+    """``lm`` on every row of E [n, T] / OBS [n, T] from its fp32 point X0 [n, p + q], the rows in lockstep (a row that
+    has stopped is left out of later passes), with the smallest margin of every discrete decision on its path ->
+    dict(x [n, k] fp32, S0, S, stop, iters, n_acc, n_C [n], acc [n, max_iter] (acc[i, j]: pass j + 2 accepted),
+    margin {name: [n]}, ambiguous [n]).
+
+    A margin is the distance of a decision's quantity to its threshold in units of that quantity's float64 noise, the
+    difference between two float64 evaluations that sum in another order (the kernel's and this one):
+      accept  S_new < S: |S - S_new| / (s_noise(S) + s_noise(S_new)); infinite when the trial point is the accepted one
+              bit for bit (S_new is then S exactly on both sides);
+      conv    S - S_new <= rtol S: |S - S_new - rtol S| / (s_noise(S) + s_noise(S_new));
+      pivot, kappa, round  ``_step_batch``;
+      lam     lam > LAMBDA_MAX is decided on a float64 lam that both sides form by the same correctly rounded x 10 and
+              / 10 from LAMBDA0, so it has no noise; ``margin["lam"]`` is only the relative distance reached.
+    A row is ambiguous when one of accept, conv, pivot, kappa or round falls below 1 on its path."""
+    E = np.asarray(E, dtype=np.float64)
+    OBS = np.asarray(OBS, dtype=bool)
+    n, k = E.shape[0], p + q
+    max_iter = max_iter or ITER_DEFAULT
+    x = np.array(X0, dtype=np.float32).reshape(n, k)
+    xt = x.copy()
+    lam, S, S0 = np.full(n, LAMBDA0), np.zeros(n), np.full(n, np.nan)
+    H, g = np.zeros((n, k, k)), np.zeros((n, k))
+    passes, n_acc, stop, nC = (np.zeros(n, dtype=np.int64) for _ in range(4))
+    acc = np.zeros((n, max_iter), dtype=bool)
+    margin = {key: np.full(n, np.inf) for key in MARGINS + ("lam",)}
+    active = np.ones(n, dtype=bool)
+    while active.any():
+        idx = np.flatnonzero(active)
+        Sn, gn, Hn, nc = _css_pass(E[idx], OBS[idx], T, p, q, xt[idx].astype(np.float64), gap_jacobian)
+        nC[idx] = nc
+        passes[idx] += 1
+        first = passes[idx] == 1
+        Sp = S[idx]
+        same = (xt[idx].view(np.int32) == x[idx].view(np.int32)).all(axis=1)
+        take = first | (Sn < Sp)
+        conv = ~first & take & (Sp - Sn <= rtol * Sp)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            den = s_noise(T, Sp) + s_noise(T, Sn)
+            m_acc = np.where(~first & ~same, np.abs(Sp - Sn) / den, np.inf)
+            m_conv = np.where(~first & take, np.abs(Sp - Sn - rtol * Sp) / den, np.inf)
+        margin["accept"][idx] = np.minimum(margin["accept"][idx], m_acc)
+        margin["conv"][idx] = np.minimum(margin["conv"][idx], m_conv)
+        S0[idx[first]] = Sn[first]
+        a = idx[take & ~first]
+        n_acc[a] += 1
+        lam[a] /= 10.0
+        x[a] = xt[a]
+        acc[a, passes[a] - 2] = True
+        t = idx[take]
+        S[t], H[t], g[t] = Sn[take], Hn[take], gn[take]
+        lam[idx[~take]] *= 10.0
+        st = np.where(conv, 1, np.where(lam[idx] > LAMBDA_MAX, 2, np.where(passes[idx] >= max_iter, 3, 0)))
+        margin["lam"][idx] = np.minimum(margin["lam"][idx], np.abs(lam[idx] / LAMBDA_MAX - 1.0))
+        stop[idx] = st
+        need = idx[st == 0]
+        if need.size:
+            xs, lam[need], found, mg = _step_batch(H[need], g[need], S[need], x[need], p, q, lam[need], T)
+            for key, v in mg.items():
+                margin[key][need] = np.minimum(margin[key][need], v)
+            xt[need[found]] = xs[found]
+            stop[need[~found]] = 2
+        active[idx] = stop[idx] == 0
+    amb = np.zeros(n, dtype=bool)
+    for key in MARGINS:
+        amb |= margin[key] < 1.0
+    return dict(x=x, S0=S0, S=S, stop=stop, iters=passes, n_acc=n_acc, n_C=nC, acc=acc, margin=margin, ambiguous=amb)
 
 
 def fit_forecast_arma_css_packed(y, X, t_fit: int, pred_start: int, n_pred: int, p: int, q: int, d: int = 0,
@@ -243,4 +460,5 @@ def optimality_gap(e, obs, T: int, p: int, q: int, x):
 
 
 __all__ = ["LAMBDA0", "LAMBDA_MAX", "RTOL", "ITER_DEFAULT", "ITER_MAX", "FP32_EPS", "css_eval", "two_filter_jacobian",
-           "lm", "css_bound", "fit_forecast_arma_css_packed", "optimality_gap"]
+           "lm", "css_bound", "fit_forecast_arma_css_packed", "optimality_gap", "MARGINS", "s_noise", "h_noise",
+           "rounding_margin", "lm_replay"]

@@ -2,7 +2,7 @@
 finite differences (gap-free, isolated gaps, gaps longer than q, a gap before row p), the two-filter form before the first
 gap, a non-increasing objective along the LM path, optimality against SciPy, the theta RMSE against Hannan-Rissanen on
 simulated MA(1) rows, the negative control's failure on gappy rows, the header constants and the frame layer's
-estimator= argument."""
+estimator= argument; the vectorised replay against the scalar LM and its decision margins on constructed rows."""
 import os
 import re
 
@@ -118,6 +118,98 @@ def test_converged_rows_are_optimal():
         worst = max(worst, S.optimality_gap(e, obs, 240, p, q, r["x"]))
     assert n_conv >= 20
     assert worst <= OPT_RTOL, worst
+
+
+def _replay_rows(p, q, n, T, seed, gaps=0.0):
+    """n simulated ARMA(p, q) rows with random stationary, invertible parameters and their HR starts -> (E, OBS, X0) of
+    the rows whose HR estimate passed the gate"""
+    rng = np.random.default_rng(seed)
+    E, OBS, X0 = [], [], []
+    for i in range(n):
+        ph = _random_poly(rng, p)
+        th = -_random_poly(rng, q)
+        e, obs = _arma_series(T, ph, th, seed * 1000 + i, gaps=gaps)
+        x0, _ = _hr_start(e, obs, T, p, q)
+        if x0 is not None:
+            E.append(e), OBS.append(obs), X0.append(x0)
+    return np.array(E), np.array(OBS), np.array(X0, dtype=np.float32)
+
+
+def _random_poly(rng, k, rmax=0.85):
+    """a_1..a_k of 1 - sum a_j z^j from random reflection coefficients in (-rmax, rmax): stationary (invertible)"""
+    a = np.zeros(0)
+    for j in range(k):
+        kap = rng.uniform(-rmax, rmax)
+        a = np.r_[a - kap * a[::-1], kap]
+    return a
+
+
+REPLAY_CASES = [(1, 1, 0.0), (0, 2, 0.05), (2, 1, 0.02), (3, 4, 0.0), (4, 2, 0.1), (8, 4, 0.0)]
+
+
+def test_vectorised_replay_equals_the_scalar_lm():
+    """lm_replay, all rows of a case in lockstep, against lm row by row on every decided row: stop code, pass count,
+    acceptance sequence and x bit-equal, S within 1e-12; max_iter 64 so that every stop code can occur.  At least 30
+    rows are compared, and every case compares some"""
+    n_cmp = 0
+    for p, q, gaps in REPLAY_CASES:
+        E, OBS, X0 = _replay_rows(p, q, 12, 160, seed=31 + p * 5 + q, gaps=gaps)
+        assert len(E) >= 4, (p, q)
+        r = S.lm_replay(E, OBS, 160, p, q, X0, max_iter=64)
+        case = 0
+        for i in np.flatnonzero(~r["ambiguous"]):
+            w = S.lm(E[i], OBS[i], 160, p, q, X0[i], 64)
+            what = (p, q, int(i))
+            assert r["stop"][i] == w["stop"] and r["iters"][i] == w["iters"] and r["n_acc"][i] == w["n_acc"], what
+            assert list(r["acc"][i, :w["iters"] - 1]) == w["acc"], what
+            assert r["x"][i].tobytes() == np.asarray(w["x"], dtype=np.float32).tobytes(), what
+            assert abs(r["S"][i] - w["S"]) <= 1e-12 * w["S"] and abs(r["S0"][i] - w["S0"]) <= 1e-12 * w["S0"], what
+            assert r["n_C"][i] == (OBS[i, p:160]).sum(), what
+            case += 1
+        assert case >= 1, (p, q)
+        n_cmp += case
+    assert n_cmp >= 30, n_cmp
+
+
+def test_replay_classifies_a_row_the_same_alone_and_in_a_batch():
+    """margins depend on the row's own path only: every row replayed alone gets the batch's margins and outputs"""
+    E, OBS, X0 = _replay_rows(3, 4, 8, 160, seed=31 + 15 + 4)
+    r = S.lm_replay(E, OBS, 160, 3, 4, X0, max_iter=64)
+    for i in range(len(E)):
+        a = S.lm_replay(E[i:i + 1], OBS[i:i + 1], 160, 3, 4, X0[i:i + 1], max_iter=64)
+        assert a["ambiguous"][0] == r["ambiguous"][i] and a["x"][0].tobytes() == r["x"][i].tobytes(), i
+        for m in S.MARGINS:
+            assert a["margin"][m][0] == pytest.approx(r["margin"][m][i], rel=1e-9), (i, m)
+
+
+def test_replay_margins_on_constructed_rows():
+    """a convergence threshold placed exactly at a pass's realised gain makes the row ambiguous, and only through the
+    conv margin; a value exactly at an fp32 rounding midpoint has margin 0; a trial point equal to the accepted one
+    is never ambiguous"""
+    E, OBS, X0 = _replay_rows(1, 1, 6, 200, seed=5)
+    r = S.lm_replay(E, OBS, 200, 1, 1, X0, max_iter=64)
+    assert not r["ambiguous"].any()
+    i = int(np.flatnonzero(r["n_acc"] >= 2)[0])
+    w = S.lm(E[i], OBS[i], 200, 1, 1, X0[i], 64)
+    k = w["acc"].index(True) + 1                      # the first accepted pass after the first one
+    gain = (w["path"][k - 1] - w["path"][k]) / w["path"][k - 1]
+    at = S.lm_replay(E[i:i + 1], OBS[i:i + 1], 200, 1, 1, X0[i:i + 1], max_iter=64, rtol=gain)
+    assert at["ambiguous"][0] and at["margin"]["conv"][0] < 1.0
+    assert all(at["margin"][m][0] >= 1.0 for m in S.MARGINS if m != "conv")
+    # just above and below the threshold, by far more than the noise: decided, and the stop follows
+    hi = S.lm_replay(E[i:i + 1], OBS[i:i + 1], 200, 1, 1, X0[i:i + 1], max_iter=64, rtol=gain * (1 + 1e-6))
+    assert not hi["ambiguous"][0] and hi["stop"][0] == 1 and hi["iters"][0] == k + 1
+    f = np.float32(1.5)
+    mid = 0.5 * (float(f) + float(np.nextafter(f, np.float32(2))))
+    assert S.rounding_margin(np.array([mid]), 1e-20)[0] == 0.0
+    assert S.rounding_margin(np.array([mid + 1e-12]), 1e-12)[0] == pytest.approx(1.0, rel=1e-3)
+    assert S.rounding_margin(np.array([1.5]), 0.0)[0] == np.inf
+    # started at its own answer with no convergence rule, the row runs until lam passes LAMBDA_MAX or the budget ends;
+    # its trial points round back to x or lower S by less than the noise, and each such pass is marked: a trial point
+    # equal to x bit for bit is decided (S is then the same on both sides), any other is held to the accept margin
+    one = S.lm_replay(E[i:i + 1], OBS[i:i + 1], 200, 1, 1, r["x"][i:i + 1], max_iter=64, rtol=0.0)
+    assert one["stop"][0] in (2, 3)
+    assert bool(one["ambiguous"][0]) == any(one["margin"][m][0] < 1.0 for m in S.MARGINS)
 
 
 def _ma1_rows(n, T, seed, theta=0.8, gaps=0.0):

@@ -37,8 +37,9 @@ def _hr(eng, yd, p, q, d, ps, npred, m=0):
 
 
 def _check(got, hr, fb, y, X, t_fit, p, q, d, m, what, oracle=True, n_opt=4):
-    """the HR rows bit for bit, the refined rows against the oracle (``oracle``; SciPy's optimum on the first ``n_opt``
-    converged rows) -> (worst ratio, refined, budget-stopped)"""
+    """the HR rows bit for bit, the refined rows against the oracle (``oracle``: css_start and css within css_bound of
+    the oracle's S at the HR and the GPU's parameters; SciPy's optimum on the first ``n_opt`` converged and the first
+    ``n_opt`` stalled rows) -> (worst ratio, refined, budget-stopped)"""
     gated = hr["ma_order"] > 0
     refined = got["css_stop"] > 0
     assert np.array_equal(refined, gated), what
@@ -50,6 +51,10 @@ def _check(got, hr, fb, y, X, t_fit, p, q, d, m, what, oracle=True, n_opt=4):
     assert not got["iters"][~gated].any(), what
     assert (got["css"][gated] <= got["css_start"][gated]).all(), what
     assert (got["iters"][gated] >= 1).all() and (got["iters"][gated] <= S.ITER_DEFAULT).all(), what
+    # a budget stop after an accepted step has lowered S strictly
+    moved = gated & ((got["phi"] != hr["phi"]).any(1) | (got["theta"] != hr["theta"]).any(1))
+    b = moved & (got["css_stop"] == 3)
+    assert (got["css"][b] < got["css_start"][b]).all(), what
     if not oracle:
         return 0.0, int(gated.sum()), int((got["css_stop"] == 3).sum())
     # the oracle on the same rows, at the GPU's parameters
@@ -60,6 +65,7 @@ def _check(got, hr, fb, y, X, t_fit, p, q, d, m, what, oracle=True, n_opt=4):
     rows = np.flatnonzero(gated & want["gated"] & ~near & (got["status"] == 0))
     T = want["T"]
     worst = 0.0
+    n_left = {1: n_opt, 2: n_opt}                  # converged and stalled rows held to SciPy's optimum
     for i in rows:
         e, obs = want["e"][i], want["obs"][i]
         xg = np.r_[got["phi"][i, :p], got["theta"][i, :q]].astype(np.float64)
@@ -70,12 +76,14 @@ def _check(got, hr, fb, y, X, t_fit, p, q, d, m, what, oracle=True, n_opt=4):
         bh = S.css_bound(e, obs, T, p, q, xh, tau_fit[i])
         w = abs(Sg - float(got["css"][i])) / bg
         _le(w, 1.0, f"{what} row {i}: |S_oracle - css| / css_bound")
+        _le(abs(Sh - float(got["css_start"][i])) / bh, 1.0, f"{what} row {i}: |S_oracle(x0) - css_start| / css_bound")
         _le(Sg - Sh, bg + bh, f"{what} row {i}: S at the GPU's x above S at HR's")
         sig = np.sqrt(Sg / C.sum())
         _le(abs(float(got["sigma"][i]) - sig) / (np.sqrt(bg / C.sum()) + 4 * S.FP32_EPS * sig), 1.0,
             f"{what} row {i}: sigma")
-        if got["css_stop"][i] == 1 and n_opt > 0:
-            n_opt -= 1
+        stop = int(got["css_stop"][i])
+        if stop in (1, 2) and n_left[stop] > 0:
+            n_left[stop] -= 1
             gap = S.optimality_gap(e, obs, T, p, q, xg)
             _le(gap, OPT_RTOL + 2 * bg / Sg, f"{what} row {i}: optimality gap")
         worst = max(worst, w)

@@ -15,7 +15,9 @@ oracles by their own modules.
 1. Call kinds (KINDS below): one engine, plain, ARIMA (same X) and backtest plans planned once.  A ragged plan is
    planned when a ragged kind of the other mode (future / holdout) than the one in force comes up.  Every batch plants
    the row mix of test_gpu_abi_contract (gaps, leading gaps, mostly missing, empty rows), so records and pending counts
-   are never zero; the ARIMA batches carry MA(1) errors on every third row.
+   are never zero; the ARIMA batches carry MA(1) errors on every third row.  The CSS kinds (ARIMA(1, 1, 1), and
+   ARIMA(8, 2, 4) with m = 32 and max_iter = 64 with phi / theta / ma_order NULL) keep the HR estimate in the
+   context's per-slab scratch between the HR kernels and the LM kernel.
 2. Sequences on one stream: every ordered pair, the ping-pong triples, (capture, eager call, replay) with the eager call
    plain or ARIMA, and a seeded sequence of ~100 calls with two multi-slab calls (2^20 + 1,001 rows, one of them
    ARIMA(2, 1, 0)).
@@ -428,6 +430,37 @@ def _r_arma(eng, yd, stats, p, q, d, ps, npred, long_order=0, se=False, t_fit=T_
     return _done(rc, r, st)
 
 
+def _r_css(eng, yd, stats, p, q, d, ps, npred, long_order=0, max_iter=0):
+    """mmf_fit_forecast_arma_css_f32: the HR call, then LM from its (phi, theta), which the context keeps in per-slab
+    scratch for the outputs a caller passes as NULL (here none: every output is a sentinel-filled buffer)"""
+    n = yd.shape[0]
+    r = _model_outs(n, npred, True)
+    r.update(css_start=_f1(n), css=_f1(n), css_stop=_i(n), iters=_i(n))
+    st = N.MmfStats() if stats else None
+    _stream(eng)
+    rc = eng._lib.mmf_fit_forecast_arma_css_f32(
+        eng._h, yd.data_ptr(), n, yd.stride(0), p, d, q, long_order, max_iter, ps, npred, _p(r["pred"]),
+        r["pred"].stride(0), *[_p(r[k]) for k in ("phi", "theta", "order", "ma_order", "sigma", "status", "css_start",
+                                                  "css", "css_stop", "iters")], _stats(st))
+    return _done(rc, r, st)
+
+
+def _r_css_scratch(eng, yd, stats, p, q, d, ps, npred, long_order=0, max_iter=0):
+    """the same call with phi, theta and ma_order NULL: the HR estimate and the gate then live in the context's
+    scratch (52 B per row per slab) between the HR kernels and arma_css_kernel"""
+    n = yd.shape[0]
+    r = {"pred": _f(n, npred), "order": _i(n), "sigma": _f1(n), "status": _i(n), "css_start": _f1(n), "css": _f1(n),
+         "css_stop": _i(n), "iters": _i(n)}
+    st = N.MmfStats() if stats else None
+    _stream(eng)
+    rc = eng._lib.mmf_fit_forecast_arma_css_f32(
+        eng._h, yd.data_ptr(), n, yd.stride(0), p, d, q, long_order, max_iter, ps, npred, _p(r["pred"]),
+        r["pred"].stride(0), None, None, _p(r["order"]), None, *[_p(r[k]) for k in ("sigma", "status", "css_start",
+                                                                                    "css", "css_stop", "iters")],
+        _stats(st))
+    return _done(rc, r, st)
+
+
 def _r_select(eng, yd, stats, grid, ps, npred, se=False, t_fit=T_FIT):
     """mmf_fit_select_arma_f32 on grid = (orders, diffs, mas); mas = None: mmf_fit_select_arima_f32"""
     orders, diffs, mas = grid
@@ -476,6 +509,8 @@ ARIMA_RAW = {
     "select_arma_max": lambda e, inp, s: _r_select(e, inp["yd"], s, GRID_MAX, T_FIT, H),
     "arima_se": lambda e, inp, s: _r_arima_se(e, inp),
     "refused_arima": lambda e, inp, s: _r_select(e, inp["yd"], s, ((1,), (0, 1), (1, 2)), T_FIT, H),
+    "css111": lambda e, inp, s: _r_css(e, inp["yd"], s, 1, 1, 1, T_FIT, H),
+    "css824": lambda e, inp, s: _r_css_scratch(e, inp["yd"], s, 8, 4, 2, T_FIT, H, long_order=32, max_iter=64),
     "big_arima": lambda e, inp, s: _r_arima(e, inp["yd"], s, 2, 1, T_FIT, H),
     "aba_arima": lambda e, inp, s: _r_arima(e, inp["yd"], s, 2, 1, T_FIT, H),
 }
@@ -527,7 +562,8 @@ KIND_ROWS = {
     "replay": (450, 24), "refused": (256, 25),
     "ar_select": (437, 41), "arima21": (1003, 42), "arima12_mid": (389, 43), "select_arima": (517, 44),
     "arma111_se": (629, 45), "arma824": (333, 46), "select_arma_ref": (301, 47), "select_arma_52k": (285, 48),
-    "select_arma_max": (259, 49), "arima_se": (707, 50), "refused_arima": (131, 51),
+    "select_arma_max": (259, 49), "arima_se": (707, 50), "refused_arima": (131, 51), "css111": (587, 53),
+    "css824": (313, 54),
     "future_b": (1000, 26), "big": (BIG, 27), "big_arima": (BIG, 52),
     "aba_1": (40000, 31), "aba_2": (40000, 32), "aba_3": (40000, 33), "aba_arima": (40003, 34),
 }
@@ -541,16 +577,16 @@ RUN = {
     "aba_1": _k_plain(T_FIT, H), "aba_2": _k_plain(T_FIT, H), "aba_3": _k_plain(T_FIT, H),
     **{name: _k_arima(name) for name in ARIMA_RAW},
 }
-ARIMA_KINDS = tuple(KIND_ROWS)[15:26]
-KINDS = tuple(KIND_ROWS)[:26]                             # the kinds every sequence draws from
+ARIMA_KINDS = tuple(KIND_ROWS)[15:28]
+KINDS = tuple(KIND_ROWS)[:28]                             # the kinds every sequence draws from
 HAS_STATS = ("future", "holdout", "warp", "se_future", "se_holdout", "ar2", "ragged_future", "ragged_holdout",
              "backtest", "host", "int16", "future_b", "big", "ar_select", "arima21", "arima12_mid", "select_arima",
-             "arma111_se", "arma824", "select_arma_ref", "select_arma_52k", "select_arma_max", "big_arima",
-             "aba_arima")
+             "arma111_se", "arma824", "select_arma_ref", "select_arma_52k", "select_arma_max", "css111", "css824",
+             "big_arima", "aba_arima")
 SEL_GRIDS = {"ar_select": (AR_ORDERS, (0,), (0,), (0, N_ROWS)), "select_arima": (*REF[:2], (0,), (T_FIT, H)),
              "select_arma_ref": (*REF, (0, N_ROWS)), "select_arma_52k": (*GRID_52K, MID),
              "select_arma_max": (*GRID_MAX, (T_FIT, H))}
-FLOAT_KEYS = ("pred", "mse", "cand_mse", "phi", "theta", "sigma", "se")
+FLOAT_KEYS = ("pred", "mse", "cand_mse", "phi", "theta", "sigma", "se", "css_start", "css")
 
 
 def _call(ctx, name, stats=False):
@@ -693,7 +729,7 @@ def test_every_ordered_pair_of_call_kinds():
 
 
 @pytest.mark.parametrize("middle", ["warp", "ragged_future", "backtest", "refused", "select_arma_max", "arima21",
-                                    "arima_se"])
+                                    "arima_se", "css824"])
 def test_ping_pong_triples(middle):
     """(TC, X, TC): a call that uses the counter sets differently -- the warp kernel (does not zero the next set), a
     ragged or backtest call (memsets its set, toggles nothing), a refused call (enqueues nothing), the fit_tc hand-off
@@ -786,8 +822,8 @@ def test_seeded_sequence_on_one_stream():
 # ARIMA(2, 1, 0) and the (p, d, q) selection on the reference grid, and the standard-error pass behind ARIMA(1, 1, 1)
 TILE_CASES = ([(inst, t) for inst in ("tc", "variant2", "se") for t in (32, 33, 1095)]
               + [("ragged", t) for t in (33, 65, 1095)] + [("backtest", t) for t in (33, 36, 1095)]
-              + [(inst, t) for inst in ("arima21", "select_arma") for t in (65, 1095)] + [("arima_se", T_FIT)])
-ARIMA_INSTS = ("arima21", "select_arma", "arima_se")
+              + [(inst, t) for inst in ("arima21", "select_arma", "css") for t in (65, 1095)] + [("arima_se", T_FIT)])
+ARIMA_INSTS = ("arima21", "select_arma", "arima_se", "css")
 
 
 def _sizes(grid, inst=None):
@@ -852,7 +888,8 @@ def _run_inst(inst, eng, yd, t_fit, bounds):
     if inst in ARIMA_INSTS:
         rc, r = {"arima21": lambda: _r_arima(eng, yd, True, 2, 1, t_fit, H),
                  "select_arma": lambda: _r_select(eng, yd, True, REF, t_fit, H),
-                 "arima_se": lambda: _r_arma(eng, yd, True, 1, 1, 1, t_fit, H, se=True, t_fit=t_fit)}[inst]()
+                 "arima_se": lambda: _r_arma(eng, yd, True, 1, 1, 1, t_fit, H, se=True, t_fit=t_fit),
+                 "css": lambda: _r_css(eng, yd, True, 1, 1, 1, t_fit, H)}[inst]()
         N.check(rc)
         return r, r.pop("n_pending")
     out, status = _f(n, H), _i(n)

@@ -9,6 +9,8 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
+#include <optional>
 #include <string>
 #include <vector>
 
@@ -297,6 +299,25 @@ DesignView view_of(const Plan& p) {
   return d;
 }
 
+// the stacked designs of a ragged plan (or of a backtest plan's origins), as the kernels that take every calendar see them
+DesignView view_of(const MultiPlan& m) {
+  DesignView d{};
+  d.a4 = m.d_a4; d.at = m.d_at; d.apred = m.d_apred; d.w = m.d_w;
+  d.n_rows = m.cals[0].n_rows; d.n_rows_pad = m.cals[0].n_rows_pad;
+  d.t_fit = m.t_fit_max; d.t_pad = m.t_pad_max; d.kept_mask = 0xFFFFu; d.has_constant = m.has_constant;
+  return d;
+}
+
+// calendar c of a ragged plan on its own (the general pass of its rows)
+DesignView view_of(const MultiPlan& m, int c) {
+  const CalMeta& cm = m.cals[c];
+  DesignView d = view_of(m);
+  d.a4 = m.d_a4 + m.a4_off[c]; d.apred = m.d_apred + (size_t)cm.row_off * P;
+  d.n_rows = cm.n_rows; d.n_rows_pad = cm.n_rows_pad; d.t_fit = cm.t_fit; d.t_pad = (cm.t_fit + 31) & ~31;
+  d.kept_mask = cm.kept_mask;
+  return d;
+}
+
 
 // float64 calendar Gram over the fit rows, in-order Cholesky with aliasing, W = L^-T on the kept columns
 // (oracle/mmf_oracle.py: whiten), A = X W in float32.  Shared by the single-calendar and the ragged plan.
@@ -517,52 +538,119 @@ int build_multi(MultiPlan& m, const double* X_all, int32_t n_cal, const int32_t*
   return MMF_OK;
 }
 
-// Enqueue the fit of ONE slab of device-resident rows on `s`.  status must be non-null.
-// ARIMA calls (arima != nullptr, with ar): y / ld_y are the slab's levels; diff_kernel writes z' into the context's
-// scratch first, and the fit passes and arima_kernel read z' with `plan` = the plan of D_d.  (p, d) selection calls
-// (asel != nullptr) run this once per listed d and end in arima_select_kernel; their d = 0 pass (arima->d == 0) fits y
-// itself with the mmf_plan_design plan; (p, d, q) selection calls (hsel != nullptr, with asel) add arma_select_kernel
-// behind it.  ARMA calls (arma != nullptr, with ar) run arma_kernel behind ar_kernel (d = 0, arima == nullptr) or
-// arima_kernel; CSS calls (css != nullptr, with arma) add arma_css_kernel behind arma_kernel.
-int run_device_slab(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, int64_t ld_y, int32_t pred_start,
-                    int32_t n_pred, float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s,
-                    int* launches, int* kernel_used, float* const* out_more, int n_out, int multimem,
-                    const SelectArgs* sel, const SeArgs* se = nullptr, const ArArgs* ar = nullptr,
-                    const ArSelArgs* arsel = nullptr, const ArimaArgs* arima = nullptr,
-                    const ArimaSelArgs* asel = nullptr, const ArmaArgs* arma = nullptr,
-                    const ArmaSelArgs* hsel = nullptr, const CssArgs* css = nullptr) {
+// Launch and kernel-choice bookkeeping of one call (mmf_stats.kernel_launches / kernel_used)
+struct Tally {
+  int launches = 0;
+  int kernel_used = 0;
+};
+
+// One call of the device path: the plain fit and the model stages behind it, each present or not.  ARIMA calls (arima,
+// with ar): y / ld_y are the levels; diff_kernel writes z' into the context's scratch first, and the fit passes and
+// arima_kernel read z' with the plan of D_d.  (p, d) selections (asel) run one call per listed d and end in
+// arima_select_kernel; their d = 0 call (arima->d == 0) fits y itself with the mmf_plan_design plan; (p, d, q) selections
+// (hsel, with asel) add arma_select_kernel behind it.  ARMA calls (arma, with ar) run arma_kernel behind ar_kernel
+// (d = 0, no arima) or arima_kernel; CSS calls (css, with arma) add arma_css_kernel behind arma_kernel.
+struct Call {
+  const float* y = nullptr;
+  int64_t ld_y = 0;
+  int32_t pred_start = 0, n_pred = 0;
+  float* out = nullptr;
+  int64_t ld_out = 0;
+  float* beta = nullptr;
+  int32_t* status = nullptr;
+  float* out_more[MAX_OUT - 1] = {};
+  int n_out = 1, multimem = 0;
+  std::optional<SelectArgs> sel;
+  std::optional<SeArgs> se;
+  std::optional<ArArgs> ar;
+  std::optional<ArSelArgs> arsel;
+  std::optional<ArimaArgs> arima;
+  std::optional<ArimaSelArgs> asel;
+  std::optional<ArmaArgs> arma;
+  std::optional<ArmaSelArgs> hsel;
+  std::optional<CssArgs> css;
+
+  // the same call on the rows from `off` on: every per-row output advanced by `off` rows (null stays null)
+  Call slice(int64_t off) const {
+    auto at = [off](auto* p, int64_t width) { return p ? p + off * width : p; };
+    Call c = *this;
+    c.y = y + off * ld_y;
+    c.out = out + off * ld_out;
+    c.beta = at(beta, P);
+    if (!asel) c.status = status + off;     // a selection's fits write the per-slab scratch; asel->status is the caller's
+    for (int i = 0; i + 1 < n_out && i < MAX_OUT - 1; ++i) c.out_more[i] = out_more[i] + off * ld_out;
+    if (sel) { c.sel->out_choice = at(sel->out_choice, 1); c.sel->out_mse = at(sel->out_mse, 1); }
+    if (se) { c.se->out_se = at(se->out_se, se->ld_se); c.se->sigma = at(se->sigma, 1); c.se->dof = at(se->dof, 1); }
+    if (ar) { c.ar->phi = at(ar->phi, MMF_AR_MAX); c.ar->order = at(ar->order, 1); c.ar->sigma = at(ar->sigma, 1); }
+    if (arsel) {
+      c.arsel->choice = at(arsel->choice, 1);
+      c.arsel->mse = at(arsel->mse, 1);
+      c.arsel->cand_mse = at(arsel->cand_mse, arsel->n_cand);
+    }
+    if (asel) {
+      c.asel->choice_p = at(asel->choice_p, 1);
+      c.asel->choice_d = at(asel->choice_d, 1);
+      c.asel->mse = at(asel->mse, 1);
+      c.asel->status = at(asel->status, 1);
+      // (p, d, q) selections: arima_select_kernel's scores go to scratch, arma_select_kernel copies them into the q = 0
+      // slice of hsel->cand_mse
+      if (!hsel) c.asel->cand_mse = at(asel->cand_mse, (int64_t)asel->n_diffs * asel->n_cand);
+    }
+    if (arma) { c.arma->theta = at(arma->theta, MMF_MA_MAX); c.arma->ma_order = at(arma->ma_order, 1); }
+    if (hsel) {
+      c.hsel->choice_q = at(hsel->choice_q, 1);
+      c.hsel->theta = at(hsel->theta, MMF_MA_MAX);
+      c.hsel->ma_order = at(hsel->ma_order, 1);
+      c.hsel->cand_mse = at(hsel->cand_mse, (int64_t)asel->n_diffs * hsel->n_mas * asel->n_cand);
+    }
+    if (css) {
+      c.css->css_start = at(css->css_start, 1);
+      c.css->css = at(css->css, 1);
+      c.css->css_stop = at(css->css_stop, 1);
+      c.css->iters = at(css->iters, 1);
+    }
+    return c;
+  }
+};
+
+// Enqueue the fit of ONE slab of n device-resident rows on the context's stream, against `plan` (ctx->plan, or the
+// differenced plan of an ARIMA call).  c.status must be non-null.
+int run_device_slab(mmf_ctx* ctx, const Plan& plan, const Call& c, int64_t n, Tally& t) {
+  const cudaStream_t s = ctx->stream;
   const DesignView d = view_of(plan);
+  const float* y = c.y;
+  int64_t ld_y = c.ld_y;
   ArimaArgs ma{};
-  if (arima != nullptr) {
-    ma = *arima;
+  if (c.arima) {
+    ma = *c.arima;
     ma.y = y;
   }
-  if (arima != nullptr && ma.d > 0) {
+  if (c.arima && ma.d > 0) {
     const int64_t ld_z = (plan.t_fit + 3) & ~3;              // 16-B row pitch: fit_tc's TMA path
     int rc = grow((void**)&ctx->d_z, &ctx->z_cap_bytes, (size_t)n * ld_z * sizeof(float));
     if (rc != MMF_OK) return rc;
     CU_TRY(launch_diff(ma, ctx->d_z, ld_z, n, ctx->sm_count, s));
-    ++*launches;
+    ++t.launches;
     y = ctx->d_z;
     ld_y = ld_z;
   }
   FitArgs a{};
-  a.y = y; a.n = n; a.ld_y = ld_y; a.pred_start = pred_start; a.n_pred = n_pred;
-  a.out = out; a.ld_out = ld_out; a.out_beta = beta; a.status = status;
-  a.n_out = n_out; a.out_multimem = multimem;
-  for (int i = 0; i + 1 < n_out && i < MAX_OUT - 1; ++i) a.out_more[i] = out_more[i];
+  a.y = y; a.n = n; a.ld_y = ld_y; a.pred_start = c.pred_start; a.n_pred = c.n_pred;
+  a.out = c.out; a.ld_out = c.ld_out; a.out_beta = c.beta; a.status = c.status;
+  a.n_out = c.n_out; a.out_multimem = c.multimem;
+  for (int i = 0; i + 1 < c.n_out && i < MAX_OUT - 1; ++i) a.out_more[i] = c.out_more[i];
   a.only_pending = 0; a.pending_count = nullptr;
   const char* why = nullptr;
   int kernel = ctx->cfg.kernel;
   // Many prediction rows (the reference's "Demand_Fitted for every date", 02:484-494): fit kernels hand
   // gamma/c to predict_tc_kernel, which writes the [n, n_pred] table with TMA stores.
-  const bool predict_ok = n_out == 1 && !multimem && ld_out % 4 == 0 && (reinterpret_cast<uintptr_t>(out) & 15u) == 0 &&
-                          n <= (int64_t)0x7fffffff - 128;
-  if (sel != nullptr && !predict_ok)
+  const bool predict_ok = c.n_out == 1 && !c.multimem && c.ld_out % 4 == 0 &&
+                          (reinterpret_cast<uintptr_t>(c.out) & 15u) == 0 && n <= (int64_t)0x7fffffff - 128;
+  if (c.sel && !predict_ok)
     return fail(MMF_E_UNSUPPORTED, "model selection needs a 16-B aligned output with ld_out %% 4 == 0");
-  // AR calls (ar != nullptr) hand gamma / c to ar_kernel, which writes the table itself: no predict_tc requirement
-  const bool many_pred = ar == nullptr && (sel != nullptr || (n_pred > 64 && kernel != MMF_KERNEL_WARP && predict_ok));
-  if (many_pred || ar != nullptr) {
+  // AR calls (ar) hand gamma / c to ar_kernel, which writes the table itself: no predict_tc requirement
+  const bool many_pred = !c.ar && (c.sel || (c.n_pred > 64 && kernel != MMF_KERNEL_WARP && predict_ok));
+  if (many_pred || c.ar) {
     int rc = grow((void**)&ctx->d_gamma, &ctx->gamma_cap_bytes, (size_t)n * P * sizeof(float));
     if (rc == MMF_OK) rc = grow((void**)&ctx->d_c, &ctx->c_cap_bytes, (size_t)n * sizeof(float));
     if (rc != MMF_OK) return rc;
@@ -599,6 +687,7 @@ int run_device_slab(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, i
   if (capturing || !ctx->set_clean[cs]) CU_TRY(cudaMemsetAsync(counters, 0, CTR_WORDS * sizeof(uint32_t), s));
   if (!capturing) ctx->set_clean[cs] = false;             // dirty from here on, whatever happens below
   if (kernel == MMF_KERNEL_TC && !capturing) a.zero_next = ctx->d_pending + CTR_WORDS * (cs ^ 1);
+  const SeArgs* se = c.se ? &*c.se : nullptr;
   if (kernel == MMF_KERNEL_TC) {
     TcLaunch tl;
     int rc = encode_2d(tl.tmap_y, y, (uint64_t)d.t_fit, (uint64_t)n, (uint64_t)ld_y * 4, 32, 128);
@@ -606,14 +695,14 @@ int run_device_slab(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, i
     memcpy(tl.tmap_at, plan.tmap_at, 128);
     if (se != nullptr) {
       CU_TRY(launch_fit_tc_se(d, a, tl, counters, ctx->sm_count, s, *se));
-      ++*launches;
+      ++t.launches;
       if (many_pred) {          // se rows of the rows fit_tc finished, before the passes behind it change any status
         CU_TRY(launch_se_outer(a, *se, ctx->sm_count, s));
-        ++*launches;
+        ++t.launches;
       }
     } else {
       CU_TRY(launch_fit_tc(d, a, tl, counters, ctx->sm_count, s, ctx->cfg.tc_variant));
-      ++*launches;
+      ++t.launches;
     }
     if (may_mask) {
       FitArgs m = a;
@@ -621,37 +710,37 @@ int run_device_slab(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, i
       m.pending_count = counters;
       CU_TRY(launch_fit_warp(d, m, ctx->sm_count, s, se));
       CU_TRY(launch_solve_rows(d, m, ctx->sm_count, s, nullptr, se));   // the records both passes queued
-      *launches += 2;
+      t.launches += 2;
     }
   } else {
     CU_TRY(launch_fit_warp(d, a, ctx->sm_count, s, se));
-    ++*launches;
+    ++t.launches;
     if (may_mask) {
       CU_TRY(launch_solve_rows(d, a, ctx->sm_count, s, nullptr, se));
-      ++*launches;
+      ++t.launches;
     }
   }
-  if (sel != nullptr) {
-    CU_TRY(launch_select(d, a, *sel, ctx->sm_count, s));
-    ++*launches;
+  if (c.sel) {
+    CU_TRY(launch_select(d, a, *c.sel, ctx->sm_count, s));
+    ++t.launches;
   }
-  if (ar != nullptr) {
-    CU_TRY(asel != nullptr    ? launch_arima_select(d, a, *ar, ma, *asel, s)
-           : arima != nullptr ? launch_arima(d, a, *ar, ma, s)
-           : arsel != nullptr ? launch_ar_select(d, a, *ar, *arsel, s) : launch_ar(d, a, *ar, s));
-    ++*launches;
-    if (hsel != nullptr) {
-      CU_TRY(launch_arma_select(d, a, *ar, ma, *asel, *hsel, s));
-      ++*launches;
+  if (c.ar) {
+    CU_TRY(c.asel    ? launch_arima_select(d, a, *c.ar, ma, *c.asel, s)
+           : c.arima ? launch_arima(d, a, *c.ar, ma, s)
+           : c.arsel ? launch_ar_select(d, a, *c.ar, *c.arsel, s) : launch_ar(d, a, *c.ar, s));
+    ++t.launches;
+    if (c.hsel) {
+      CU_TRY(launch_arma_select(d, a, *c.ar, ma, *c.asel, *c.hsel, s));
+      ++t.launches;
     }
-    if (arma != nullptr) {
+    if (c.arma) {
       ArimaArgs mh = ma;
-      if (arima == nullptr) { mh.y = a.y; mh.ld_y = a.ld_y; mh.t_fit = d.t_fit; mh.d = 0; }
-      CU_TRY(launch_arma(d, a, *ar, mh, *arma, s));
-      ++*launches;
-      if (css != nullptr) {
-        CU_TRY(launch_arma_css(d, a, *ar, mh, *arma, *css, s));
-        ++*launches;
+      if (!c.arima) { mh.y = a.y; mh.ld_y = a.ld_y; mh.t_fit = d.t_fit; mh.d = 0; }
+      CU_TRY(launch_arma(d, a, *c.ar, mh, *c.arma, s));
+      ++t.launches;
+      if (c.css) {
+        CU_TRY(launch_arma_css(d, a, *c.ar, mh, *c.arma, *c.css, s));
+        ++t.launches;
       }
     }
   }
@@ -661,14 +750,14 @@ int run_device_slab(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, i
     memcpy(pl.tmap_blo, plan.tmap_blo, 128);
     // the map stops at the last whole 16 B of a row (TMA clips with 16-B granularity); the kernel stores the
     // n_pred % 4 columns behind it itself, so the caller's columns from n_pred on are never written
-    pl.n_tma = n_pred & ~3;
-    int rc = encode_2d(pl.tmap_out, out, (uint64_t)(pl.n_tma > 0 ? pl.n_tma : n_pred), (uint64_t)n, (uint64_t)ld_out * 4,
-                       32, 64);   // one box per warpgroup half
+    pl.n_tma = c.n_pred & ~3;
+    int rc = encode_2d(pl.tmap_out, c.out, (uint64_t)(pl.n_tma > 0 ? pl.n_tma : c.n_pred), (uint64_t)n,
+                       (uint64_t)c.ld_out * 4, 32, 64);   // one box per warpgroup half
     if (rc != MMF_OK) return rc;
     CU_TRY(launch_predict_tc(d, a, pl, ctx->sm_count, s));
-    ++*launches;
+    ++t.launches;
   }
-  *kernel_used = kernel;
+  t.kernel_used = kernel;
   ctx->last_set = cs;
   if (!capturing) {                                       // toggle only once every launch of the call is enqueued
     ctx->set_clean[cs ^ 1] = (kernel == MMF_KERNEL_TC);   // zeroed by this call's tensor-core kernel
@@ -677,7 +766,7 @@ int run_device_slab(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, i
   return MMF_OK;
 }
 
-// Enqueue the fit for device-resident buffers on `s`: slab by slab, so that the per-row scratch (a 256-B record and a
+// Enqueue the fit for device-resident buffers: slab by slab, so that the per-row scratch (a 256-B record and a
 // work-list entry per row for the series with gaps, gamma / c for the many-rows predict kernel) is proportional to a
 // slab, not to the batch.  One slab for batches up to a million rows; beyond that the slab is sized so the scratch
 // stays under ~5 % of the input (10 M x 365: 4 slabs, 0.7 GB instead of 2.6 GB).  Slabs run back to back on the
@@ -694,103 +783,182 @@ int64_t slab_rows(const Plan& plan, int64_t n) {
   return slab;
 }
 
-// slab_pending (nullable, one word per slab): each slab's count of rows handed to the general pass is copied there
-// before the next slab's tensor-core kernel zeroes the counter set it was kept in (0 for a slab fit by the warp kernel).
-// `plan`: the design every slab is fit against (ctx->plan, or the differenced plan of an ARIMA call)
-int run_device(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, int64_t ld_y, int32_t pred_start,
-               int32_t n_pred, float* out, int64_t ld_out, float* beta, int32_t* status, cudaStream_t s,
-               int* launches, int* kernel_used, float* const* out_more = nullptr, int n_out = 1, int multimem = 0,
-               const SelectArgs* sel = nullptr, uint32_t* slab_pending = nullptr, const SeArgs* se = nullptr,
-               const ArArgs* ar = nullptr, const ArSelArgs* arsel = nullptr, const ArimaArgs* arima = nullptr,
-               const ArmaArgs* arma = nullptr, const CssArgs* css = nullptr) {
-  const int64_t slab = slab_rows(plan, n);
+// One fit a call runs in every slab, against `plan`.  Single-model calls have one stage; the (p, d) and (p, d, q)
+// selections one per listed d.
+struct Stage {
+  const Plan* plan;
+  Call call;
+};
+
+// The slabs are cut by `slab_plan` (the plan of the call's one stage, or a selection's level plan: the plain fit of the
+// level rows would cut them so), and every slab runs each stage in turn.  slab_pending (nullable, one word per slab
+// and stage): each fit's count of rows handed to the general pass is copied there before the next fit's tensor-core
+// kernel zeroes the counter set it was kept in (0 for a fit by the warp kernel).
+int run_device(mmf_ctx* ctx, const Plan& slab_plan, const std::vector<Stage>& stages, int64_t n, Tally& t,
+               uint32_t* slab_pending = nullptr) {
+  const cudaStream_t s = ctx->stream;
+  const int64_t slab = slab_rows(slab_plan, n);
   // CSS calls read the HR (phi, theta, ma_order) back: what the caller did not ask for goes to per-slab scratch
-  float* hr_phi = nullptr;
-  float* hr_theta = nullptr;
-  int32_t* hr_ma = nullptr;
-  if (css != nullptr && (ar->phi == nullptr || arma->theta == nullptr || arma->ma_order == nullptr)) {
+  const Call& c0 = stages[0].call;
+  float* hr = nullptr;
+  if (c0.css && (c0.ar->phi == nullptr || c0.arma->theta == nullptr || c0.arma->ma_order == nullptr)) {
     const size_t per_row = (MMF_AR_MAX + MMF_MA_MAX + 1) * sizeof(float);
     int rc = grow((void**)&ctx->d_css_hr, &ctx->css_hr_cap, (size_t)slab * per_row);
     if (rc != MMF_OK) return rc;
-    hr_phi = ctx->d_css_hr;
-    hr_theta = hr_phi + (size_t)slab * MMF_AR_MAX;
-    hr_ma = reinterpret_cast<int32_t*>(hr_theta + (size_t)slab * MMF_MA_MAX);
+    hr = ctx->d_css_hr;
   }
   for (int64_t off = 0, i = 0; off < n; off += slab, ++i) {
     const int64_t m = std::min(slab, n - off);
-    float* more[MAX_OUT - 1] = {};
-    for (int i = 0; i + 1 < n_out && i < MAX_OUT - 1; ++i) more[i] = out_more[i] + off * ld_out;
-    SelectArgs sel_slab;
-    if (sel != nullptr) {
-      sel_slab = *sel;
-      if (sel_slab.out_choice) sel_slab.out_choice += off;
-      if (sel_slab.out_mse) sel_slab.out_mse += off;
-    }
-    SeArgs se_slab{};
-    if (se != nullptr) {
-      se_slab = *se;
-      if (se_slab.out_se) se_slab.out_se += off * se_slab.ld_se;
-      se_slab.sigma += off;
-      if (se_slab.dof) se_slab.dof += off;
-    }
-    ArArgs ar_slab{};
-    if (ar != nullptr) {
-      ar_slab = *ar;
-      if (ar_slab.phi) ar_slab.phi += off * MMF_AR_MAX;
-      else if (css != nullptr) ar_slab.phi = hr_phi;
-      if (ar_slab.order) ar_slab.order += off;
-      if (ar_slab.sigma) ar_slab.sigma += off;
-    }
-    ArSelArgs arsel_slab{};
-    if (arsel != nullptr) {
-      arsel_slab = *arsel;
-      if (arsel_slab.choice) arsel_slab.choice += off;
-      if (arsel_slab.mse) arsel_slab.mse += off;
-      if (arsel_slab.cand_mse) arsel_slab.cand_mse += off * arsel_slab.n_cand;
-    }
-    ArmaArgs arma_slab{};
-    if (arma != nullptr) {
-      arma_slab = *arma;
-      if (arma_slab.theta) arma_slab.theta += off * MMF_MA_MAX;
-      else if (css != nullptr) arma_slab.theta = hr_theta;
-      if (arma_slab.ma_order) arma_slab.ma_order += off;
-      else if (css != nullptr) arma_slab.ma_order = hr_ma;
-    }
-    CssArgs css_slab{};
-    if (css != nullptr) {
-      css_slab = *css;
-      if (css_slab.css_start) css_slab.css_start += off;
-      if (css_slab.css) css_slab.css += off;
-      if (css_slab.css_stop) css_slab.css_stop += off;
-      if (css_slab.iters) css_slab.iters += off;
-    }
-    const int rc = run_device_slab(ctx, plan, y + off * ld_y, m, ld_y, pred_start, n_pred, out + off * ld_out, ld_out,
-                                   beta ? beta + off * P : nullptr, status + off, s, launches, kernel_used, more, n_out,
-                                   multimem, sel != nullptr ? &sel_slab : nullptr, se != nullptr ? &se_slab : nullptr,
-                                   ar != nullptr ? &ar_slab : nullptr, arsel != nullptr ? &arsel_slab : nullptr, arima,
-                                   nullptr, arma != nullptr ? &arma_slab : nullptr, nullptr,
-                                   css != nullptr ? &css_slab : nullptr);
-    if (rc != MMF_OK) return rc;
-    if (slab_pending != nullptr) {
-      if (*kernel_used == MMF_KERNEL_TC)
-        CU_TRY(cudaMemcpyAsync(slab_pending + i, ctx->d_pending + CTR_WORDS * ctx->last_set, sizeof(uint32_t),
-                               cudaMemcpyDeviceToDevice, s));
-      else
-        CU_TRY(cudaMemsetAsync(slab_pending + i, 0, sizeof(uint32_t), s));
+    for (size_t k = 0; k < stages.size(); ++k) {
+      Call c = stages[k].call.slice(off);
+      if (hr != nullptr) {
+        if (!c.ar->phi) c.ar->phi = hr;
+        if (!c.arma->theta) c.arma->theta = hr + (size_t)slab * MMF_AR_MAX;
+        if (!c.arma->ma_order) c.arma->ma_order = reinterpret_cast<int32_t*>(hr + (size_t)slab * (MMF_AR_MAX + MMF_MA_MAX));
+      }
+      const int rc = run_device_slab(ctx, *stages[k].plan, c, m, t);
+      if (rc != MMF_OK) return rc;
+      if (slab_pending != nullptr) {
+        uint32_t* dst = slab_pending + i * (int64_t)stages.size() + k;
+        if (t.kernel_used == MMF_KERNEL_TC)
+          CU_TRY(cudaMemcpyAsync(dst, ctx->d_pending + CTR_WORDS * ctx->last_set, sizeof(uint32_t),
+                                 cudaMemcpyDeviceToDevice, s));
+        else
+          CU_TRY(cudaMemsetAsync(dst, 0, sizeof(uint32_t), s));
+      }
     }
   }
   return MMF_OK;
 }
 
-// The status scratch is only referenced by a graph whose capture passed out_status == NULL; otherwise it may move.
-int grow_status_scratch(mmf_ctx* ctx, int64_t n, cudaStream_t s) {
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  if (cudaStreamIsCapturing(s, &cap) == cudaSuccess && cap != cudaStreamCaptureStatusNone) ctx->status_scratch_captured = true;
+// grow() for scratch no captured CUDA graph refers to: it may move while one is pinned
+int grow_unpinned(void** ptr, size_t* cap, size_t need) {
   const mmf_ctx* saved = g_grow_ctx;
-  if (!ctx->status_scratch_captured) g_grow_ctx = nullptr;
-  const int rc = grow((void**)&ctx->d_status_scratch, &ctx->status_scratch_cap, (size_t)n * sizeof(int32_t));
+  g_grow_ctx = nullptr;
+  const int rc = grow(ptr, cap, need);
   g_grow_ctx = saved;
   return rc;
+}
+
+// The status scratch is only referenced by a graph whose capture passed out_status == NULL; otherwise it may move.
+int grow_status_scratch(mmf_ctx* ctx, int64_t n) {
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(ctx->stream, &cap) == cudaSuccess && cap != cudaStreamCaptureStatusNone)
+    ctx->status_scratch_captured = true;
+  const size_t need = (size_t)n * sizeof(int32_t);
+  return ctx->status_scratch_captured ? grow((void**)&ctx->d_status_scratch, &ctx->status_scratch_cap, need)
+                                      : grow_unpinned((void**)&ctx->d_status_scratch, &ctx->status_scratch_cap, need);
+}
+
+// a call without a status buffer writes the context's status scratch (n words)
+int status_or_scratch(mmf_ctx* ctx, int32_t** status, int64_t n) {
+  if (*status != nullptr) return MMF_OK;
+  const int rc = grow_status_scratch(ctx, n);
+  if (rc == MMF_OK) *status = ctx->d_status_scratch;
+  return rc;
+}
+
+// A call with stats times its kernels from here (before its first launch) to stats_tail.
+int stats_begin(mmf_ctx* ctx, const mmf_stats* stats) {
+  if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, ctx->stream));
+  return MMF_OK;
+}
+
+// The stats of a call that ran stats_begin: waits for the stream, then the kernel time, the rows handed to the general
+// pass (`pend`, plus the n_pend words at `pend_dev`, read once the stream is done) and the launch bookkeeping.  Nothing
+// without stats.
+int stats_tail(mmf_ctx* ctx, mmf_stats* stats, int64_t n, const Tally& t, const uint32_t* pend_dev = nullptr,
+               size_t n_pend = 0, uint32_t pend = 0) {
+  if (!stats) return MMF_OK;
+  CU_TRY(cudaEventRecord(ctx->ev_k1, ctx->stream));
+  CU_TRY(cudaEventSynchronize(ctx->ev_k1));
+  CU_TRY(cudaEventElapsedTime(&stats->kernel_ms, ctx->ev_k0, ctx->ev_k1));
+  stats->total_ms = stats->kernel_ms;
+  std::vector<uint32_t> words(n_pend);
+  if (n_pend > 0) CU_TRY(cudaMemcpy(words.data(), pend_dev, n_pend * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  stats->n_pending = pend;
+  for (uint32_t v : words) stats->n_pending += v;
+  stats->n_series = n;
+  stats->kernel_launches = t.launches;
+  stats->kernel_used = t.kernel_used;
+  return MMF_OK;
+}
+
+// The device path of a fit call, its arguments checked (n > 0, device set): status or its scratch, the slab-pending
+// scratch when stats need it, the enqueue of every slab, the stats.
+int enqueue(mmf_ctx* ctx, const Plan& slab_plan, std::vector<Stage> stages, int64_t n, mmf_stats* stats) {
+  for (Stage& st : stages)
+    if (int rc = status_or_scratch(ctx, &st.call.status, n)) return rc;
+  // Several fits: every fit's tensor-core kernel zeroes the counter set the fit before it used, so the pending count
+  // of each is copied aside as it completes and summed at the end.  A call with stats synchronises and so is never
+  // captured: this scratch is not part of any graph and may grow while one is pinned.
+  const int64_t slab = slab_rows(slab_plan, n);
+  const size_t n_fits = (size_t)((n + slab - 1) / slab) * stages.size();
+  uint32_t* slab_pending = nullptr;
+  if (stats && n_fits > 1) {
+    if (int rc = grow_unpinned((void**)&ctx->d_slab_pending, &ctx->slab_pending_cap, n_fits * sizeof(uint32_t))) return rc;
+    slab_pending = ctx->d_slab_pending;
+  }
+  Tally t;
+  if (int rc = stats_begin(ctx, stats)) return rc;
+  if (int rc = run_device(ctx, slab_plan, stages, n, t, slab_pending)) return rc;
+  if (slab_pending != nullptr) return stats_tail(ctx, stats, n, t, slab_pending, n_fits);
+  return stats_tail(ctx, stats, n, t, ctx->d_pending + CTR_WORDS * ctx->last_set, t.kernel_used == MMF_KERNEL_TC ? 1 : 0);
+}
+
+// ---- argument checks shared by the entry points
+// the prediction rows [pred_start, pred_start + n_pred) inside the n_rows planned rows, and ld_out >= n_pred
+int check_window(int32_t pred_start, int32_t n_pred, int32_t n_rows, int64_t ld_out) {
+  if (n_pred < 1 || pred_start < 0 || (int64_t)pred_start + n_pred > n_rows)
+    return fail(MMF_E_INVALID, "prediction rows [%d,%d) outside the planned design (%d rows)", pred_start,
+                pred_start + n_pred, n_rows);
+  if (ld_out < n_pred) return fail(MMF_E_INVALID, "ld_out=%lld < n_pred=%d", (long long)ld_out, n_pred);
+  return MMF_OK;
+}
+
+// v[first .. count) ascending and distinct in [0, hi]
+int check_ascending(const char* name, const int32_t* v, int32_t count, int32_t hi, int first = 0) {
+  for (int j = first; j < count; ++j)
+    if (v[j] < 0 || v[j] > hi || (j > 0 && v[j] <= v[j - 1]))
+      return fail(MMF_E_INVALID, "%s must be ascending and distinct in [0,%d] (%s[%d]=%d)", name, hi, name, j, v[j]);
+  return MMF_OK;
+}
+
+// every pointer of `need`, and every non-null pointer of `opt`, is device (or managed) memory
+bool on_device(std::initializer_list<const void*> need, std::initializer_list<const void*> opt) {
+  for (const void* p : need)
+    if (!is_device_ptr(p)) return false;
+  for (const void* p : opt)
+    if (p && !is_device_ptr(p)) return false;
+  return true;
+}
+
+// Hannan-Rissanen long AR order for long_order = 0: min(32, max(2 max(p, q), floor(ln(t_fit - d)^2))), where lmax is
+// the largest p or q the call fits
+int32_t hr_long_order(int32_t lmax, int32_t t_fit_d) {
+  const double lt = std::log((double)t_fit_d);
+  return std::min<int32_t>(MMF_HR_LONG_MAX, std::max<int32_t>(2 * lmax, (int32_t)std::floor(lt * lt)));
+}
+
+// the plain-fit fields of a call
+Call plain_call(const float* y, int64_t ld_y, int32_t pred_start, int32_t n_pred, float* out, int64_t ld_out,
+                int32_t* status) {
+  Call c;
+  c.y = y; c.ld_y = ld_y; c.pred_start = pred_start; c.n_pred = n_pred; c.out = out; c.ld_out = ld_out; c.status = status;
+  return c;
+}
+
+ArArgs ar_args(int32_t p, float* phi, int32_t* order, float* sigma, const Plan& plan) {
+  ArArgs ar{};
+  ar.p = p; ar.phi = phi; ar.order = order; ar.sigma = sigma; ar.nz = plan.d_nz;
+  return ar;
+}
+
+// the levels' row pitch and fit rows of an ARIMA call (its y is the slab's), d = 0 .. MMF_DIFF_MAX
+ArimaArgs arima_args(int64_t ld_y, int32_t t_fit, int32_t d) {
+  ArimaArgs ma{};
+  ma.ld_y = ld_y; ma.t_fit = t_fit; ma.d = d;
+  return ma;
 }
 
 struct GrowScope {                                        // entry points that may reallocate scratch name their ctx
@@ -1004,10 +1172,7 @@ static int fit_forecast_impl(mmf_ctx* ctx, const void* y_any, int32_t dtype, int
   if (n < 0) return fail(MMF_E_INVALID, "n < 0");
   if (n > 0 && (!y || !out_pred)) return fail(MMF_E_INVALID, "y or out_pred is NULL");
   if (ld_y < pl.t_fit) return fail(MMF_E_INVALID, "ld_y=%lld < t_fit=%d", (long long)ld_y, pl.t_fit);
-  if (n_pred < 1 || pred_start < 0 || (int64_t)pred_start + n_pred > pl.n_rows)
-    return fail(MMF_E_INVALID, "prediction rows [%d,%d) outside the planned design (%d rows)", pred_start,
-                pred_start + n_pred, pl.n_rows);
-  if (ld_out < n_pred) return fail(MMF_E_INVALID, "ld_out=%lld < n_pred=%d", (long long)ld_out, n_pred);
+  if (int rc = check_window(pred_start, n_pred, pl.n_rows, ld_out)) return rc;
   if (stats) memset(stats, 0, sizeof(*stats));
   if (n == 0) return MMF_OK;
   CU_TRY(cudaSetDevice(ctx->device));
@@ -1015,53 +1180,15 @@ static int fit_forecast_impl(mmf_ctx* ctx, const void* y_any, int32_t dtype, int
   const bool y_dev = is_device_ptr(y), o_dev = is_device_ptr(out_pred);
   const bool b_dev = out_beta ? is_device_ptr(out_beta) : true;
   const bool s_dev = out_status ? is_device_ptr(out_status) : true;
-  int launches = 0, kernel_used = 0;
-  int64_t h2d = 0, d2h = 0;
-
+  Call c = plain_call(y, ld_y, pred_start, n_pred, out_pred, ld_out, out_status);
+  c.beta = out_beta;
   if (!is_int && y_dev && o_dev && b_dev && s_dev) {
     // ------------------------------------------------ all device: just enqueue
-    int32_t* status = out_status;
-    if (!status) {
-      int rc = grow_status_scratch(ctx, n, ctx->stream);
-      if (rc != MMF_OK) return rc;
-      status = ctx->d_status_scratch;
-    }
-    // Several slabs: every slab's tensor-core kernel zeroes the counter set the slab before it used, so the pending
-    // count of each slab is copied aside as it completes and summed here.  A call with stats synchronises and so is
-    // never captured: this scratch is not part of any graph and may grow while one is pinned.
-    const int64_t slab = slab_rows(ctx->plan, n);
-    const int64_t n_slabs = (n + slab - 1) / slab;
-    uint32_t* slab_pending = nullptr;
-    if (stats && n_slabs > 1) {
-      const mmf_ctx* saved = g_grow_ctx;
-      g_grow_ctx = nullptr;
-      const int rc = grow((void**)&ctx->d_slab_pending, &ctx->slab_pending_cap, (size_t)n_slabs * sizeof(uint32_t));
-      g_grow_ctx = saved;
-      if (rc != MMF_OK) return rc;
-      slab_pending = ctx->d_slab_pending;
-    }
-    if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, ctx->stream));
-    int rc = run_device(ctx, ctx->plan, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_beta, status,
-                        ctx->stream, &launches, &kernel_used, nullptr, 1, 0, nullptr, slab_pending);
-    if (rc != MMF_OK) return rc;
-    if (stats) {
-      CU_TRY(cudaEventRecord(ctx->ev_k1, ctx->stream));
-      CU_TRY(cudaEventSynchronize(ctx->ev_k1));
-      CU_TRY(cudaEventElapsedTime(&stats->kernel_ms, ctx->ev_k0, ctx->ev_k1));
-      stats->total_ms = stats->kernel_ms;
-      if (slab_pending != nullptr) {
-        std::vector<uint32_t> pend((size_t)n_slabs);
-        CU_TRY(cudaMemcpy(pend.data(), slab_pending, pend.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
-        stats->n_pending = 0;
-        for (uint32_t v : pend) stats->n_pending += v;
-      } else {
-        uint32_t pend = 0;
-        CU_TRY(cudaMemcpy(&pend, ctx->d_pending + CTR_WORDS * ctx->last_set, sizeof(pend), cudaMemcpyDeviceToHost));
-        stats->n_pending = (kernel_used == MMF_KERNEL_TC) ? pend : 0;
-      }
-    }
+    return enqueue(ctx, pl, {{&pl, c}}, n, stats);
   } else {
     // ------------------------------------------------ host buffers (or an integer series buffer): pipelined chunks
+    Tally t;
+    int64_t h2d = 0, d2h = 0;
     int64_t chunk = ctx->cfg.chunk_series > 0 ? ctx->cfg.chunk_series : 32768;
     if (chunk > n) chunk = n;
     const int64_t pitch = (pl.t_fit + 3) & ~3;                 // staged row pitch (floats), TMA-friendly
@@ -1122,20 +1249,19 @@ static int fit_forecast_impl(mmf_ctx* ctx, const void* y_any, int32_t dtype, int
       explicit HotScope(NarrowPool* q) : p(q) { if (p) narrow_pool_begin_call(p); }
       ~HotScope() { if (p) narrow_pool_end_call(p); }
     } hot_scope(narrow ? ctx->narrow_pool : nullptr);
-    const mmf_ctx* pinned_scope = g_grow_ctx;
-    g_grow_ctx = nullptr;                                       // staging slots are never part of a captured graph
-    for (int i = 0; i < NBUF; ++i) {
+    for (int i = 0; i < NBUF; ++i) {                           // staging slots are never part of a captured graph
       Staging& s = ctx->st[i];
       int rc = MMF_OK;
-      if (!y_dev || is_int) rc = grow((void**)&s.d_y, &s.y_cap, (size_t)chunk * pitch * sizeof(float));
+      if (!y_dev || is_int) rc = grow_unpinned((void**)&s.d_y, &s.y_cap, (size_t)chunk * pitch * sizeof(float));
       if (rc == MMF_OK && (is_int || narrow) && !y_dev)
-        rc = grow(&s.d_yraw, &s.yraw_cap, narrow ? (size_t)chunk * npitch * 2 : (size_t)chunk * rpitch * esize);
-      if (rc == MMF_OK && !o_dev) rc = grow((void**)&s.d_out, &s.out_cap, (size_t)chunk * opitch * sizeof(float));
-      if (rc == MMF_OK && out_beta && !b_dev) rc = grow((void**)&s.d_beta, &s.beta_cap, (size_t)chunk * P * sizeof(float));
-      if (rc == MMF_OK && (!out_status || !s_dev)) rc = grow((void**)&s.d_status, &s.status_cap, (size_t)chunk * sizeof(int32_t));
-      if (rc != MMF_OK) { g_grow_ctx = pinned_scope; return rc; }
+        rc = grow_unpinned(&s.d_yraw, &s.yraw_cap, narrow ? (size_t)chunk * npitch * 2 : (size_t)chunk * rpitch * esize);
+      if (rc == MMF_OK && !o_dev) rc = grow_unpinned((void**)&s.d_out, &s.out_cap, (size_t)chunk * opitch * sizeof(float));
+      if (rc == MMF_OK && out_beta && !b_dev)
+        rc = grow_unpinned((void**)&s.d_beta, &s.beta_cap, (size_t)chunk * P * sizeof(float));
+      if (rc == MMF_OK && (!out_status || !s_dev))
+        rc = grow_unpinned((void**)&s.d_status, &s.status_cap, (size_t)chunk * sizeof(int32_t));
+      if (rc != MMF_OK) return rc;
     }
-    g_grow_ctx = pinned_scope;
     CU_TRY(cudaEventRecord(ctx->ev_a, ctx->stream));
     CU_TRY(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_a, 0));
     CU_TRY(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_a, 0));
@@ -1163,7 +1289,7 @@ static int fit_forecast_impl(mmf_ctx* ctx, const void* y_any, int32_t dtype, int
           h2d += m * (int64_t)pl.t_fit * (int64_t)esize;
         }
         CU_TRY(launch_widen(dtype, raw, raw_ld, s.d_y, pitch, m, pl.t_fit, ctx->sm_count, ctx->stream));
-        ++launches;
+        ++t.launches;
         yk = s.d_y; ldk = pitch;
       } else if (y_dev) { yk = y + off * ld_y; ldk = ld_y; }
       else if ([&]() -> bool {
@@ -1195,7 +1321,7 @@ static int fit_forecast_impl(mmf_ctx* ctx, const void* y_any, int32_t dtype, int
         CU_TRY(cudaEventRecord(s.ev_h2d, ctx->s_h2d));
         CU_TRY(cudaStreamWaitEvent(ctx->stream, s.ev_h2d, 0));
         CU_TRY(launch_widen(MMF_DT_U16, s.d_yraw, npitch, s.d_y, pitch, m, pl.t_fit, ctx->sm_count, ctx->stream));
-        ++launches;
+        ++t.launches;
         yk = s.d_y; ldk = pitch;
         h2d += m * (int64_t)pl.t_fit * 2;
       } else {
@@ -1212,14 +1338,13 @@ static int fit_forecast_impl(mmf_ctx* ctx, const void* y_any, int32_t dtype, int
         yk = s.d_y; ldk = pitch;
         h2d += m * (int64_t)pl.t_fit * 4;
       }
-      float* ok = o_dev ? out_pred + off * ld_out : s.d_out;
-      const int64_t ldo = o_dev ? ld_out : opitch;
-      float* bk = out_beta ? (b_dev ? out_beta + off * P : s.d_beta) : nullptr;
-      int32_t* sk = (out_status && s_dev) ? out_status + off : s.d_status;
+      c.y = yk; c.ld_y = ldk;
+      c.out = o_dev ? out_pred + off * ld_out : s.d_out;
+      c.ld_out = o_dev ? ld_out : opitch;
+      c.beta = out_beta ? (b_dev ? out_beta + off * P : s.d_beta) : nullptr;
+      c.status = (out_status && s_dev) ? out_status + off : s.d_status;
       if (it >= NBUF) CU_TRY(cudaStreamWaitEvent(ctx->stream, s.ev_d2h, 0));        // output staging drained
-      int rc = run_device(ctx, ctx->plan, yk, m, ldk, pred_start, n_pred, ok, ldo, bk, sk, ctx->stream, &launches,
-                          &kernel_used);
-      if (rc != MMF_OK) return rc;
+      if (int rc = run_device(ctx, pl, {{&pl, c}}, m, t)) return rc;
       CU_TRY(cudaEventRecord(s.ev_comp, ctx->stream));
       bool any_d2h = false;
       if (!o_dev) {
@@ -1251,14 +1376,12 @@ static int fit_forecast_impl(mmf_ctx* ctx, const void* y_any, int32_t dtype, int
     if (stats) {
       CU_TRY(cudaEventElapsedTime(&stats->total_ms, ctx->ev_a, ctx->ev_b));
       stats->kernel_ms = 0.f;   // kernels overlap the copies here; use a device-pointer call to time them
+      stats->n_series = n;
+      stats->h2d_bytes = h2d;
+      stats->d2h_bytes = d2h;
+      stats->kernel_launches = t.launches;
+      stats->kernel_used = t.kernel_used;
     }
-  }
-  if (stats) {
-    stats->n_series = n;
-    stats->h2d_bytes = h2d;
-    stats->d2h_bytes = d2h;
-    stats->kernel_launches = launches;
-    stats->kernel_used = kernel_used;
   }
   return MMF_OK;
 }
@@ -1287,24 +1410,15 @@ int mmf_fit_forecast_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
   if (!out_se && !out_sigma && !out_dof)
     return fail(MMF_E_INVALID, "out_se, out_sigma and out_dof are all NULL: use mmf_fit_forecast_f32");
   if (ld_y < pl.t_fit) return fail(MMF_E_INVALID, "ld_y=%lld < t_fit=%d", (long long)ld_y, pl.t_fit);
-  if (n_pred < 1 || pred_start < 0 || (int64_t)pred_start + n_pred > pl.n_rows)
-    return fail(MMF_E_INVALID, "prediction rows [%d,%d) outside the planned design (%d rows)", pred_start,
-                pred_start + n_pred, pl.n_rows);
-  if (ld_out < n_pred) return fail(MMF_E_INVALID, "ld_out=%lld < n_pred=%d", (long long)ld_out, n_pred);
+  if (int rc = check_window(pred_start, n_pred, pl.n_rows, ld_out)) return rc;
   if (out_se && ld_se < n_pred) return fail(MMF_E_INVALID, "ld_se=%lld < n_pred=%d", (long long)ld_se, n_pred);
   if (stats) memset(stats, 0, sizeof(*stats));
   if (n == 0) return MMF_OK;
   CU_TRY(cudaSetDevice(ctx->device));
-  if (!is_device_ptr(y) || !is_device_ptr(out_pred) || (out_se && !is_device_ptr(out_se)) ||
-      (out_sigma && !is_device_ptr(out_sigma)) || (out_dof && !is_device_ptr(out_dof)) ||
-      (out_status && !is_device_ptr(out_status)))
+  if (!on_device({y, out_pred}, {out_se, out_sigma, out_dof, out_status}))
     return fail(MMF_E_UNSUPPORTED, "mmf_fit_forecast_se_f32 takes device buffers only");
-  int32_t* status = out_status;
-  if (!status) {
-    int rc = grow_status_scratch(ctx, n, ctx->stream);
-    if (rc != MMF_OK) return rc;
-    status = ctx->d_status_scratch;
-  }
+  Call c = plain_call(y, ld_y, pred_start, n_pred, out_pred, ld_out, out_status);
+  if (int rc = status_or_scratch(ctx, &c.status, n)) return rc;
   SeArgs se{};
   se.out_se = out_se; se.ld_se = ld_se; se.sigma = out_sigma; se.dof = out_dof; se.sfac = pl.d_sfac;
   if (!se.sigma) {
@@ -1312,84 +1426,8 @@ int mmf_fit_forecast_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
     if (rc != MMF_OK) return rc;
     se.sigma = ctx->d_sigma_scratch;
   }
-  const int64_t slab = slab_rows(ctx->plan, n);
-  const int64_t n_slabs = (n + slab - 1) / slab;
-  uint32_t* slab_pending = nullptr;
-  if (stats && n_slabs > 1) {
-    const mmf_ctx* saved = g_grow_ctx;
-    g_grow_ctx = nullptr;
-    const int rc = grow((void**)&ctx->d_slab_pending, &ctx->slab_pending_cap, (size_t)n_slabs * sizeof(uint32_t));
-    g_grow_ctx = saved;
-    if (rc != MMF_OK) return rc;
-    slab_pending = ctx->d_slab_pending;
-  }
-  int launches = 0, kernel_used = 0;
-  if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, ctx->stream));
-  int rc = run_device(ctx, ctx->plan, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, nullptr, status, ctx->stream,
-                      &launches, &kernel_used, nullptr, 1, 0, nullptr, slab_pending, &se);
-  if (rc != MMF_OK) return rc;
-  if (stats) {
-    CU_TRY(cudaEventRecord(ctx->ev_k1, ctx->stream));
-    CU_TRY(cudaEventSynchronize(ctx->ev_k1));
-    CU_TRY(cudaEventElapsedTime(&stats->kernel_ms, ctx->ev_k0, ctx->ev_k1));
-    stats->total_ms = stats->kernel_ms;
-    std::vector<uint32_t> pend((size_t)n_slabs, 0u);
-    if (slab_pending != nullptr)
-      CU_TRY(cudaMemcpy(pend.data(), slab_pending, pend.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
-    else if (kernel_used == MMF_KERNEL_TC)
-      CU_TRY(cudaMemcpy(pend.data(), ctx->d_pending + CTR_WORDS * ctx->last_set, sizeof(uint32_t), cudaMemcpyDeviceToHost));
-    for (uint32_t v : pend) stats->n_pending += v;
-    stats->n_series = n;
-    stats->kernel_launches = launches;
-    stats->kernel_used = kernel_used;
-  }
-  return MMF_OK;
-}
-
-// the enqueue / stats tail of the AR entry points (arguments already checked, n > 0, device set)
-static int run_ar_call(mmf_ctx* ctx, const Plan& plan, const float* y, int64_t n, int64_t ld_y, int32_t pred_start,
-                       int32_t n_pred, float* out_pred, int64_t ld_out, int32_t* out_status, const ArArgs& ar,
-                       const ArSelArgs* arsel, const ArimaArgs* arima, mmf_stats* stats,
-                       const ArmaArgs* arma = nullptr, const CssArgs* css = nullptr) {
-  int32_t* status = out_status;
-  if (!status) {
-    int rc = grow_status_scratch(ctx, n, ctx->stream);
-    if (rc != MMF_OK) return rc;
-    status = ctx->d_status_scratch;
-  }
-  const int64_t slab = slab_rows(plan, n);
-  const int64_t n_slabs = (n + slab - 1) / slab;
-  uint32_t* slab_pending = nullptr;
-  if (stats && n_slabs > 1) {
-    const mmf_ctx* saved = g_grow_ctx;
-    g_grow_ctx = nullptr;
-    const int rc = grow((void**)&ctx->d_slab_pending, &ctx->slab_pending_cap, (size_t)n_slabs * sizeof(uint32_t));
-    g_grow_ctx = saved;
-    if (rc != MMF_OK) return rc;
-    slab_pending = ctx->d_slab_pending;
-  }
-  int launches = 0, kernel_used = 0;
-  if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, ctx->stream));
-  int rc = run_device(ctx, plan, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, nullptr, status, ctx->stream,
-                      &launches, &kernel_used, nullptr, 1, 0, nullptr, slab_pending, nullptr, &ar, arsel, arima, arma,
-                      css);
-  if (rc != MMF_OK) return rc;
-  if (stats) {
-    CU_TRY(cudaEventRecord(ctx->ev_k1, ctx->stream));
-    CU_TRY(cudaEventSynchronize(ctx->ev_k1));
-    CU_TRY(cudaEventElapsedTime(&stats->kernel_ms, ctx->ev_k0, ctx->ev_k1));
-    stats->total_ms = stats->kernel_ms;
-    std::vector<uint32_t> pend((size_t)n_slabs, 0u);
-    if (slab_pending != nullptr)
-      CU_TRY(cudaMemcpy(pend.data(), slab_pending, pend.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
-    else if (kernel_used == MMF_KERNEL_TC)
-      CU_TRY(cudaMemcpy(pend.data(), ctx->d_pending + CTR_WORDS * ctx->last_set, sizeof(uint32_t), cudaMemcpyDeviceToHost));
-    for (uint32_t v : pend) stats->n_pending += v;
-    stats->n_series = n;
-    stats->kernel_launches = launches;
-    stats->kernel_used = kernel_used;
-  }
-  return MMF_OK;
+  c.se = se;
+  return enqueue(ctx, pl, {{&pl, c}}, n, stats);
 }
 
 int mmf_fit_forecast_ar_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order, int32_t pred_start,
@@ -1403,20 +1441,15 @@ int mmf_fit_forecast_ar_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
   if (n > 0 && (!y || !out_pred)) return fail(MMF_E_INVALID, "y or out_pred is NULL");
   if (ar_order < 1 || ar_order > MMF_AR_MAX) return fail(MMF_E_INVALID, "ar_order=%d outside [1,%d]", ar_order, MMF_AR_MAX);
   if (ld_y < pl.t_fit) return fail(MMF_E_INVALID, "ld_y=%lld < t_fit=%d", (long long)ld_y, pl.t_fit);
-  if (n_pred < 1 || pred_start < 0 || (int64_t)pred_start + n_pred > pl.n_rows)
-    return fail(MMF_E_INVALID, "prediction rows [%d,%d) outside the planned design (%d rows)", pred_start,
-                pred_start + n_pred, pl.n_rows);
-  if (ld_out < n_pred) return fail(MMF_E_INVALID, "ld_out=%lld < n_pred=%d", (long long)ld_out, n_pred);
+  if (int rc = check_window(pred_start, n_pred, pl.n_rows, ld_out)) return rc;
   if (stats) memset(stats, 0, sizeof(*stats));
   if (n == 0) return MMF_OK;
   CU_TRY(cudaSetDevice(ctx->device));
-  if (!is_device_ptr(y) || !is_device_ptr(out_pred) || (out_phi && !is_device_ptr(out_phi)) ||
-      (out_order && !is_device_ptr(out_order)) || (out_sigma && !is_device_ptr(out_sigma)) ||
-      (out_status && !is_device_ptr(out_status)))
+  if (!on_device({y, out_pred}, {out_phi, out_order, out_sigma, out_status}))
     return fail(MMF_E_UNSUPPORTED, "mmf_fit_forecast_ar_f32 takes device buffers only");
-  ArArgs ar{};
-  ar.p = ar_order; ar.phi = out_phi; ar.order = out_order; ar.sigma = out_sigma; ar.nz = pl.d_nz;
-  return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, nullptr, stats);
+  Call c = plain_call(y, ld_y, pred_start, n_pred, out_pred, ld_out, out_status);
+  c.ar = ar_args(ar_order, out_phi, out_order, out_sigma, pl);
+  return enqueue(ctx, pl, {{&pl, c}}, n, stats);
 }
 
 int mmf_fit_select_ar_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
@@ -1431,34 +1464,26 @@ int mmf_fit_select_ar_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y,
   if (n > 0 && (!y || !out_pred)) return fail(MMF_E_INVALID, "y or out_pred is NULL");
   if (!orders || n_orders < 1 || n_orders > MMF_ARSEL_MAX_CAND)
     return fail(MMF_E_INVALID, "n_orders=%d outside [1,%d] (or orders is NULL)", n_orders, MMF_ARSEL_MAX_CAND);
-  for (int j = 0; j < n_orders; ++j)
-    if (orders[j] < 0 || orders[j] > MMF_AR_MAX || (j > 0 && orders[j] <= orders[j - 1]))
-      return fail(MMF_E_INVALID, "orders must be ascending and distinct in [0,%d] (orders[%d]=%d)", MMF_AR_MAX, j,
-                  orders[j]);
+  if (int rc = check_ascending("orders", orders, n_orders, MMF_AR_MAX)) return rc;
   if (n_hold < 1 || (int64_t)pl.t_fit + n_hold > pl.n_rows)
     return fail(MMF_E_INVALID, "held-out rows [%d,%lld) outside the planned design (%d rows)", pl.t_fit,
                 (long long)pl.t_fit + n_hold, pl.n_rows);
   if (ld_y < (int64_t)pl.t_fit + n_hold)
     return fail(MMF_E_INVALID, "ld_y=%lld < t_fit + n_hold=%lld", (long long)ld_y, (long long)pl.t_fit + n_hold);
-  if (n_pred < 1 || pred_start < 0 || (int64_t)pred_start + n_pred > pl.n_rows)
-    return fail(MMF_E_INVALID, "prediction rows [%d,%d) outside the planned design (%d rows)", pred_start,
-                pred_start + n_pred, pl.n_rows);
-  if (ld_out < n_pred) return fail(MMF_E_INVALID, "ld_out=%lld < n_pred=%d", (long long)ld_out, n_pred);
+  if (int rc = check_window(pred_start, n_pred, pl.n_rows, ld_out)) return rc;
   if (stats) memset(stats, 0, sizeof(*stats));
   if (n == 0) return MMF_OK;
   CU_TRY(cudaSetDevice(ctx->device));
-  if (!is_device_ptr(y) || !is_device_ptr(out_pred) || (out_choice && !is_device_ptr(out_choice)) ||
-      (out_mse && !is_device_ptr(out_mse)) || (out_cand_mse && !is_device_ptr(out_cand_mse)) ||
-      (out_phi && !is_device_ptr(out_phi)) || (out_order && !is_device_ptr(out_order)) ||
-      (out_sigma && !is_device_ptr(out_sigma)) || (out_status && !is_device_ptr(out_status)))
+  if (!on_device({y, out_pred}, {out_choice, out_mse, out_cand_mse, out_phi, out_order, out_sigma, out_status}))
     return fail(MMF_E_UNSUPPORTED, "mmf_fit_select_ar_f32 takes device buffers only");
-  ArArgs ar{};
-  ar.p = orders[n_orders - 1]; ar.phi = out_phi; ar.order = out_order; ar.sigma = out_sigma; ar.nz = pl.d_nz;
+  Call c = plain_call(y, ld_y, pred_start, n_pred, out_pred, ld_out, out_status);
+  c.ar = ar_args(orders[n_orders - 1], out_phi, out_order, out_sigma, pl);
   ArSelArgs sel{};
   sel.n_hold = n_hold; sel.n_cand = n_orders;
   for (int j = 0; j < n_orders; ++j) sel.cand[j] = orders[j];
   sel.choice = out_choice; sel.mse = out_mse; sel.cand_mse = out_cand_mse;
-  return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, &sel, nullptr, stats);
+  c.arsel = sel;
+  return enqueue(ctx, pl, {{&pl, c}}, n, stats);
 }
 
 // ---- regression with ARIMA(p, d, 0) errors (DESIGN.md section 2 item 11) ------------------------------------------
@@ -1526,23 +1551,17 @@ int mmf_fit_forecast_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t 
   if (diff_order < 1 || diff_order > ap.max_diff)
     return fail(MMF_E_INVALID, "diff_order=%d outside [1,%d] (the planned max_diff)", diff_order, ap.max_diff);
   if (ld_y < ap.t_fit) return fail(MMF_E_INVALID, "ld_y=%lld < t_fit=%d", (long long)ld_y, ap.t_fit);
-  if (n_pred < 1 || pred_start < 0 || (int64_t)pred_start + n_pred > ap.n_rows)
-    return fail(MMF_E_INVALID, "prediction rows [%d,%d) outside the planned design (%d rows)", pred_start,
-                pred_start + n_pred, ap.n_rows);
-  if (ld_out < n_pred) return fail(MMF_E_INVALID, "ld_out=%lld < n_pred=%d", (long long)ld_out, n_pred);
+  if (int rc = check_window(pred_start, n_pred, ap.n_rows, ld_out)) return rc;
   if (stats) memset(stats, 0, sizeof(*stats));
   if (n == 0) return MMF_OK;
   CU_TRY(cudaSetDevice(ctx->device));
-  if (!is_device_ptr(y) || !is_device_ptr(out_pred) || (out_phi && !is_device_ptr(out_phi)) ||
-      (out_order && !is_device_ptr(out_order)) || (out_sigma && !is_device_ptr(out_sigma)) ||
-      (out_status && !is_device_ptr(out_status)))
+  if (!on_device({y, out_pred}, {out_phi, out_order, out_sigma, out_status}))
     return fail(MMF_E_UNSUPPORTED, "mmf_fit_forecast_arima_f32 takes device buffers only");
   const Plan& pl = ap.diff[diff_order - 1];
-  ArArgs ar{};
-  ar.p = ar_order; ar.phi = out_phi; ar.order = out_order; ar.sigma = out_sigma; ar.nz = pl.d_nz;
-  ArimaArgs ma{};
-  ma.y = y; ma.ld_y = ld_y; ma.t_fit = ap.t_fit; ma.d = diff_order;
-  return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, &ma, stats);
+  Call c = plain_call(y, ld_y, pred_start, n_pred, out_pred, ld_out, out_status);
+  c.ar = ar_args(ar_order, out_phi, out_order, out_sigma, pl);
+  c.arima = arima_args(ld_y, ap.t_fit, diff_order);
+  return enqueue(ctx, pl, {{&pl, c}}, n, stats);
 }
 
 // ---- regression with ARIMA(p, d, q) errors (DESIGN.md section 2 items 13, 16) --------------------------------------------
@@ -1574,37 +1593,24 @@ static int arma_call(mmf_ctx* ctx, const char* name, const float* y, int64_t n, 
   if (long_order != 0 && (long_order < lmin || long_order > MMF_HR_LONG_MAX))
     return fail(MMF_E_INVALID, "long_order=%d outside {0} and [%d,%d]", long_order, lmin, MMF_HR_LONG_MAX);
   if (ld_y < T) return fail(MMF_E_INVALID, "ld_y=%lld < t_fit=%d", (long long)ld_y, T);
-  if (n_pred < 1 || pred_start < 0 || (int64_t)pred_start + n_pred > n_rows)
-    return fail(MMF_E_INVALID, "prediction rows [%d,%d) outside the planned design (%d rows)", pred_start,
-                pred_start + n_pred, n_rows);
-  if (ld_out < n_pred) return fail(MMF_E_INVALID, "ld_out=%lld < n_pred=%d", (long long)ld_out, n_pred);
+  if (int rc = check_window(pred_start, n_pred, n_rows, ld_out)) return rc;
   if (stats) memset(stats, 0, sizeof(*stats));
   if (n == 0) return MMF_OK;
   CU_TRY(cudaSetDevice(ctx->device));
-  if (!is_device_ptr(y) || !is_device_ptr(out_pred) || (out_phi && !is_device_ptr(out_phi)) ||
-      (out_theta && !is_device_ptr(out_theta)) || (out_order && !is_device_ptr(out_order)) ||
-      (out_ma_order && !is_device_ptr(out_ma_order)) || (out_sigma && !is_device_ptr(out_sigma)) ||
-      (out_status && !is_device_ptr(out_status)) ||
-      (css && ((css->css_start && !is_device_ptr(css->css_start)) || (css->css && !is_device_ptr(css->css)) ||
-               (css->css_stop && !is_device_ptr(css->css_stop)) || (css->iters && !is_device_ptr(css->iters)))))
+  if (!on_device({y, out_pred}, {out_phi, out_theta, out_order, out_ma_order, out_sigma, out_status,
+                                 css ? css->css_start : nullptr, css ? css->css : nullptr, css ? css->css_stop : nullptr,
+                                 css ? css->iters : nullptr}))
     return fail(MMF_E_UNSUPPORTED, "%s takes device buffers only", name);
-  ArArgs ar{};
-  ar.p = ar_order; ar.phi = out_phi; ar.order = out_order; ar.sigma = out_sigma; ar.nz = pl.d_nz;
+  Call c = plain_call(y, ld_y, pred_start, n_pred, out_pred, ld_out, out_status);
+  c.ar = ar_args(ar_order, out_phi, out_order, out_sigma, pl);
   ArmaArgs hr{};
   hr.q = ma_order;
-  if (long_order == 0) {                   // min(32, max(2 max(p, q), floor(ln(t_fit - d)^2)))
-    const double lt = std::log((double)(T - diff_order));
-    long_order = std::min<int32_t>(MMF_HR_LONG_MAX, std::max<int32_t>(2 * lmin, (int32_t)std::floor(lt * lt)));
-  }
-  hr.m = long_order;
+  hr.m = long_order != 0 ? long_order : hr_long_order(lmin, T - diff_order);
   hr.theta = out_theta; hr.ma_order = out_ma_order;
-  if (diff_order == 0)
-    return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, nullptr,
-                       stats, &hr, css);
-  ArimaArgs ma{};
-  ma.y = y; ma.ld_y = ld_y; ma.t_fit = ap.t_fit; ma.d = diff_order;
-  return run_ar_call(ctx, pl, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, out_status, ar, nullptr, &ma, stats, &hr,
-                     css);
+  c.arma = hr;
+  if (diff_order > 0) c.arima = arima_args(ld_y, ap.t_fit, diff_order);
+  if (css) c.css = *css;
+  return enqueue(ctx, pl, {{&pl, c}}, n, stats);
 }
 
 int mmf_fit_forecast_arma_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
@@ -1657,26 +1663,15 @@ int mmf_arima_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int3
   if (stats) memset(stats, 0, sizeof(*stats));
   if (n == 0) return MMF_OK;
   CU_TRY(cudaSetDevice(ctx->device));
-  if (!is_device_ptr(y) || !is_device_ptr(phi) || !is_device_ptr(order) || !is_device_ptr(sigma) ||
-      !is_device_ptr(out_se) || (diffs && !is_device_ptr(diffs)) || (theta && !is_device_ptr(theta)) ||
-      (ma_order && !is_device_ptr(ma_order)))
+  if (!on_device({y, phi, order, sigma, out_se}, {diffs, theta, ma_order}))
     return fail(MMF_E_UNSUPPORTED, "mmf_arima_se_f32 takes device buffers only");
   ArimaSeArgs a{};
   a.y = y; a.ld_y = ld_y; a.t_fit = t_fit; a.diff_order = diff_order; a.diffs = diffs;
   a.phi = phi; a.order = order; a.theta = theta; a.ma_order = ma_order; a.sigma = sigma;
   a.pred_start = pred_start; a.n_pred = n_pred; a.out = out_se; a.ld_se = ld_se; a.n = n;
-  if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, ctx->stream));
+  if (int rc = stats_begin(ctx, stats)) return rc;
   CU_TRY(launch_arima_se(a, ctx->sm_count, ctx->stream));
-  if (stats) {
-    CU_TRY(cudaEventRecord(ctx->ev_k1, ctx->stream));
-    CU_TRY(cudaEventSynchronize(ctx->ev_k1));
-    CU_TRY(cudaEventElapsedTime(&stats->kernel_ms, ctx->ev_k0, ctx->ev_k1));
-    stats->total_ms = stats->kernel_ms;
-    stats->n_series = n;
-    stats->kernel_launches = 1;
-    stats->kernel_used = MMF_KERNEL_WARP;
-  }
-  return MMF_OK;
+  return stats_tail(ctx, stats, n, Tally{1, MMF_KERNEL_WARP});
 }
 
 // ---- (p, d) and (p, d, q) selection by hold-out MSE on levels (DESIGN.md section 2 items 12, 14) ------------------------
@@ -1695,23 +1690,15 @@ static int select_arima_call(mmf_ctx* ctx, const char* name, bool with_q, const 
   if (n > 0 && (!y || !out_pred)) return fail(MMF_E_INVALID, "y or out_pred is NULL");
   if (!orders || n_orders < 1 || n_orders > MMF_ARSEL_MAX_CAND)
     return fail(MMF_E_INVALID, "n_orders=%d outside [1,%d] (or orders is NULL)", n_orders, MMF_ARSEL_MAX_CAND);
-  for (int j = 0; j < n_orders; ++j)
-    if (orders[j] < 0 || orders[j] > MMF_AR_MAX || (j > 0 && orders[j] <= orders[j - 1]))
-      return fail(MMF_E_INVALID, "orders must be ascending and distinct in [0,%d] (orders[%d]=%d)", MMF_AR_MAX, j,
-                  orders[j]);
+  if (int rc = check_ascending("orders", orders, n_orders, MMF_AR_MAX)) return rc;
   if (!diffs || n_diffs < 1 || n_diffs > MMF_DIFF_MAX + 1)
     return fail(MMF_E_INVALID, "n_diffs=%d outside [1,%d] (or diffs is NULL)", n_diffs, MMF_DIFF_MAX + 1);
-  for (int j = 0; j < n_diffs; ++j)
-    if (diffs[j] < 0 || diffs[j] > MMF_DIFF_MAX || (j > 0 && diffs[j] <= diffs[j - 1]))
-      return fail(MMF_E_INVALID, "diffs must be ascending and distinct in [0,%d] (diffs[%d]=%d)", MMF_DIFF_MAX, j,
-                  diffs[j]);
+  if (int rc = check_ascending("diffs", diffs, n_diffs, MMF_DIFF_MAX)) return rc;
   if (with_q) {
     if (!mas || n_mas < 1 || n_mas > MMF_MA_MAX + 1)
       return fail(MMF_E_INVALID, "n_mas=%d outside [1,%d] (or mas is NULL)", n_mas, MMF_MA_MAX + 1);
     if (mas[0] != 0) return fail(MMF_E_INVALID, "mas[0]=%d: the MA orders must start with 0", mas[0]);
-    for (int j = 1; j < n_mas; ++j)
-      if (mas[j] > MMF_MA_MAX || mas[j] <= mas[j - 1])
-        return fail(MMF_E_INVALID, "mas must be ascending and distinct in [0,%d] (mas[%d]=%d)", MMF_MA_MAX, j, mas[j]);
+    if (int rc = check_ascending("mas", mas, n_mas, MMF_MA_MAX, 1)) return rc;
     if (n_orders * (n_mas - 1) > MMF_ARMASEL_MAX_PQ)
       return fail(MMF_E_INVALID, "%d x %d (p, q >= 1) pairs above MMF_ARMASEL_MAX_PQ=%d", n_orders, n_mas - 1,
                   MMF_ARMASEL_MAX_PQ);
@@ -1739,19 +1726,12 @@ static int select_arima_call(mmf_ctx* ctx, const char* name, bool with_q, const 
                 n_rows);
   if (ld_y < (int64_t)T + n_hold)
     return fail(MMF_E_INVALID, "ld_y=%lld < t_fit + n_hold=%lld", (long long)ld_y, (long long)T + n_hold);
-  if (n_pred < 1 || pred_start < 0 || (int64_t)pred_start + n_pred > n_rows)
-    return fail(MMF_E_INVALID, "prediction rows [%d,%d) outside the planned design (%d rows)", pred_start,
-                pred_start + n_pred, n_rows);
-  if (ld_out < n_pred) return fail(MMF_E_INVALID, "ld_out=%lld < n_pred=%d", (long long)ld_out, n_pred);
+  if (int rc = check_window(pred_start, n_pred, n_rows, ld_out)) return rc;
   if (stats) memset(stats, 0, sizeof(*stats));
   if (n == 0) return MMF_OK;
   CU_TRY(cudaSetDevice(ctx->device));
-  if (!is_device_ptr(y) || !is_device_ptr(out_pred) || (out_choice_p && !is_device_ptr(out_choice_p)) ||
-      (out_choice_d && !is_device_ptr(out_choice_d)) || (out_mse && !is_device_ptr(out_mse)) ||
-      (out_cand_mse && !is_device_ptr(out_cand_mse)) || (out_phi && !is_device_ptr(out_phi)) ||
-      (out_order && !is_device_ptr(out_order)) || (out_sigma && !is_device_ptr(out_sigma)) ||
-      (out_status && !is_device_ptr(out_status)) || (out_choice_q && !is_device_ptr(out_choice_q)) ||
-      (out_theta && !is_device_ptr(out_theta)) || (out_ma_order && !is_device_ptr(out_ma_order)))
+  if (!on_device({y, out_pred}, {out_choice_p, out_choice_d, out_mse, out_cand_mse, out_phi, out_order, out_sigma,
+                                 out_status, out_choice_q, out_theta, out_ma_order}))
     return fail(MMF_E_UNSUPPORTED, "%s takes device buffers only", name);
 
   // (p, d, q) selection: the (p, q >= 1) pairs q-major, and their row sets R(q, L = max(p, q)) in order of appearance
@@ -1776,92 +1756,41 @@ static int select_arima_call(mmf_ctx* ctx, const char* name, bool with_q, const 
   }
 
   // slabs as the plain fit of the level rows would cut them; per slab, one fit and one arima_select_kernel per listed d
+  // (their status goes to per-slab scratch, arima_select_kernel writes the caller's)
   const Plan& level_plan = use_plain ? pl : ap.diff[0];
   const int64_t slab = slab_rows(level_plan, n);
-  const int64_t n_slabs = (n + slab - 1) / slab;
   int rc = grow((void**)&ctx->d_asel_best, &ctx->asel_best_cap, (size_t)slab * sizeof(ArimaSelBest));
   if (rc == MMF_OK) rc = grow((void**)&ctx->d_asel_status, &ctx->asel_status_cap, (size_t)slab * sizeof(int32_t));
   if (rc == MMF_OK && with_q)
     rc = grow((void**)&ctx->d_hsel_q0, &ctx->hsel_q0_cap, (size_t)slab * n_diffs * n_orders * sizeof(float));
   if (rc != MMF_OK) return rc;
-  uint32_t* slab_pending = nullptr;        // rows each fit handed to the general pass (stats)
-  if (stats) {
-    const mmf_ctx* saved = g_grow_ctx;
-    g_grow_ctx = nullptr;
-    rc = grow((void**)&ctx->d_slab_pending, &ctx->slab_pending_cap, (size_t)(n_slabs * n_diffs) * sizeof(uint32_t));
-    g_grow_ctx = saved;
-    if (rc != MMF_OK) return rc;
-    slab_pending = ctx->d_slab_pending;
-  }
-  const cudaStream_t s = ctx->stream;
-  int launches = 0, kernel_used = 0;
-  if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, s));
-  for (int64_t off = 0, i = 0; off < n; off += slab, ++i) {
-    const int64_t m = std::min(slab, n - off);
-    for (int k = 0; k < n_diffs; ++k) {
-      const int dd = diffs[k];
-      const Plan& plan = dd == 0 ? pl : ap.diff[dd - 1];
-      ArArgs ar{};
-      ar.p = orders[n_orders - 1];
-      ar.phi = out_phi ? out_phi + off * MMF_AR_MAX : nullptr;
-      ar.order = out_order ? out_order + off : nullptr;
-      ar.sigma = out_sigma ? out_sigma + off : nullptr;
-      ar.nz = plan.d_nz;
-      ArimaArgs ma{};
-      ma.ld_y = ld_y; ma.t_fit = T; ma.d = dd;
-      ArimaSelArgs sel{};
-      sel.n_hold = n_hold; sel.n_cand = n_orders;
-      for (int j = 0; j < n_orders; ++j) sel.cand[j] = orders[j];
-      sel.d_index = k; sel.n_diffs = n_diffs;
-      sel.best = ctx->d_asel_best;
-      sel.choice_p = out_choice_p ? out_choice_p + off : nullptr;
-      sel.choice_d = out_choice_d ? out_choice_d + off : nullptr;
-      sel.mse = out_mse ? out_mse + off : nullptr;
-      sel.cand_mse = out_cand_mse ? out_cand_mse + off * n_diffs * n_orders : nullptr;
-      sel.status = out_status ? out_status + off : nullptr;
+  std::vector<Stage> stages;
+  for (int k = 0; k < n_diffs; ++k) {
+    const int dd = diffs[k];
+    const Plan& plan = dd == 0 ? pl : ap.diff[dd - 1];
+    Call c = plain_call(y, ld_y, pred_start, n_pred, out_pred, ld_out, ctx->d_asel_status);
+    c.ar = ar_args(orders[n_orders - 1], out_phi, out_order, out_sigma, plan);
+    c.arima = arima_args(ld_y, T, dd);
+    ArimaSelArgs sel{};
+    sel.n_hold = n_hold; sel.n_cand = n_orders;
+    for (int j = 0; j < n_orders; ++j) sel.cand[j] = orders[j];
+    sel.d_index = k; sel.n_diffs = n_diffs;
+    sel.best = ctx->d_asel_best;
+    sel.choice_p = out_choice_p; sel.choice_d = out_choice_d; sel.mse = out_mse; sel.cand_mse = out_cand_mse;
+    sel.status = out_status;
+    if (with_q) {
+      // arima_select_kernel's scores go to scratch: arma_select_kernel copies them into the q = 0 slice
+      sel.cand_mse = ctx->d_hsel_q0;
       ArmaSelArgs hsd = hs;
-      if (with_q) {
-        // arima_select_kernel's scores go to scratch: arma_select_kernel copies them into the q = 0 slice
-        sel.cand_mse = ctx->d_hsel_q0;
-        hsd.cand_q0 = ctx->d_hsel_q0;
-        hsd.cand_mse = out_cand_mse ? out_cand_mse + off * n_diffs * n_mas * n_orders : nullptr;
-        hsd.choice_q = out_choice_q ? out_choice_q + off : nullptr;
-        hsd.theta = out_theta ? out_theta + off * MMF_MA_MAX : nullptr;
-        hsd.ma_order = out_ma_order ? out_ma_order + off : nullptr;
-        hsd.m = long_order;
-        if (long_order == 0) {             // min(32, max(2 max(orders, mas), floor(ln(t_fit - d)^2)))
-          const double lt = std::log((double)(T - dd));
-          const int32_t lmax = std::max(orders[n_orders - 1], mas[n_mas - 1]);
-          hsd.m = std::min<int32_t>(MMF_HR_LONG_MAX, std::max<int32_t>(2 * lmax, (int32_t)std::floor(lt * lt)));
-        }
-      }
-      rc = run_device_slab(ctx, plan, y + off * ld_y, m, ld_y, pred_start, n_pred, out_pred + off * ld_out, ld_out,
-                           nullptr, ctx->d_asel_status, s, &launches, &kernel_used, nullptr, 1, 0, nullptr, nullptr,
-                           &ar, nullptr, &ma, &sel, nullptr, with_q ? &hsd : nullptr);
-      if (rc != MMF_OK) return rc;
-      if (slab_pending != nullptr) {
-        uint32_t* dst = slab_pending + i * n_diffs + k;
-        if (kernel_used == MMF_KERNEL_TC)
-          CU_TRY(cudaMemcpyAsync(dst, ctx->d_pending + CTR_WORDS * ctx->last_set, sizeof(uint32_t),
-                                 cudaMemcpyDeviceToDevice, s));
-        else
-          CU_TRY(cudaMemsetAsync(dst, 0, sizeof(uint32_t), s));
-      }
+      hsd.cand_q0 = ctx->d_hsel_q0;
+      hsd.cand_mse = out_cand_mse; hsd.choice_q = out_choice_q; hsd.theta = out_theta; hsd.ma_order = out_ma_order;
+      hsd.m = long_order != 0 ? long_order : hr_long_order(std::max(orders[n_orders - 1], mas[n_mas - 1]), T - dd);
+      c.hsel = hsd;
     }
+    c.asel = sel;
+    stages.push_back({&plan, c});
   }
-  if (stats) {
-    CU_TRY(cudaEventRecord(ctx->ev_k1, s));
-    CU_TRY(cudaEventSynchronize(ctx->ev_k1));
-    CU_TRY(cudaEventElapsedTime(&stats->kernel_ms, ctx->ev_k0, ctx->ev_k1));
-    stats->total_ms = stats->kernel_ms;
-    std::vector<uint32_t> pend((size_t)(n_slabs * n_diffs), 0u);
-    CU_TRY(cudaMemcpy(pend.data(), slab_pending, pend.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
-    for (uint32_t v : pend) stats->n_pending += v;
-    stats->n_series = n;
-    stats->kernel_launches = launches;
-    stats->kernel_used = kernel_used;
-  }
-  return MMF_OK;
+  return enqueue(ctx, level_plan, std::move(stages), n, stats);
 }
 
 int mmf_fit_select_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
@@ -1928,8 +1857,7 @@ int mmf_fit_forecast_ragged_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t
   if (n == 0) return MMF_OK;
   if (n > (int64_t)0x7fffffff - 128) return fail(MMF_E_UNSUPPORTED, "n too large for 32-bit TMA coordinates");
   CU_TRY(cudaSetDevice(ctx->device));
-  if (!is_device_ptr(y) || !is_device_ptr(out_pred) || (out_status && !is_device_ptr(out_status)))
-    return fail(MMF_E_INVALID, "the ragged entry point takes device buffers only");
+  if (!on_device({y, out_pred}, {out_status})) return fail(MMF_E_INVALID, "the ragged entry point takes device buffers only");
   if (ld_y % 4 != 0 || (reinterpret_cast<uintptr_t>(y) & 15u) != 0 || (reinterpret_cast<uintptr_t>(out_pred) & 15u) != 0)
     return fail(MMF_E_UNSUPPORTED, "ragged batches need 16-B aligned y / out_pred and ld_y %% 4 == 0 (TMA)");
   cudaStream_t s = ctx->stream;
@@ -1937,11 +1865,7 @@ int mmf_fit_forecast_ragged_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t
   CU_TRY(cudaStreamIsCapturing(s, &cap));
   if (cap != cudaStreamCaptureStatusNone) return fail(MMF_E_UNSUPPORTED, "ragged batches cannot be captured into a CUDA graph");
   int32_t* status = out_status;
-  if (!status) {
-    int rc = grow_status_scratch(ctx, n, s);
-    if (rc != MMF_OK) return rc;
-    status = ctx->d_status_scratch;
-  }
+  if (int rc = status_or_scratch(ctx, &status, n)) return rc;
   // ---- per-call tables: tiles of 128 rows inside one calendar, the y buffer clipped at every calendar's t_fit
   const bool same = m.key_y == y && m.key_n == n && m.key_ld == ld_y && m.key_rows.size() == (size_t)m.n_cal + 1 &&
                     memcmp(m.key_rows.data(), cal_row_start, sizeof(int64_t) * ((size_t)m.n_cal + 1)) == 0;
@@ -2014,10 +1938,7 @@ int mmf_fit_forecast_ragged_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t
   CU_TRY(cudaMemsetAsync(counters, 0, CTR_WORDS * sizeof(uint32_t), s));
   CU_TRY(cudaMemsetAsync(m.d_pending_by_cal, 0, (size_t)m.n_cal * sizeof(uint32_t), s));
   if (may_mask) a.rec_count = counters + 1;
-  DesignView d{};
-  d.a4 = m.d_a4; d.at = m.d_at; d.apred = m.d_apred; d.w = m.d_w;
-  d.n_rows = m.cals[0].n_rows; d.n_rows_pad = m.cals[0].n_rows_pad;
-  d.t_fit = m.t_fit_max; d.t_pad = m.t_pad_max; d.kept_mask = 0xFFFFu; d.has_constant = m.has_constant;
+  const DesignView d = view_of(m);
   MultiView mv{};
   mv.cals = m.d_cals; mv.tiles = m.d_tiles; mv.tmaps_y = m.d_tmaps_y; mv.pending_by_cal = m.d_pending_by_cal;
   mv.n_cal = m.n_cal; mv.n_tiles = m.n_tiles;
@@ -2025,10 +1946,10 @@ int mmf_fit_forecast_ragged_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t
   int rc = encode_2d(tl.tmap_y, y, (uint64_t)m.cals[0].t_fit, (uint64_t)n, (uint64_t)ld_y * 4, 32, 128);   // unused by ragged tiles
   if (rc != MMF_OK) return rc;
   memcpy(tl.tmap_at, m.tmap_at, 128);
-  if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, s));
-  int launches = 0;
+  if (int rc = stats_begin(ctx, stats)) return rc;
+  Tally t{0, MMF_KERNEL_TC};
   CU_TRY(launch_fit_tc(d, a, tl, counters, ctx->sm_count, s, 0, &mv));
-  ++launches;
+  ++t.launches;
   uint32_t pend = 0;
   if (may_mask) {
     // rows the streaming pass could not finish (first 8 values missing, too many gaps): the general pass runs once
@@ -2042,21 +1963,17 @@ int mmf_fit_forecast_ragged_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t
         if (by_cal[c] == 0) continue;
         const CalMeta& cm = m.cals[c];
         const int64_t r0 = cal_row_start[c], nr = cal_row_start[c + 1] - r0;
-        DesignView dc = d;
-        dc.a4 = m.d_a4 + m.a4_off[c]; dc.apred = m.d_apred + (size_t)cm.row_off * P;
-        dc.n_rows = cm.n_rows; dc.n_rows_pad = cm.n_rows_pad; dc.t_fit = cm.t_fit; dc.t_pad = (cm.t_fit + 31) & ~31;
-        dc.kept_mask = cm.kept_mask;
         FitArgs ac = a;
         ac.y = y + r0 * ld_y; ac.n = nr; ac.out = out_pred + r0 * ld_out; ac.status = status + r0;
         ac.pred_start = cm.pred_start; ac.recs = a.recs + r0; ac.row_base = r0; ac.cal_id = c;
         if (a.out_gamma != nullptr) { ac.out_gamma = a.out_gamma + r0 * P; ac.out_c = a.out_c + r0; }
         ac.only_pending = 1; ac.pending_count = nullptr;
-        CU_TRY(launch_fit_warp(dc, ac, ctx->sm_count, s));
-        ++launches;
+        CU_TRY(launch_fit_warp(view_of(m, c), ac, ctx->sm_count, s));
+        ++t.launches;
       }
     }
     CU_TRY(launch_solve_rows(d, a, ctx->sm_count, s, m.d_cals));
-    ++launches;
+    ++t.launches;
   }
   if (m.many_pred) {
     PredictLaunch pl;
@@ -2065,17 +1982,10 @@ int mmf_fit_forecast_ragged_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t
     memcpy(pl.tmap_out, m.tmap_bhi, 128);                  // unused by the ragged kernel (per-calendar maps instead)
     pl.n_tma = 0;                                          // unused as well: each calendar's map clips its own block
     CU_TRY(launch_predict_tc(d, a, pl, ctx->sm_count, s, m.d_units, m.n_units, m.d_tmaps_out));
-    ++launches;
+    ++t.launches;
   }
   ctx->last_set = cs;
-  if (stats) {
-    CU_TRY(cudaEventRecord(ctx->ev_k1, s));
-    CU_TRY(cudaEventSynchronize(ctx->ev_k1));
-    CU_TRY(cudaEventElapsedTime(&stats->kernel_ms, ctx->ev_k0, ctx->ev_k1));
-    stats->total_ms = stats->kernel_ms;
-    stats->n_series = n; stats->n_pending = pend; stats->kernel_launches = launches; stats->kernel_used = MMF_KERNEL_TC;
-  }
-  return MMF_OK;
+  return stats_tail(ctx, stats, n, t, nullptr, 0, pend);
 }
 
 // ---- rolling-origin backtest: K origins in one pass (DESIGN.md sections 2 item 8, 4.12) -------------------------
@@ -2191,8 +2101,7 @@ int mmf_backtest_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, floa
   if (ld_y % 4 != 0 || (reinterpret_cast<uintptr_t>(y) & 15u) != 0)
     return fail(MMF_E_UNSUPPORTED, "backtests need a 16-B aligned y with ld_y %% 4 == 0 (TMA)");
   CU_TRY(cudaSetDevice(ctx->device));
-  if (!is_device_ptr(y) || (out_pred && !is_device_ptr(out_pred)) || (out_metrics && !is_device_ptr(out_metrics)) ||
-      (out_count && !is_device_ptr(out_count)) || (out_status && !is_device_ptr(out_status)))
+  if (!on_device({y}, {out_pred, out_metrics, out_count, out_status}))
     return fail(MMF_E_UNSUPPORTED, "mmf_backtest_f32 takes device buffers only");
   cudaStream_t s = ctx->stream;
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
@@ -2208,12 +2117,8 @@ int mmf_backtest_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, floa
   const int64_t n_slabs = (n + slab - 1) / slab;
   const bool may_mask = !ctx->cfg.assume_finite;
   int32_t* status = out_status;
-  if (!status) {
-    int rc = grow_status_scratch(ctx, (int64_t)K * n, s);
-    if (rc != MMF_OK) return rc;
-    status = ctx->d_status_scratch;
-  }
-  int rc = grow((void**)&ctx->d_bt_ctr, &ctx->bt_ctr_cap, 2 * MMF_BT_MAX_ORIGINS * sizeof(uint32_t));
+  int rc = status_or_scratch(ctx, &status, (int64_t)K * n);
+  if (rc == MMF_OK) rc = grow((void**)&ctx->d_bt_ctr, &ctx->bt_ctr_cap, 2 * MMF_BT_MAX_ORIGINS * sizeof(uint32_t));
   if (rc == MMF_OK && K > 1) rc = grow((void**)&ctx->d_bt_mom, &ctx->bt_mom_cap, (size_t)(K - 1) * 2 * slab * P * sizeof(float));
   if (rc == MMF_OK && may_mask) rc = grow((void**)&ctx->d_bt_recs, &ctx->bt_recs_cap, (size_t)K * slab * sizeof(SolveRec));
   if (rc == MMF_OK && may_mask) rc = grow((void**)&ctx->d_bt_rows, &ctx->bt_rows_cap, (size_t)K * slab * sizeof(int64_t));
@@ -2221,10 +2126,7 @@ int mmf_backtest_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, floa
   if (rc == MMF_OK && !out_pred) rc = grow((void**)&ctx->d_bt_pred, &ctx->bt_pred_cap, (size_t)K * slab * ld_scr * sizeof(float));
   uint32_t* slab_pending = nullptr;
   if (rc == MMF_OK && stats) {
-    const mmf_ctx* saved = g_grow_ctx;
-    g_grow_ctx = nullptr;
-    rc = grow((void**)&ctx->d_slab_pending, &ctx->slab_pending_cap, (size_t)n_slabs * sizeof(uint32_t));
-    g_grow_ctx = saved;
+    rc = grow_unpinned((void**)&ctx->d_slab_pending, &ctx->slab_pending_cap, (size_t)n_slabs * sizeof(uint32_t));
     slab_pending = ctx->d_slab_pending;
   }
   if (rc != MMF_OK) return rc;
@@ -2232,14 +2134,11 @@ int mmf_backtest_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, floa
   uint32_t* counters = ctx->d_pending + CTR_WORDS * cs;
   ctx->set_clean[cs] = false;
   const DesignView d = view_of(b.common);
-  DesignView dm{};                                         // the origins' stacked designs, as a ragged plan's
-  dm.a4 = b.cals.d_a4; dm.at = b.cals.d_at; dm.apred = b.cals.d_apred; dm.w = b.cals.d_w;
-  dm.n_rows = b.cals.cals[0].n_rows; dm.n_rows_pad = b.cals.cals[0].n_rows_pad;
-  dm.t_fit = b.cals.t_fit_max; dm.t_pad = b.cals.t_pad_max; dm.kept_mask = 0xFFFFu; dm.has_constant = b.cals.has_constant;
+  const DesignView dm = view_of(b.cals);                   // the origins' stacked designs, as a ragged plan's
   uint32_t* rec_count = ctx->d_bt_ctr;
   uint32_t* pend_by_origin = ctx->d_bt_ctr + MMF_BT_MAX_ORIGINS;
-  if (stats) CU_TRY(cudaEventRecord(ctx->ev_k0, s));
-  int launches = 0;
+  if (int rc = stats_begin(ctx, stats)) return rc;
+  Tally t{0, MMF_KERNEL_TC};
   for (int64_t off = 0, si = 0; off < n; off += slab, ++si) {
     const int64_t m = std::min(slab, n - off);
     float* obase = out_pred ? out_pred + off * ld_out : ctx->d_bt_pred;
@@ -2266,25 +2165,21 @@ int mmf_backtest_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, floa
     if (rc != MMF_OK) return rc;
     memcpy(tl.tmap_at, b.common.tmap_at, 128);
     CU_TRY(launch_fit_tc_bt(d, a, tl, counters, ctx->sm_count, s, bt));
-    ++launches;
+    ++t.launches;
     if (may_mask) {
       // per origin: the general pass for the rows the fast path left to it (exits at once when there are none), then
       // the solve of the queued records, calendar = origin
       for (int k = 0; k < K; ++k) {
         const CalMeta& cm = b.cals.cals[k];
-        DesignView dk = dm;
-        dk.a4 = b.cals.d_a4 + b.cals.a4_off[k]; dk.apred = b.cals.d_apred + (size_t)cm.row_off * P;
-        dk.n_rows = cm.n_rows; dk.n_rows_pad = cm.n_rows_pad; dk.t_fit = cm.t_fit; dk.t_pad = (cm.t_fit + 31) & ~31;
-        dk.kept_mask = cm.kept_mask;
         FitArgs ak = a;
         ak.out = obase + (int64_t)k * okstride * ldo; ak.status = status + (int64_t)k * n + off;
         ak.pred_start = cm.pred_start; ak.recs = ctx->d_bt_recs + (int64_t)k * m; ak.rec_rows = ctx->d_bt_rows + (int64_t)k * m;
         ak.rec_count = rec_count + k; ak.row_base = 0; ak.cal_id = k;
         ak.only_pending = 1; ak.pending_count = pend_by_origin + k;
-        CU_TRY(launch_fit_warp(dk, ak, ctx->sm_count, s));
+        CU_TRY(launch_fit_warp(view_of(b.cals, k), ak, ctx->sm_count, s));
         ak.pending_count = nullptr;
         CU_TRY(launch_solve_rows(dm, ak, ctx->sm_count, s, b.cals.d_cals));
-        launches += 2;
+        t.launches += 2;
       }
     }
     ScoreArgs sa{};
@@ -2293,23 +2188,13 @@ int mmf_backtest_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, floa
     sa.out_kstride = n; sa.n = m; sa.n_origin = K; sa.horizon = H;
     if (sa.metrics || sa.count) {
       CU_TRY(launch_bt_score(sa, ctx->sm_count, s));
-      ++launches;
+      ++t.launches;
     }
     if (slab_pending != nullptr)
       CU_TRY(cudaMemcpyAsync(slab_pending + si, counters, sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
   }
   ctx->last_set = cs;
-  if (stats) {
-    CU_TRY(cudaEventRecord(ctx->ev_k1, s));
-    CU_TRY(cudaEventSynchronize(ctx->ev_k1));
-    CU_TRY(cudaEventElapsedTime(&stats->kernel_ms, ctx->ev_k0, ctx->ev_k1));
-    stats->total_ms = stats->kernel_ms;
-    std::vector<uint32_t> pend((size_t)n_slabs);
-    CU_TRY(cudaMemcpy(pend.data(), slab_pending, pend.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
-    for (uint32_t v : pend) stats->n_pending += v;
-    stats->n_series = n; stats->kernel_launches = launches; stats->kernel_used = MMF_KERNEL_TC;
-  }
-  return MMF_OK;
+  return stats_tail(ctx, stats, n, t, slab_pending, (size_t)n_slabs);
 }
 
 int mmf_fit_forecast_bcast_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t pred_start,
@@ -2324,24 +2209,15 @@ int mmf_fit_forecast_bcast_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t 
   if (multimem < 0 || multimem > 2) return fail(MMF_E_INVALID, "multimem must be 0, 1 (multimem.st) or 2 (bulk stores to the multicast address)");
   if (multimem && n_out != 1) return fail(MMF_E_INVALID, "multimem=1 takes exactly one (multicast) pointer");
   if (ld_y < pl.t_fit) return fail(MMF_E_INVALID, "ld_y=%lld < t_fit=%d", (long long)ld_y, pl.t_fit);
-  if (n_pred < 1 || pred_start < 0 || (int64_t)pred_start + n_pred > pl.n_rows)
-    return fail(MMF_E_INVALID, "prediction rows [%d,%d) outside the planned design (%d rows)", pred_start,
-                pred_start + n_pred, pl.n_rows);
-  if (ld_out < n_pred) return fail(MMF_E_INVALID, "ld_out=%lld < n_pred=%d", (long long)ld_out, n_pred);
+  if (int rc = check_window(pred_start, n_pred, pl.n_rows, ld_out)) return rc;
   if (n == 0) return MMF_OK;
   CU_TRY(cudaSetDevice(ctx->device));
   if (!is_device_ptr(y)) return fail(MMF_E_INVALID, "the broadcast variant takes device buffers only");
-  int32_t* status = out_status;
-  if (!status) {
-    int rc = grow_status_scratch(ctx, n, ctx->stream);
-    if (rc != MMF_OK) return rc;
-    status = ctx->d_status_scratch;
-  }
-  float* more[MAX_OUT - 1] = {};
-  for (int i = 1; i < n_out; ++i) more[i - 1] = reinterpret_cast<float*>(out_ptrs[i]);
-  int launches = 0, kernel_used = 0;
-  return run_device(ctx, ctx->plan, y, n, ld_y, pred_start, n_pred, reinterpret_cast<float*>(out_ptrs[0]), ld_out,
-                    out_beta, status, ctx->stream, &launches, &kernel_used, more, n_out, multimem);
+  Call c = plain_call(y, ld_y, pred_start, n_pred, reinterpret_cast<float*>(out_ptrs[0]), ld_out, out_status);
+  c.beta = out_beta;
+  c.n_out = n_out; c.multimem = multimem;
+  for (int i = 1; i < n_out; ++i) c.out_more[i - 1] = reinterpret_cast<float*>(out_ptrs[i]);
+  return enqueue(ctx, pl, {{&pl, c}}, n, nullptr);
 }
 
 int mmf_fit_select_forecast_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
@@ -2367,22 +2243,16 @@ int mmf_fit_select_forecast_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t
   if (ld_out < n_pred) return fail(MMF_E_INVALID, "ld_out < n_pred");
   if (n == 0) return MMF_OK;
   CU_TRY(cudaSetDevice(ctx->device));
-  if (!is_device_ptr(y) || !is_device_ptr(out_pred)) return fail(MMF_E_INVALID, "device buffers only");
-  int32_t* status = out_status;
-  if (!status) {
-    int rc = grow_status_scratch(ctx, n, ctx->stream);
-    if (rc != MMF_OK) return rc;
-    status = ctx->d_status_scratch;
-  }
+  if (!on_device({y, out_pred}, {})) return fail(MMF_E_INVALID, "device buffers only");
   SelectArgs sel{};
   sel.n_hold = n_hold;
   sel.n_cand = n_cand;
   for (int i = 0; i < n_cand; ++i) sel.cand[i] = candidates[i];
   sel.out_choice = out_choice;
   sel.out_mse = out_mse;
-  int launches = 0, kernel_used = 0;
-  return run_device(ctx, ctx->plan, y, n, ld_y, pred_start, n_pred, out_pred, ld_out, nullptr, status, ctx->stream,
-                    &launches, &kernel_used, nullptr, 1, 0, &sel);
+  Call c = plain_call(y, ld_y, pred_start, n_pred, out_pred, ld_out, out_status);
+  c.sel = sel;
+  return enqueue(ctx, pl, {{&pl, c}}, n, nullptr);
 }
 
 // ---- device-side packer (pack.cu): every pointer is a device pointer, work is enqueued on the ctx stream

@@ -79,7 +79,7 @@ ar_kernel(const DesignView d, const FitArgs a, const ArArgs ar) {
           for (int k = 2; k <= AR_MAX; ++k)
             if (k <= p) M &= comb << (k - 1);
           uint32_t ok = (uint32_t)(M >> 32);
-          const int jmax = S - t0 - 1;                           // t0 + 1 + j <= S
+          const int jmax = S - t0 - 1 + LATE_RESTART;            // t0 + 1 + j <= S
           if (jmax < 31) ok &= (2u << jmax) - 1u;
           if (ok) s0 = t0 + 1 + (31 - __clz(ok));
         }
@@ -280,7 +280,7 @@ ar_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const ArS
           for (int k = 2; k <= AR_MAX; ++k)
             if (k <= p) M &= comb << (k - 1);
           uint32_t ok = (uint32_t)(M >> 32);
-          const int jmax = S - t0 - 1;                           // t0 + 1 + j <= S
+          const int jmax = S - t0 - 1 + LATE_RESTART;            // t0 + 1 + j <= S
           if (jmax < 31) ok &= (2u << jmax) - 1u;
           if (ok) s0 = t0 + 1 + (31 - __clz(ok));
         }

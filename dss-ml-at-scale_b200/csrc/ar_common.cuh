@@ -16,6 +16,14 @@ constexpr int NSUB = TC / 32;              // 32-row steps of a warp per staged 
 static_assert((4 * TC) % THREADS == 0, "whole float4s of the staged chunk per thread");
 constexpr int AR_MAX = MMF_AR_MAX;
 constexpr int MA_MAX = MMF_MA_MAX;
+// Rows past the latest restart of pass B that ar.cu and arima.cu allow: 0.  The negative-control build
+// (-DMMF_AR_LATE_RESTART, tests/test_gpu_arima_contract.py) allows one row past S, where the state need not be made of
+// observations, so that a prediction depends on the requested window.  Never loaded by the product.
+#ifdef MMF_AR_LATE_RESTART
+constexpr int LATE_RESTART = 1;
+#else
+constexpr int LATE_RESTART = 0;
+#endif
 
 __device__ __forceinline__ bool finite_f(float v) { return (__float_as_uint(v) & 0x7f800000u) != 0x7f800000u; }
 __device__ __forceinline__ float qnan() { return __int_as_float(0x7fc00000); }

@@ -107,7 +107,7 @@ arima_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const ArimaAr
           for (int k = 2; k <= AR_MAX; ++k)
             if (k <= pm) M &= comb << (k - 1);
           uint32_t ok = (uint32_t)(M >> 32);
-          const int jmax = S - t0 - 1;                           // t0 + 1 + j <= S
+          const int jmax = S - t0 - 1 + LATE_RESTART;            // t0 + 1 + j <= S
           if (jmax < 31) ok &= (2u << jmax) - 1u;
           if (ok) s0 = t0 + 1 + (31 - __clz(ok));
         }
@@ -351,7 +351,7 @@ arima_select_kernel(const DesignView d, const FitArgs a, const ArArgs ar, const 
         const uint32_t ok = (uint32_t)(M >> 32);
         if (t0 < S) {
           uint32_t okb = ok;
-          const int jmax = S - t0 - 1;                           // t0 + 1 + j <= S
+          const int jmax = S - t0 - 1 + LATE_RESTART;            // t0 + 1 + j <= S
           if (jmax < 31) okb &= (2u << jmax) - 1u;
           if (okb) s0 = t0 + 1 + (31 - __clz(okb));
         }

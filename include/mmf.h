@@ -208,11 +208,19 @@ int mmf_fit_forecast_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
  *   filled residuals u_s = e_s (observed) or sum_j phi_j u_{s-j} (missing, and every s >= t_fit), u_s = 0 for s < 0;
  *   out_pred[i, t - pred_start] = c + a_t.gamma + sum_j phi_j u_{t-j}: one-step-ahead in sample, the dynamic forecast
  *   from origin t_fit beyond it.  y is never read at or beyond t_fit.
+ * A row's prediction does not depend on the requested window, to the bit: the recursion may restart at the latest row
+ * s <= min(pred_start, t_fit) whose p predecessors are all observed (their u are plain residuals), and that restart
+ * changes no bit of any requested row.
  * 1 <= ar_order <= MMF_AR_MAX.  out_phi [n][MMF_AR_MAX] (zero beyond the series' order), out_order [n] and out_sigma [n]
  * (sqrt(sigma_eps^2)) are nullable; empty series (status 1) get order 0, phi 0, sigma NaN and NaN predictions.  Device
  * buffers only (host pointers: MMF_E_UNSUPPORTED); any ld_out >= n_pred and any base pointer, only columns [0, n_pred)
  * written; enqueue-only unless `stats` is non-NULL; mmf_config.kernel and assume_finite are honoured.  Refused arguments
- * write nothing.
+ * write nothing.  The kernel rule of every ARIMA-family call: each fit the call runs picks its kernel by the buffer it
+ * reads.  A fit of y itself (d = 0) needs a 16-B aligned y with ld_y % 4 == 0 for the tensor-core kernel; otherwise
+ * MMF_KERNEL_AUTO runs the warp kernel and MMF_KERNEL_TC refuses the call (MMF_E_UNSUPPORTED, "tensor-core kernel not
+ * applicable", nothing written).  A fit of z' (d >= 1) reads the context's 16-B-pitch scratch, so it runs the
+ * tensor-core kernel under AUTO and TC whatever y's layout.  A selection that lists d = 0 and d >= 1 on such a y thus
+ * mixes the kernels under AUTO, and stats->n_pending counts the rows of its tensor-core fits only.
  * replaces: SARIMAX(p, 0, 0) + exog fit and predict of the reference's per-group model (02:441-450, 472-488 with p > 0),
  * for a caller-fixed order and the two-step (OLS, then Yule-Walker on the residuals) estimator. */
 int mmf_fit_forecast_ar_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
@@ -268,7 +276,10 @@ int mmf_fit_select_ar_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y,
  * out_pred[i, t - pred_start] = yhat_t for the rows [pred_start, pred_start + n_pred) of the planned design: one step
  * ahead in sample, the integrated dynamic forecast beyond t_fit.  y is read on [0, t_fit) only.  A missing fit value
  * is replaced by its prediction, so later rows integrate from the filled level; a missing value before the first
- * observed one makes the predictions NaN until an observed level restarts the chain.
+ * observed one makes the predictions NaN until an observed level restarts the chain.  A row's prediction does not
+ * depend on the requested window, to the bit: the recursion may restart at the latest z' row s <= min(pred_start,
+ * t_fit) - d whose max(p, 1) predecessors in z' are all observed (so are the levels the integration of row s + d reads),
+ * and that restart changes no bit of any requested row.
  * out_phi [n][MMF_AR_MAX], out_order [n], out_sigma [n] are those of the AR part on z'; out_status [n] is the status of
  * the fit on z' (1 when z' has no observed fit row: NaN predictions, order 0, phi 0, sigma NaN).  All nullable except
  * out_pred.  Otherwise the contract of mmf_fit_forecast_ar_f32: device buffers only, any ld_out >= n_pred and any base

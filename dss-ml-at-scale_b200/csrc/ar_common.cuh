@@ -81,16 +81,19 @@ __device__ __forceinline__ int load_fit(const FitArgs& a, int64_t row, bool live
   return st;
 }
 
-// used columns k of the dof rule (section 2 item 7): the calendar's kept columns that are non-zero on an observed fit row
+// used columns k of the dof rule (section 2 item 7) and their mask (arma_joint.cu's J): the calendar's kept columns that are non-zero on an observed fit row
 // (colmask, per lane; a column that is zero there has a zero pivot and is skipped, as in the fit kernels), less those the
 // pivoted solve dropped for the series' mask (status 2 only; a dropped column's gamma is pinned to exactly 0)
-__device__ __forceinline__ int used_columns(const DesignView& d, uint32_t colmask, int st, const float (&g)[P]) {
+__device__ __forceinline__ uint32_t used_mask(const DesignView& d, uint32_t colmask, int st, const float (&g)[P]) {
   uint32_t used = d.kept_mask & __reduce_or_sync(0xffffffffu, colmask);
   if (st == MMF_STATUS_RANKDEF) {
 #pragma unroll
     for (int q = 0; q < P; ++q) used &= g[q] != 0.f ? ~0u : ~(1u << q);
   }
-  return __popc(used);
+  return used;
+}
+__device__ __forceinline__ int used_columns(const DesignView& d, uint32_t colmask, int st, const float (&g)[P]) {
+  return __popc(used_mask(d, colmask, st, g));
 }
 
 // out[row][0 .. N) = v, lane k writing v[k] (nothing when out is null)

@@ -549,7 +549,8 @@ struct Tally {
 // arima_kernel read z' with the plan of D_d.  (p, d) selections (asel) run one call per listed d and end in
 // arima_select_kernel; their d = 0 call (arima->d == 0) fits y itself with the mmf_plan_design plan; (p, d, q) selections
 // (hsel, with asel) add arma_select_kernel behind it.  ARMA calls (arma, with ar) run arma_kernel behind ar_kernel
-// (d = 0, no arima) or arima_kernel; CSS calls (css, with arma) add arma_css_kernel behind arma_kernel.
+// (d = 0, no arima) or arima_kernel; CSS calls (css, with arma) add arma_css_kernel behind arma_kernel, joint calls (joint,
+// with css) arma_joint_kernel in its place.
 struct Call {
   const float* y = nullptr;
   int64_t ld_y = 0;
@@ -569,6 +570,7 @@ struct Call {
   std::optional<ArmaArgs> arma;
   std::optional<ArmaSelArgs> hsel;
   std::optional<CssArgs> css;
+  std::optional<JointArgs> joint;
 
   // the same call on the rows from `off` on: every per-row output advanced by `off` rows (null stays null)
   Call slice(int64_t off) const {
@@ -609,6 +611,7 @@ struct Call {
       c.css->css_stop = at(css->css_stop, 1);
       c.css->iters = at(css->iters, 1);
     }
+    if (joint) c.joint->beta = at(joint->beta, P);
     return c;
   }
 };
@@ -739,7 +742,8 @@ int run_device_slab(mmf_ctx* ctx, const Plan& plan, const Call& c, int64_t n, Ta
       CU_TRY(launch_arma(d, a, *c.ar, mh, *c.arma, s));
       ++t.launches;
       if (c.css) {
-        CU_TRY(launch_arma_css(d, a, *c.ar, mh, *c.arma, *c.css, s));
+        CU_TRY(c.joint ? launch_arma_joint(d, a, *c.ar, mh, *c.arma, *c.css, *c.joint, s)
+                       : launch_arma_css(d, a, *c.ar, mh, *c.arma, *c.css, s));
         ++t.launches;
       }
     }
@@ -798,7 +802,7 @@ int run_device(mmf_ctx* ctx, const Plan& slab_plan, const std::vector<Stage>& st
                uint32_t* slab_pending = nullptr) {
   const cudaStream_t s = ctx->stream;
   const int64_t slab = slab_rows(slab_plan, n);
-  // CSS calls read the HR (phi, theta, ma_order) back: what the caller did not ask for goes to per-slab scratch
+  // CSS and joint calls read the HR (phi, theta, ma_order) back: what the caller did not ask for goes to per-slab scratch
   const Call& c0 = stages[0].call;
   float* hr = nullptr;
   if (c0.css && (c0.ar->phi == nullptr || c0.arma->theta == nullptr || c0.arma->ma_order == nullptr)) {
@@ -1564,14 +1568,14 @@ int mmf_fit_forecast_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t 
   return enqueue(ctx, pl, {{&pl, c}}, n, stats);
 }
 
-// ---- regression with ARIMA(p, d, q) errors (DESIGN.md section 2 items 13, 16) --------------------------------------------
-// The HR call (css == nullptr) and the CSS call: the same checks, plans and launches; the CSS call adds arma_css_kernel
-// behind arma_kernel in every slab.
+// ---- regression with ARIMA(p, d, q) errors (DESIGN.md section 2 items 13, 16, 17) ----------------------------------------
+// The HR call (css == nullptr), the CSS call and the joint call (joint != nullptr, with css): the same checks, plans and
+// launches; the CSS call adds arma_css_kernel behind arma_kernel in every slab, the joint call arma_joint_kernel.
 static int arma_call(mmf_ctx* ctx, const char* name, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
                      int32_t diff_order, int32_t ma_order, int32_t long_order, int32_t pred_start, int32_t n_pred,
                      float* out_pred, int64_t ld_out, float* out_phi, float* out_theta, int32_t* out_order,
                      int32_t* out_ma_order, float* out_sigma, int32_t* out_status, mmf_stats* stats,
-                     const CssArgs* css) {
+                     const CssArgs* css, const JointArgs* joint = nullptr) {
   if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
   GrowScope grow_scope(ctx);
   if (n < 0) return fail(MMF_E_INVALID, "n < 0");
@@ -1599,7 +1603,7 @@ static int arma_call(mmf_ctx* ctx, const char* name, const float* y, int64_t n, 
   CU_TRY(cudaSetDevice(ctx->device));
   if (!on_device({y, out_pred}, {out_phi, out_theta, out_order, out_ma_order, out_sigma, out_status,
                                  css ? css->css_start : nullptr, css ? css->css : nullptr, css ? css->css_stop : nullptr,
-                                 css ? css->iters : nullptr}))
+                                 css ? css->iters : nullptr, joint ? joint->beta : nullptr}))
     return fail(MMF_E_UNSUPPORTED, "%s takes device buffers only", name);
   Call c = plain_call(y, ld_y, pred_start, n_pred, out_pred, ld_out, out_status);
   c.ar = ar_args(ar_order, out_phi, out_order, out_sigma, pl);
@@ -1610,6 +1614,7 @@ static int arma_call(mmf_ctx* ctx, const char* name, const float* y, int64_t n, 
   c.arma = hr;
   if (diff_order > 0) c.arima = arima_args(ld_y, ap.t_fit, diff_order);
   if (css) c.css = *css;
+  if (joint) c.joint = *joint;
   return enqueue(ctx, pl, {{&pl, c}}, n, stats);
 }
 
@@ -1638,6 +1643,25 @@ int mmf_fit_forecast_arma_css_f32(mmf_ctx* ctx, const float* y, int64_t n, int64
   return arma_call(ctx, "mmf_fit_forecast_arma_css_f32", y, n, ld_y, ar_order, diff_order, ma_order, long_order,
                    pred_start, n_pred, out_pred, ld_out, out_phi, out_theta, out_order, out_ma_order, out_sigma,
                    out_status, stats, &css);
+}
+
+int mmf_fit_forecast_arma_joint_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
+                                    int32_t diff_order, int32_t ma_order, int32_t long_order, int32_t max_iter,
+                                    int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out, float* out_beta,
+                                    float* out_phi, float* out_theta, int32_t* out_order, int32_t* out_ma_order,
+                                    float* out_sigma, int32_t* out_status, float* out_css_start, float* out_css,
+                                    int32_t* out_css_stop, int32_t* out_iters, mmf_stats* stats) {
+  if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
+  if (max_iter < 0 || max_iter > MMF_CSS_ITER_MAX)
+    return fail(MMF_E_INVALID, "max_iter=%d outside [0,%d]", max_iter, MMF_CSS_ITER_MAX);
+  CssArgs css{};
+  css.max_iter = max_iter == 0 ? MMF_CSS_ITER_DEFAULT : max_iter;
+  css.css_start = out_css_start; css.css = out_css; css.css_stop = out_css_stop; css.iters = out_iters;
+  JointArgs joint{};
+  joint.beta = out_beta;
+  return arma_call(ctx, "mmf_fit_forecast_arma_joint_f32", y, n, ld_y, ar_order, diff_order, ma_order, long_order,
+                   pred_start, n_pred, out_pred, ld_out, out_phi, out_theta, out_order, out_ma_order, out_sigma,
+                   out_status, stats, &css, &joint);
 }
 
 // ---- standard errors of the ARIMA-family forecasts (DESIGN.md section 2 item 15) ---------------------------------------

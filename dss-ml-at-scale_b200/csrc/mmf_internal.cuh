@@ -309,6 +309,15 @@ struct CssArgs {
 cudaError_t launch_arma_css(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
                             const ArmaArgs& hr, const CssArgs& cs, cudaStream_t s);
 
+// ARIMA(p, d, q) errors with beta estimated jointly by conditional least squares (arma_joint.cu, DESIGN.md section 2
+// item 17): arma_joint_kernel runs where arma_css_kernel runs for the CSS call, with the same CssArgs, and adds the
+// whitened coefficients of the series' used columns to the parameter vector
+struct JointArgs {
+  float* beta;                            // nullable [n][P]: W gamma (+ c on the intercept) of the shipped gamma
+};
+cudaError_t launch_arma_joint(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
+                              const ArmaArgs& hr, const CssArgs& cs, const JointArgs& jt, cudaStream_t s);
+
 // per-series (p, d, q) selection by hold-out MSE on levels (arma_select.cu, DESIGN.md section 2 item 14): one launch per
 // listed d, right behind that d's arima_select_kernel (same fit, z', gamma / c and running best), for the q >= 1 blocks.
 // Candidate lane c is the pair (pq_p[c], pq_q[c]), q-major; its normal equations are those of row set pq_rs[c], the rows

@@ -578,7 +578,7 @@ class ForecastEngine:
 
     def fit_forecast_arma(self, y, ar_order: int, ma_order: int, diff_order: int = 0, pred_start: int = 0,
                           n_pred: int | None = None, long_order: int = 0, want_stats: bool = False,
-                          want_se: bool = False, estimator: str = "hr", max_iter: int = 0):
+                          want_se: bool = False, estimator: str = "hr", max_iter: int = 0, joint_beta: bool = False):
         """Regression with ARIMA(``ar_order``, ``diff_order``, ``ma_order``) errors (``mmf_fit_forecast_arma_f32``,
         DESIGN.md section 2 item 13): the plain fit (on the differenced series and design for ``diff_order`` >= 1),
         then Hannan-Rissanen on its residuals -- a long AR of order ``long_order`` (0: the default) gives innovation
@@ -595,13 +595,23 @@ class ForecastEngine:
         from the Hannan-Rissanen estimate, for at most ``max_iter`` passes (0: 20, at most 64).  A series that accepts no
         step keeps the HR outputs bit for bit; ``sigma`` is sqrt(S / |C|) for every gated series.  The result adds
         ``css_start`` (S at the HR estimate), ``css`` (S shipped), ``css_stop`` (1 converged, 2 stalled, 3 budget, 0 not
-        refined) and ``iters`` (passes run)."""
+        refined) and ``iters`` (passes run).
+
+        ``joint_beta=True`` with ``estimator="css"`` (``mmf_fit_forecast_arma_joint_f32``, DESIGN.md section 2 item 17)
+        estimates the regression coefficients jointly with (phi, theta): the whitened coefficients of every gated series'
+        used design columns join the Levenberg-Marquardt parameter vector, started from the plain fit's (regression with
+        ARIMA errors, R's ``arima(xreg=, method="CSS")``).  The result adds ``beta`` [n, 16], the coefficients of the raw
+        design columns the series ships (of the differenced design for ``diff_order`` >= 1; NaN for empty series).  With
+        ``want_se=True`` the standard errors take the joint (phi, theta, sigma); beta's estimation uncertainty is not
+        included."""
         import torch
         if estimator not in ("hr", "css"):
             raise ValueError(f"estimator must be 'hr' or 'css', got {estimator!r}")
         css = estimator == "css"
         if not css and int(max_iter) != 0:
             raise ValueError("max_iter= is the pass budget of estimator='css'")
+        if joint_beta and not css:
+            raise ValueError("joint_beta=True needs estimator='css' (beta joins the conditional least-squares fit)")
         if int(diff_order) >= 1:
             if getattr(self, "_arima", None) is None:
                 raise RuntimeError("plan_arima() (or plan_calendar(..., max_diff=d)) must be called first")
@@ -630,11 +640,21 @@ class ForecastEngine:
             css_end = torch.empty(n, device=dev, dtype=torch.float32)
             css_stop = torch.empty(n, device=dev, dtype=torch.int32)
             iters = torch.empty(n, device=dev, dtype=torch.int32)
-            N.check(self._lib.mmf_fit_forecast_arma_css_f32(
-                self._h, yp, n, ld_y, int(ar_order), int(diff_order), int(ma_order), int(long_order), int(max_iter),
-                int(pred_start), int(n_pred), out.data_ptr(), out.stride(0), phi.data_ptr(), theta.data_ptr(),
-                order.data_ptr(), ma.data_ptr(), sigma.data_ptr(), status.data_ptr(), css_start.data_ptr(),
-                css_end.data_ptr(), css_stop.data_ptr(), iters.data_ptr(), C.byref(st) if st is not None else None))
+            if joint_beta:
+                beta = torch.empty((n, N.MMF_P), device=dev, dtype=torch.float32)
+                N.check(self._lib.mmf_fit_forecast_arma_joint_f32(
+                    self._h, yp, n, ld_y, int(ar_order), int(diff_order), int(ma_order), int(long_order),
+                    int(max_iter), int(pred_start), int(n_pred), out.data_ptr(), out.stride(0), beta.data_ptr(),
+                    phi.data_ptr(), theta.data_ptr(), order.data_ptr(), ma.data_ptr(), sigma.data_ptr(),
+                    status.data_ptr(), css_start.data_ptr(), css_end.data_ptr(), css_stop.data_ptr(), iters.data_ptr(),
+                    C.byref(st) if st is not None else None))
+            else:
+                N.check(self._lib.mmf_fit_forecast_arma_css_f32(
+                    self._h, yp, n, ld_y, int(ar_order), int(diff_order), int(ma_order), int(long_order),
+                    int(max_iter), int(pred_start), int(n_pred), out.data_ptr(), out.stride(0), phi.data_ptr(),
+                    theta.data_ptr(), order.data_ptr(), ma.data_ptr(), sigma.data_ptr(), status.data_ptr(),
+                    css_start.data_ptr(), css_end.data_ptr(), css_stop.data_ptr(), iters.data_ptr(),
+                    C.byref(st) if st is not None else None))
         else:
             N.check(self._lib.mmf_fit_forecast_arma_f32(self._h, yp, n, ld_y, int(ar_order), int(diff_order),
                                                         int(ma_order), int(long_order), int(pred_start), int(n_pred),
@@ -645,6 +665,8 @@ class ForecastEngine:
                "status": status}
         if css:
             res.update(css_start=css_start, css=css_end, css_stop=css_stop, iters=iters)
+            if joint_beta:
+                res["beta"] = beta
         if want_se:
             self._add_se(res, y, t_fit, pred_start, n_pred, int(diff_order))
         if st is not None:

@@ -339,7 +339,7 @@ def _host(x):
 
 
 def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, interval=False, ar=None, diff=None,
-                 ma=None, want_se=False, estimator=None):
+                 ma=None, want_se=False, estimator=None, joint_beta=False):
     """Run the engine over every bucket: yields (bucket, out_days, n_pred, y_host, pred_host, se_host or None).
     ``interval``: prediction standard errors too (``fit_forecast_se``), one call per calendar bucket.
     ``ar``: regression with AR(ar) errors (``fit_forecast_ar``), one call per calendar bucket; a tuple of orders
@@ -351,7 +351,8 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
     tuple of MA orders (with ``ar`` and ``diff`` tuples) chooses (p, d, q) per series by hold-out MSE over the last
     ``horizon`` rows (``fit_select_arma``).
     ``want_se``: the ARIMA-family call's forecast standard errors too (``want_se=True``, DESIGN.md section 2 item 15).
-    ``estimator``: the fixed-order ARIMA(p, d, q) call's estimator (None: the engine's default, Hannan-Rissanen)."""
+    ``estimator``: the fixed-order ARIMA(p, d, q) call's estimator (None: the engine's default, Hannan-Rissanen);
+    ``joint_beta``: with ``estimator="css"``, beta estimated jointly with (phi, theta)."""
     se_kw = {"want_se": True} if want_se else {}
     if interval and select is not None:
         raise ValueError("interval= is not offered with select= (model selection returns point forecasts)")
@@ -376,6 +377,8 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
             from .engine import device_packed
             yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
             est_kw = {"estimator": estimator} if estimator is not None else {}
+            if joint_beta:
+                est_kw["joint_beta"] = True
             res = eng.fit_forecast_arma(yd, ar, ma, diff or 0, pred_start, n_pred, **se_kw, **est_kw)
             pred, se = _host(res["pred"]), (_host(res["se"]) if want_se else None)
         elif isinstance(diff, tuple):
@@ -550,6 +553,16 @@ def _estimator(estimator, ma, select, interval):
     return estimator
 
 
+def _joint_beta(joint_beta, estimator):
+    """validated ``joint_beta=``: True needs ``estimator="css"`` (DESIGN.md section 2 item 17)"""
+    if not joint_beta:
+        return False
+    if estimator != "css":
+        raise ValueError(f"joint_beta=True needs estimator='css' (beta joins the conditional least-squares fit), "
+                         f"got estimator={estimator!r}")
+    return True
+
+
 def _ar_orders_for(diff, ar, select, interval, mode):
     """``ar=`` validated against ``diff=``: one order in 0..8 for a single d, the tuple of candidate orders for a tuple
     of d's, and _ar_order's result without differencing"""
@@ -667,7 +680,7 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
                     freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                     engine: ForecastEngine | None = None, pack: str = "host", select=None,
                     null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None, ma=None,
-                    conf_int=None, estimator=None) -> pd.DataFrame:
+                    conf_int=None, estimator=None, joint_beta=False) -> pd.DataFrame:
     """Fit + forecast every group in ``pdf``; returns ``tuning_schema`` rows
     (keys..., Date, Demand, Demand_Fitted), groups in key order, dates ascending.
 
@@ -734,6 +747,10 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     least squares (``ForecastEngine.fit_forecast_arma(..., estimator="css")``, DESIGN.md section 2 item 16); schema
     unchanged, ``conf_int=`` works as above.  ``estimator=None`` (or ``"hr"``) leaves everything as it was.  Refused
     without ``ma=``, with candidate MA orders, ``select=`` or ``interval=``.
+    ``joint_beta=True`` with ``estimator="css"`` estimates the design's coefficients jointly with (phi, theta)
+    (``ForecastEngine.fit_forecast_arma(..., joint_beta=True)``, DESIGN.md section 2 item 17: regression with ARIMA errors
+    as SARIMAX fits it, by the conditional likelihood); schema unchanged, ``conf_int=`` works as above.  Refused without
+    ``estimator="css"``.
     """
     eng = engine or default_engine()
     keys = list(keys)
@@ -741,6 +758,7 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     z = _z_of(interval)
     cz = _conf_z(conf_int, ar, select, interval)
     est = _estimator(estimator, ma, select, interval)
+    jb = _joint_beta(joint_beta, est)
     if ma is None:
         diff = _diff_order(diff, ar, select, interval, mode)
         ar = _ar_orders_for(diff, ar, select, interval, mode)
@@ -755,7 +773,7 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     parts, lengths = [], []
     for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
                                                               pack == "device", z is not None, ar, diff, ma,
-                                                              cz is not None, est):
+                                                              cz is not None, est, jb):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n), n_pred)
         # key columns keep the dtype they came in with (no per-row string inference on N x T values)
@@ -847,7 +865,7 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
                    freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                    engine: ForecastEngine | None = None, pack: str = "host", select=None,
                    null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None, ma=None,
-                   conf_int=None, estimator=None):
+                   conf_int=None, estimator=None, joint_beta=False):
     """Arrow ``Table``/``RecordBatch`` in -> Arrow ``Table`` with ``tuning_schema`` out (the ``mapInArrow``
     flavour of the boundary).  No pandas frame of the rows on either side: keys are dictionary-encoded on the way
     in and expanded from a dictionary on the way out, dates and values are NumPy views of Arrow buffers.
@@ -855,7 +873,8 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     ``tuning_schema(..., interval=True)``).  ``ar=p`` fits regression with AR(p) errors and ``ar=(0, 1, 2, 3, 4)`` chooses the order per series, as in
     ``forecast_groups``; ``diff=d`` with ``ar=p`` fits ARIMA(p, d, 0) errors as there, and ``ma=q`` ARIMA(p, d, q); tuples of ``ar``, ``diff`` and
     ``ma`` choose (p, d, q) per series.  ``conf_int=level`` adds the same two columns for those forecasts, and
-    ``estimator="css"`` refines a fixed ``ma=q``'s estimate, as in ``forecast_groups``."""
+    ``estimator="css"`` refines a fixed ``ma=q``'s estimate and ``joint_beta=True`` adds beta to it, as in
+    ``forecast_groups``."""
     import pyarrow as pa
 
     if isinstance(table, pa.RecordBatch):
@@ -865,6 +884,7 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     z = _z_of(interval)
     cz = _conf_z(conf_int, ar, select, interval)
     est = _estimator(estimator, ma, select, interval)
+    jb = _joint_beta(joint_beta, est)
     if ma is None:
         diff = _diff_order(diff, ar, select, interval, mode)
         ar = _ar_orders_for(diff, ar, select, interval, mode)
@@ -876,7 +896,7 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     parts, lengths = [], []
     for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
                                                               pack == "device", z is not None, ar, diff, ma,
-                                                              cz is not None, est):
+                                                              cz is not None, est, jb):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n, dtype=np.int32), n_pred)
         cols = []

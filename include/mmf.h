@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define MMF_VERSION 112          /* 0.1.12 */
+#define MMF_VERSION 113          /* 0.1.13 */
 #define MMF_P 16                 /* design columns (zero-pad narrower designs) */
 #define MMF_PIVOT_TOL 1e-3f      /* per-series relative Cholesky pivot threshold */
 #define MMF_CAL_TOL 1e-10        /* aliasing threshold on the float64 calendar Gram */
@@ -367,6 +367,32 @@ int mmf_fit_forecast_arma_css_f32(mmf_ctx* ctx, const float* y, int64_t n, int64
                                   float* out_theta, int32_t* out_order, int32_t* out_ma_order, float* out_sigma,
                                   int32_t* out_status, float* out_css_start, float* out_css, int32_t* out_css_stop,
                                   int32_t* out_iters, mmf_stats* stats);
+
+/* ---- ARIMA(p, d, q) errors with beta estimated jointly (DESIGN.md section 2 item 17) ---------------------------------
+ * mmf_fit_forecast_arma_joint_f32: mmf_fit_forecast_arma_css_f32 with the regression coefficients added to the
+ * parameter vector (R's arima(xreg =, method = "CSS")): x = (phi_1..phi_p, theta_1..theta_q, gamma_j for j in J), J the
+ * series' used columns of the dof rule (kept by the plan, non-zero on an observed fit row, not dropped for the series'
+ * mask), gamma the whitened coefficients of the plan the call fits (mmf_plan_design's for d = 0, D_d's for d >= 1), c
+ * (the fit's centring constant, 0 for d >= 1) held fixed.  The residual of a pass is e_s = z'_s - (c + a_s . gamma) in
+ * fp32 at the pass's gamma; S, the gap rule, the exact Jacobian (the gamma columns through the same recursion: d u~_s =
+ * -a_{s,j} and d eps~_s = -a_{s,j} - d pr_s on an observed row, d u~_s = d pr_s and d eps~_s = 0 on a missing one), the
+ * step, its constants and the stops are the CSS call's, on the (n_x + 1)-square system, n_x = p + q + |J| <= 28; the
+ * step-down tests apply to (phi, theta) only.  Start: x0 = (the HR (phi, theta), the fit's gamma on J), so out_css_start
+ * is the CSS call's bit for bit.
+ * Outputs: as mmf_fit_forecast_arma_css_f32's, a series that accepted a step getting the recursion at the shipped
+ * (gamma, phi, theta): c + a_s . gamma + pr_s, integrated to levels for d >= 1.  out_beta [n][MMF_P] (nullable) = W gamma
+ * (+ c on the intercept when the plan has a constant) of the gamma each series ships, in the fp32 order of
+ * mmf_fit_forecast_f32's out_beta (so a d = 0 series that kept the fit's gamma gets its out_beta bit for bit); for d >= 1
+ * the coefficients of Delta^d X.  NaN for empty series.  With J empty every output is mmf_fit_forecast_arma_css_f32's bit
+ * for bit.  Otherwise the contract of mmf_fit_forecast_arma_css_f32 (plans, refusals, device buffers only, scratch).
+ * replaces: SARIMAX(p, d, q) + exog fit with the exog coefficients estimated jointly (02:441-450, 472-481), by the
+ * conditional likelihood. */
+int mmf_fit_forecast_arma_joint_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
+                                    int32_t diff_order, int32_t ma_order, int32_t long_order, int32_t max_iter,
+                                    int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out, float* out_beta,
+                                    float* out_phi, float* out_theta, int32_t* out_order, int32_t* out_ma_order,
+                                    float* out_sigma, int32_t* out_status, float* out_css_start, float* out_css,
+                                    int32_t* out_css_stop, int32_t* out_iters, mmf_stats* stats);
 
 /* ---- (p, d) selection by hold-out MSE on levels (DESIGN.md section 2 item 12) -----------------------------------------
  * mmf_fit_select_arima_f32: orders [n_orders] (1 .. MMF_ARSEL_MAX_CAND ascending distinct values in [0, MMF_AR_MAX]) and

@@ -3,9 +3,11 @@ Hannan-Rissanen call it refines, on scripts/bench_arma.py's shapes (C4 future an
 holdout), gap-free and with 1e-3 of the values missing, for ARMA(1, 0, 1), ARIMA(1, 1, 1) and ARIMA(1, 2, 1).  Each arm
 alternates the HR call with the CSS call over several rounds after a warm-up, timed with CUDA events; prints ms per call
 (median), ms per pass (the CSS call's extra time over the mean pass count), the distribution of passes and stop codes,
-the share of rows refined, in holdout mode the hold-out MSE of both, and the card's name and power limit.
+the share of rows refined, in holdout mode the hold-out MSE of both, and the card's name and power limit.  ``--joint`` adds
+the joint call (mmf_fit_forecast_arma_joint_f32, beta estimated with (phi, theta)) to the alternation, with its ms per
+call and per pass, passes, stops, share refined and hold-out MSE.
 
-    python scripts/bench_arma_css.py [--series 1000000] [--steps 3] [--rounds 3] [--shapes ...] [--out FILE]
+    python scripts/bench_arma_css.py [--series 1000000] [--steps 3] [--rounds 3] [--shapes ...] [--joint] [--out FILE]
 """
 import argparse
 import json
@@ -41,6 +43,7 @@ def main():
     ap.add_argument("--shapes", default="C4_future,C4_holdout,weekly157")
     ap.add_argument("--gaps", default="0,0.001")
     ap.add_argument("--orders", default=",".join(ORDERS))
+    ap.add_argument("--joint", action="store_true")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     name, limit = card()
@@ -61,13 +64,20 @@ def main():
                 p, d, q = ORDERS[oname]
                 hr_call = lambda: eng.fit_forecast_arma(yf, p, q, d, ps, npred)          # noqa: E731
                 css_call = lambda: eng.fit_forecast_arma(yf, p, q, d, ps, npred, estimator="css")  # noqa: E731
+                joint_call = lambda: eng.fit_forecast_arma(yf, p, q, d, ps, npred, estimator="css",  # noqa: E731
+                                                           joint_beta=True)
                 hr_call(), css_call()
-                t_hr, t_css = [], []
+                if args.joint:
+                    joint_call()
+                t_hr, t_css, t_joint = [], [], []
                 for _ in range(args.rounds):
                     ms, hr = timed(hr_call, args.steps)
                     t_hr.append(ms)
                     ms, cs = timed(css_call, args.steps)
                     t_css.append(ms)
+                    if args.joint:
+                        ms, jt = timed(joint_call, args.steps)
+                        t_joint.append(ms)
                 g = (cs["css_stop"] > 0).cpu().numpy()
                 it = cs["iters"].cpu().numpy()[g]
                 stop = cs["css_stop"].cpu().numpy()[g]
@@ -78,9 +88,20 @@ def main():
                            iters_pct=[float(v) for v in np.percentile(it, [50, 90, 100])] if it.size else [],
                            stops=np.bincount(stop, minlength=4)[1:].tolist())
                 rec["ms_per_pass"] = (rec["css_ms"] - rec["hr_ms"]) / max(rec["iters_mean"], 1.0)
+                arms = (("hr", hr), ("css", cs))
+                if args.joint:
+                    itj = jt["iters"].cpu().numpy()[g]
+                    rec.update(joint_ms=float(np.median(t_joint)),
+                               joint_refined=float(((jt["phi"] != hr["phi"]).any(1) | (jt["theta"] != hr["theta"]).any(1)
+                                                    | ((jt["pred"] != hr["pred"]) & ~(jt["pred"].isnan() & hr["pred"].isnan()))
+                                                    .any(1)).float().mean()),
+                               joint_iters_mean=float(itj.mean()) if itj.size else 0.0,
+                               joint_stops=np.bincount(jt["css_stop"].cpu().numpy()[g], minlength=4)[1:].tolist())
+                    rec["joint_ms_per_pass"] = (rec["joint_ms"] - rec["hr_ms"]) / max(rec["joint_iters_mean"], 1.0)
+                    arms += (("joint", jt),)
                 if mode == "holdout":
                     yh = yg[:, t_fit:t].float()
-                    for k, r in (("hr", hr), ("css", cs)):
+                    for k, r in arms:
                         e = (r["pred"][:, t_fit:t] - yh)
                         ok = torch.isfinite(e)
                         rec[f"mse_{k}"] = float((torch.where(ok, e, 0.0) ** 2).sum() / ok.sum())

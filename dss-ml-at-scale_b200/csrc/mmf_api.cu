@@ -223,6 +223,8 @@ struct mmf_ctx {
   float* d_hsel_q0 = nullptr;  size_t hsel_q0_cap = 0;     // (p, d, q) selection, per slab: the q = 0 scores
   float* d_css_hr = nullptr;  size_t css_hr_cap = 0;       // CSS calls, per slab: the HR phi / theta / ma_order the
                                                            // caller did not ask for
+  int32_t* d_refit = nullptr;  size_t refit_cap = 0;       // selection refits, per slab: the winner's outputs the caller
+                                                           // did not ask for, the row list and its length
   float* d_bt_mom = nullptr;  size_t bt_mom_cap = 0;   // backtest scratch, per slab: moments at the earlier origins,
   SolveRec* d_bt_recs = nullptr;  size_t bt_recs_cap = 0;   // [K][slab] records, [K][slab] work lists,
   int64_t* d_bt_rows = nullptr;  size_t bt_rows_cap = 0;
@@ -550,7 +552,8 @@ struct Tally {
 // arima_select_kernel; their d = 0 call (arima->d == 0) fits y itself with the mmf_plan_design plan; (p, d, q) selections
 // (hsel, with asel) add arma_select_kernel behind it.  ARMA calls (arma, with ar) run arma_kernel behind ar_kernel
 // (d = 0, no arima) or arima_kernel; CSS calls (css, with arma) add arma_css_kernel behind arma_kernel, joint calls (joint,
-// with css) arma_joint_kernel in its place.
+// with css) arma_joint_kernel in its place.  Refit stages of a (p, d, q) selection (refit, with ar, arima, arma and css)
+// run the fit of their d, refit_list_kernel and arma_css_list_kernel (joint: arma_joint_list_kernel).
 struct Call {
   const float* y = nullptr;
   int64_t ld_y = 0;
@@ -571,6 +574,7 @@ struct Call {
   std::optional<ArmaSelArgs> hsel;
   std::optional<CssArgs> css;
   std::optional<JointArgs> joint;
+  std::optional<RefitArgs> refit;
 
   // the same call on the rows from `off` on: every per-row output advanced by `off` rows (null stays null)
   Call slice(int64_t off) const {
@@ -579,7 +583,7 @@ struct Call {
     c.y = y + off * ld_y;
     c.out = out + off * ld_out;
     c.beta = at(beta, P);
-    if (!asel) c.status = status + off;     // a selection's fits write the per-slab scratch; asel->status is the caller's
+    if (!asel && !refit) c.status = status + off;   // selection and refit fits write the per-slab scratch
     for (int i = 0; i + 1 < n_out && i < MAX_OUT - 1; ++i) c.out_more[i] = out_more[i] + off * ld_out;
     if (sel) { c.sel->out_choice = at(sel->out_choice, 1); c.sel->out_mse = at(sel->out_mse, 1); }
     if (se) { c.se->out_se = at(se->out_se, se->ld_se); c.se->sigma = at(se->sigma, 1); c.se->dof = at(se->dof, 1); }
@@ -612,6 +616,7 @@ struct Call {
       c.css->iters = at(css->iters, 1);
     }
     if (joint) c.joint->beta = at(joint->beta, P);
+    if (refit) { c.refit->choice_d = at(refit->choice_d, 1); c.refit->choice_q = at(refit->choice_q, 1); }
     return c;
   }
 };
@@ -727,7 +732,16 @@ int run_device_slab(mmf_ctx* ctx, const Plan& plan, const Call& c, int64_t n, Ta
     CU_TRY(launch_select(d, a, *c.sel, ctx->sm_count, s));
     ++t.launches;
   }
-  if (c.ar) {
+  if (c.refit) {
+    // the winners of this d: refit_list_kernel lists them (and writes the refit outputs of the rows the list leaves
+    // out), then the list kernel refits them from the winner's outputs.  ma is this d's (ma.y = a.y for d = 0)
+    CU_TRY(cudaMemsetAsync(c.refit->count, 0, sizeof(uint32_t), s));
+    const JointArgs jt = c.joint ? *c.joint : JointArgs{};
+    CU_TRY(launch_refit_list(d, a, ma, *c.css, jt, *c.refit, s));
+    CU_TRY(c.joint ? launch_arma_joint_list(d, a, *c.ar, ma, *c.arma, *c.css, jt, *c.refit, s)
+                   : launch_arma_css_list(d, a, *c.ar, ma, *c.arma, *c.css, *c.refit, s));
+    t.launches += 2;
+  } else if (c.ar) {
     CU_TRY(c.asel    ? launch_arima_select(d, a, *c.ar, ma, *c.asel, s)
            : c.arima ? launch_arima(d, a, *c.ar, ma, s)
            : c.arsel ? launch_ar_select(d, a, *c.ar, *c.arsel, s) : launch_ar(d, a, *c.ar, s));
@@ -811,6 +825,15 @@ int run_device(mmf_ctx* ctx, const Plan& slab_plan, const std::vector<Stage>& st
     if (rc != MMF_OK) return rc;
     hr = ctx->d_css_hr;
   }
+  // selections with refit stages: the refit reads the winner back (phi, theta, order, ma_order, choice_d, choice_q), so
+  // what the caller did not ask for goes to per-slab scratch in every stage; the row list and its length live there too
+  int32_t* rs = nullptr;
+  if (stages.back().call.refit) {
+    const size_t words = (size_t)slab * (MMF_AR_MAX + MMF_MA_MAX + 5) + 1;
+    int rc = grow((void**)&ctx->d_refit, &ctx->refit_cap, words * sizeof(int32_t));
+    if (rc != MMF_OK) return rc;
+    rs = ctx->d_refit;
+  }
   for (int64_t off = 0, i = 0; off < n; off += slab, ++i) {
     const int64_t m = std::min(slab, n - off);
     for (size_t k = 0; k < stages.size(); ++k) {
@@ -819,6 +842,33 @@ int run_device(mmf_ctx* ctx, const Plan& slab_plan, const std::vector<Stage>& st
         if (!c.ar->phi) c.ar->phi = hr;
         if (!c.arma->theta) c.arma->theta = hr + (size_t)slab * MMF_AR_MAX;
         if (!c.arma->ma_order) c.arma->ma_order = reinterpret_cast<int32_t*>(hr + (size_t)slab * (MMF_AR_MAX + MMF_MA_MAX));
+      }
+      if (rs != nullptr) {
+        auto or_scratch = [](auto*& p, int32_t* w) { if (!p) p = reinterpret_cast<decltype(p + 0)>(w); };
+        int32_t* w = rs;
+        int32_t* phi = w;       w += (size_t)slab * MMF_AR_MAX;
+        int32_t* theta = w;     w += (size_t)slab * MMF_MA_MAX;
+        int32_t* order = w;     w += slab;
+        int32_t* ma_order = w;  w += slab;
+        int32_t* choice_d = w;  w += slab;
+        int32_t* choice_q = w;  w += slab;
+        int32_t* rows = w;      w += slab;
+        or_scratch(c.ar->phi, phi);
+        or_scratch(c.ar->order, order);
+        if (c.hsel) {
+          or_scratch(c.hsel->theta, theta);
+          or_scratch(c.hsel->ma_order, ma_order);
+          or_scratch(c.hsel->choice_q, choice_q);
+          or_scratch(c.asel->choice_d, choice_d);
+        }
+        if (c.refit) {
+          or_scratch(c.arma->theta, theta);
+          or_scratch(c.arma->ma_order, ma_order);
+          or_scratch(c.refit->choice_d, choice_d);
+          or_scratch(c.refit->choice_q, choice_q);
+          c.refit->rows = rows;
+          c.refit->count = reinterpret_cast<uint32_t*>(w);
+        }
       }
       const int rc = run_device_slab(ctx, *stages[k].plan, c, m, t);
       if (rc != MMF_OK) return rc;
@@ -1050,6 +1100,7 @@ int mmf_destroy(mmf_ctx* ctx) {
   free_arima(ctx->arima);
   cudaFree(ctx->d_z);
   cudaFree(ctx->d_asel_best); cudaFree(ctx->d_asel_status); cudaFree(ctx->d_hsel_q0); cudaFree(ctx->d_css_hr);
+  cudaFree(ctx->d_refit);
   cudaFree(ctx->d_bt_mom); cudaFree(ctx->d_bt_recs); cudaFree(ctx->d_bt_rows); cudaFree(ctx->d_bt_ctr); cudaFree(ctx->d_bt_pred);
   for (int i = 0; i < NBUF; ++i) {
     Staging& s = ctx->st[i];
@@ -1698,16 +1749,18 @@ int mmf_arima_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int3
   return stats_tail(ctx, stats, n, Tally{1, MMF_KERNEL_WARP});
 }
 
-// ---- (p, d) and (p, d, q) selection by hold-out MSE on levels (DESIGN.md section 2 items 12, 14) ------------------------
+// ---- (p, d) and (p, d, q) selection by hold-out MSE on levels (DESIGN.md section 2 items 12, 14, 18) --------------------
 // The MA arguments (mas .. out_ma_order) are those of mmf_fit_select_arma_f32 (with_q); mmf_fit_select_arima_f32 passes
-// none and launches no arma_select_kernel.
+// none and launches no arma_select_kernel.  The refit calls (css, with_q; joint with css) add one refit stage per listed
+// d behind the selection's stages.
 static int select_arima_call(mmf_ctx* ctx, const char* name, bool with_q, const float* y, int64_t n, int64_t ld_y,
                              int32_t n_hold, const int32_t* orders, int32_t n_orders, const int32_t* diffs,
                              int32_t n_diffs, const int32_t* mas, int32_t n_mas, int32_t long_order, int32_t pred_start,
                              int32_t n_pred, float* out_pred, int64_t ld_out, int32_t* out_choice_p,
                              int32_t* out_choice_d, int32_t* out_choice_q, float* out_mse, float* out_cand_mse,
                              float* out_phi, float* out_theta, int32_t* out_order, int32_t* out_ma_order,
-                             float* out_sigma, int32_t* out_status, mmf_stats* stats) {
+                             float* out_sigma, int32_t* out_status, mmf_stats* stats, const CssArgs* css = nullptr,
+                             const JointArgs* joint = nullptr) {
   if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
   GrowScope grow_scope(ctx);
   if (n < 0) return fail(MMF_E_INVALID, "n < 0");
@@ -1755,7 +1808,9 @@ static int select_arima_call(mmf_ctx* ctx, const char* name, bool with_q, const 
   if (n == 0) return MMF_OK;
   CU_TRY(cudaSetDevice(ctx->device));
   if (!on_device({y, out_pred}, {out_choice_p, out_choice_d, out_mse, out_cand_mse, out_phi, out_order, out_sigma,
-                                 out_status, out_choice_q, out_theta, out_ma_order}))
+                                 out_status, out_choice_q, out_theta, out_ma_order, css ? css->css_start : nullptr,
+                                 css ? css->css : nullptr, css ? css->css_stop : nullptr, css ? css->iters : nullptr,
+                                 joint ? joint->beta : nullptr}))
     return fail(MMF_E_UNSUPPORTED, "%s takes device buffers only", name);
 
   // (p, d, q) selection: the (p, q >= 1) pairs q-major, and their row sets R(q, L = max(p, q)) in order of appearance
@@ -1814,6 +1869,27 @@ static int select_arima_call(mmf_ctx* ctx, const char* name, bool with_q, const 
     c.asel = sel;
     stages.push_back({&plan, c});
   }
+  // the refit of the winners: per listed d, that d's fit again (the selection's z', gamma / c and status scratch hold the
+  // last d's by then; the status goes to scratch), then the list of the winners with this d and q >= 1 and their refit
+  // at the winner's (p, q) with long order m_d.  ar.p / hr.q: the largest listed orders (read by no product kernel)
+  for (int k = 0; css && k < n_diffs; ++k) {
+    const int dd = diffs[k];
+    const Plan& plan = dd == 0 ? pl : ap.diff[dd - 1];
+    Call c = plain_call(y, ld_y, pred_start, n_pred, out_pred, ld_out, ctx->d_asel_status);
+    c.ar = ar_args(orders[n_orders - 1], out_phi, out_order, out_sigma, plan);
+    c.arima = arima_args(ld_y, T, dd);
+    ArmaArgs hr{};
+    hr.q = mas[n_mas - 1];
+    hr.m = long_order != 0 ? long_order : hr_long_order(std::max(orders[n_orders - 1], mas[n_mas - 1]), T - dd);
+    hr.theta = out_theta; hr.ma_order = out_ma_order;
+    c.arma = hr;
+    c.css = *css;
+    if (joint) c.joint = *joint;
+    RefitArgs rf{};
+    rf.choice_d = out_choice_d; rf.choice_q = out_choice_q; rf.first = k == 0;
+    c.refit = rf;
+    stages.push_back({&plan, c});
+  }
   return enqueue(ctx, level_plan, std::move(stages), n, stats);
 }
 
@@ -1839,6 +1915,48 @@ int mmf_fit_select_arma_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
                            n_mas, long_order, pred_start, n_pred, out_pred, ld_out, out_choice_p, out_choice_d,
                            out_choice_q, out_mse, out_cand_mse, out_phi, out_theta, out_order, out_ma_order, out_sigma,
                            out_status, stats);
+}
+
+int mmf_fit_select_arma_css_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
+                                const int32_t* orders, int32_t n_orders, const int32_t* diffs, int32_t n_diffs,
+                                const int32_t* mas, int32_t n_mas, int32_t long_order, int32_t max_iter,
+                                int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out,
+                                int32_t* out_choice_p, int32_t* out_choice_d, int32_t* out_choice_q, float* out_mse,
+                                float* out_cand_mse, float* out_phi, float* out_theta, int32_t* out_order,
+                                int32_t* out_ma_order, float* out_sigma, int32_t* out_status, float* out_css_start,
+                                float* out_css, int32_t* out_css_stop, int32_t* out_iters, mmf_stats* stats) {
+  if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
+  if (max_iter < 0 || max_iter > MMF_CSS_ITER_MAX)
+    return fail(MMF_E_INVALID, "max_iter=%d outside [0,%d]", max_iter, MMF_CSS_ITER_MAX);
+  CssArgs css{};
+  css.max_iter = max_iter == 0 ? MMF_CSS_ITER_DEFAULT : max_iter;
+  css.css_start = out_css_start; css.css = out_css; css.css_stop = out_css_stop; css.iters = out_iters;
+  return select_arima_call(ctx, "mmf_fit_select_arma_css_f32", true, y, n, ld_y, n_hold, orders, n_orders, diffs,
+                           n_diffs, mas, n_mas, long_order, pred_start, n_pred, out_pred, ld_out, out_choice_p,
+                           out_choice_d, out_choice_q, out_mse, out_cand_mse, out_phi, out_theta, out_order,
+                           out_ma_order, out_sigma, out_status, stats, &css);
+}
+
+int mmf_fit_select_arma_joint_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
+                                  const int32_t* orders, int32_t n_orders, const int32_t* diffs, int32_t n_diffs,
+                                  const int32_t* mas, int32_t n_mas, int32_t long_order, int32_t max_iter,
+                                  int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out, float* out_beta,
+                                  int32_t* out_choice_p, int32_t* out_choice_d, int32_t* out_choice_q, float* out_mse,
+                                  float* out_cand_mse, float* out_phi, float* out_theta, int32_t* out_order,
+                                  int32_t* out_ma_order, float* out_sigma, int32_t* out_status, float* out_css_start,
+                                  float* out_css, int32_t* out_css_stop, int32_t* out_iters, mmf_stats* stats) {
+  if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
+  if (max_iter < 0 || max_iter > MMF_CSS_ITER_MAX)
+    return fail(MMF_E_INVALID, "max_iter=%d outside [0,%d]", max_iter, MMF_CSS_ITER_MAX);
+  CssArgs css{};
+  css.max_iter = max_iter == 0 ? MMF_CSS_ITER_DEFAULT : max_iter;
+  css.css_start = out_css_start; css.css = out_css; css.css_stop = out_css_stop; css.iters = out_iters;
+  JointArgs joint{};
+  joint.beta = out_beta;
+  return select_arima_call(ctx, "mmf_fit_select_arma_joint_f32", true, y, n, ld_y, n_hold, orders, n_orders, diffs,
+                           n_diffs, mas, n_mas, long_order, pred_start, n_pred, out_pred, ld_out, out_choice_p,
+                           out_choice_d, out_choice_q, out_mse, out_cand_mse, out_phi, out_theta, out_order,
+                           out_ma_order, out_sigma, out_status, stats, &css, &joint);
 }
 
 // ---- ragged batches: many calendars, one launch ------------------------------------------------------------------

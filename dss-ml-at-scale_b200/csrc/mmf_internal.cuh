@@ -318,6 +318,26 @@ struct JointArgs {
 cudaError_t launch_arma_joint(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
                               const ArmaArgs& hr, const CssArgs& cs, const JointArgs& jt, cudaStream_t s);
 
+// the refit of a (p, d, q) selection's winners (DESIGN.md section 2 item 18): one stage per listed d behind the
+// selection's stages, on that d's fit.  refit_list_kernel lists the slab's rows whose winner is (p, d, q >= 1) and writes
+// the refit outputs of the rows no refit kernel touches; arma_css_list_kernel / arma_joint_list_kernel run the fixed-order
+// kernels over the list, p and q of each row read from ArArgs::order / ArmaArgs::ma_order (the winner's).  ArArgs::p and
+// ArmaArgs::q are the call's largest listed orders there.
+struct RefitArgs {
+  const int32_t* choice_d;                // [n] the selection's winner (caller buffers or scratch: never null here)
+  const int32_t* choice_q;
+  int32_t first;                          // the call's first refit stage: it also writes the rows with no eligible candidate
+  int32_t* rows;                          // [n] per-slab scratch: the list (any order), and its length
+  uint32_t* count;
+};
+cudaError_t launch_refit_list(const DesignView& d, const FitArgs& a, const ArimaArgs& ma, const CssArgs& cs,
+                              const JointArgs& jt, const RefitArgs& rf, cudaStream_t s);
+cudaError_t launch_arma_css_list(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
+                                 const ArmaArgs& hr, const CssArgs& cs, const RefitArgs& rf, cudaStream_t s);
+cudaError_t launch_arma_joint_list(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
+                                   const ArmaArgs& hr, const CssArgs& cs, const JointArgs& jt, const RefitArgs& rf,
+                                   cudaStream_t s);
+
 // per-series (p, d, q) selection by hold-out MSE on levels (arma_select.cu, DESIGN.md section 2 item 14): one launch per
 // listed d, right behind that d's arima_select_kernel (same fit, z', gamma / c and running best), for the q >= 1 blocks.
 // Candidate lane c is the pair (pq_p[c], pq_q[c]), q-major; its normal equations are those of row set pq_rs[c], the rows

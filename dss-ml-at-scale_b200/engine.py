@@ -786,7 +786,7 @@ class ForecastEngine:
 
     def fit_select_arma(self, y, n_hold: int, orders=(0, 1, 2, 3, 4), diffs=(0, 1, 2), mas=(0, 1, 2, 3, 4),
                         pred_start: int = 0, n_pred: int | None = None, long_order: int = 0, want_stats: bool = False,
-                        want_se: bool = False):
+                        want_se: bool = False, refit: str | None = None, joint_beta: bool = False, max_iter: int = 0):
         """Regression with ARIMA(p, d, q) errors, (p, d, q) chosen per series by hold-out MSE on levels
         (``mmf_fit_select_arma_f32``, DESIGN.md section 2 item 14).  The candidates are every triple of ``orders``,
         ``diffs`` and ``mas`` (ascending, distinct, 0 .. MMF_MA_MAX, ``mas[0] == 0``), d, then q, then p ascending:
@@ -795,8 +795,24 @@ class ForecastEngine:
         floor(ln(t_fit - d)^2)))).  At most 32 pairs (p, q >= 1).  Scores, eligibility and the first-minimum choice are
         ``fit_select_arima``'s; a q >= 1 candidate that fails the Hannan-Rissanen gate scores as (p, d, 0) and never
         wins.  Returns ``fit_select_arima``'s dict plus ``choice_q``, ``theta`` and ``ma_order``; ``cand_mse[i, k, l,
-        j]`` is the score of ``(orders[j], diffs[k], mas[l])``.  With ``mas=(0,)`` the call is ``fit_select_arima``."""
+        j]`` is the score of ``(orders[j], diffs[k], mas[l])``.  With ``mas=(0,)`` the call is ``fit_select_arima``.
+
+        ``refit="css"`` (``mmf_fit_select_arma_css_f32``, DESIGN.md section 2 item 18) refits every series' winner at its
+        own (p, d, q), as the reference fits its final model on the tuned order: a winner with q >= 1 gets every output of
+        ``fit_forecast_arma(p, q, d, long_order=m_d, estimator="css", max_iter=max_iter)`` bit for bit, a winner with
+        q = 0 keeps the selection's.  The choice, ``mse`` and ``cand_mse`` stay the selection's (the refit does not choose
+        again).  The result adds ``css_start``, ``css``, ``css_stop`` and ``iters`` (NaN, NaN, 0, 0 where nothing was
+        refit).  ``joint_beta=True`` (``mmf_fit_select_arma_joint_f32``) refits the q >= 1 winners with beta estimated
+        jointly (``fit_forecast_arma(..., joint_beta=True)``) and adds ``beta`` [n, 16]: the joint call's for those, W
+        gamma of the winner's plain fit for q = 0 winners, NaN where no candidate is eligible.  With ``want_se=True`` the
+        standard errors take the refit's (phi, theta, sigma)."""
         import torch
+        if refit not in (None, "css"):
+            raise ValueError(f"refit must be None or 'css', got {refit!r}")
+        if refit is None and int(max_iter) != 0:
+            raise ValueError("max_iter= is the pass budget of refit='css'")
+        if joint_beta and refit is None:
+            raise ValueError("joint_beta=True needs refit='css' (beta joins the conditional least-squares refit)")
         orders = [int(m) for m in orders]
         diffs = [int(d) for d in diffs]
         mas = [int(q) for q in mas]
@@ -832,16 +848,31 @@ class ForecastEngine:
         dl = (C.c_int32 * max(len(diffs), 1))(*diffs)
         ql = (C.c_int32 * max(len(mas), 1))(*mas)
         st = N.MmfStats() if want_stats else None
-        N.check(self._lib.mmf_fit_select_arma_f32(self._h, yp, n, ld_y, int(n_hold), cand, len(orders), dl, len(diffs),
-                                                  ql, len(mas), int(long_order), int(pred_start), int(n_pred),
-                                                  out.data_ptr(), out.stride(0), choice_p.data_ptr(),
-                                                  choice_d.data_ptr(), choice_q.data_ptr(), mse.data_ptr(),
-                                                  cand_mse.data_ptr(), phi.data_ptr(), theta.data_ptr(),
-                                                  order.data_ptr(), ma_order.data_ptr(), sigma.data_ptr(),
-                                                  status.data_ptr(), C.byref(st) if st is not None else None))
         res = {"pred": out, "choice_p": choice_p, "choice_d": choice_d, "choice_q": choice_q, "mse": mse,
                "cand_mse": cand_mse, "phi": phi, "theta": theta, "order": order, "ma_order": ma_order, "sigma": sigma,
                "status": status}
+        head = (self._h, yp, n, ld_y, int(n_hold), cand, len(orders), dl, len(diffs), ql, len(mas), int(long_order))
+        tail = (choice_p.data_ptr(), choice_d.data_ptr(), choice_q.data_ptr(), mse.data_ptr(), cand_mse.data_ptr(),
+                phi.data_ptr(), theta.data_ptr(), order.data_ptr(), ma_order.data_ptr(), sigma.data_ptr(),
+                status.data_ptr())
+        if refit is None:
+            N.check(self._lib.mmf_fit_select_arma_f32(*head, int(pred_start), int(n_pred), out.data_ptr(), out.stride(0),
+                                                      *tail, C.byref(st) if st is not None else None))
+        else:
+            res.update(css_start=torch.empty(n, device=dev, dtype=torch.float32),
+                       css=torch.empty(n, device=dev, dtype=torch.float32),
+                       css_stop=torch.empty(n, device=dev, dtype=torch.int32),
+                       iters=torch.empty(n, device=dev, dtype=torch.int32))
+            css_out = (res["css_start"].data_ptr(), res["css"].data_ptr(), res["css_stop"].data_ptr(),
+                       res["iters"].data_ptr(), C.byref(st) if st is not None else None)
+            if joint_beta:
+                res["beta"] = torch.empty((n, N.MMF_P), device=dev, dtype=torch.float32)
+                N.check(self._lib.mmf_fit_select_arma_joint_f32(*head, int(max_iter), int(pred_start), int(n_pred),
+                                                                out.data_ptr(), out.stride(0), res["beta"].data_ptr(),
+                                                                *tail, *css_out))
+            else:
+                N.check(self._lib.mmf_fit_select_arma_css_f32(*head, int(max_iter), int(pred_start), int(n_pred),
+                                                              out.data_ptr(), out.stride(0), *tail, *css_out))
         if want_se:
             self._add_se(res, y, t_fit, pred_start, n_pred, 0, diffs=choice_d)
         if st is not None:

@@ -339,7 +339,7 @@ def _host(x):
 
 
 def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, interval=False, ar=None, diff=None,
-                 ma=None, want_se=False, estimator=None, joint_beta=False):
+                 ma=None, want_se=False, estimator=None, joint_beta=False, refit=None):
     """Run the engine over every bucket: yields (bucket, out_days, n_pred, y_host, pred_host, se_host or None).
     ``interval``: prediction standard errors too (``fit_forecast_se``), one call per calendar bucket.
     ``ar``: regression with AR(ar) errors (``fit_forecast_ar``), one call per calendar bucket; a tuple of orders
@@ -352,7 +352,9 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
     ``horizon`` rows (``fit_select_arma``).
     ``want_se``: the ARIMA-family call's forecast standard errors too (``want_se=True``, DESIGN.md section 2 item 15).
     ``estimator``: the fixed-order ARIMA(p, d, q) call's estimator (None: the engine's default, Hannan-Rissanen);
-    ``joint_beta``: with ``estimator="css"``, beta estimated jointly with (phi, theta)."""
+    ``joint_beta``: with ``estimator="css"``, beta estimated jointly with (phi, theta).
+    ``refit``: with candidate MA orders, the winner refit by conditional least squares (``joint_beta`` with it: beta
+    jointly)."""
     se_kw = {"want_se": True} if want_se else {}
     if interval and select is not None:
         raise ValueError("interval= is not offered with select= (model selection returns point forecasts)")
@@ -371,7 +373,8 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
         if isinstance(ma, tuple):
             from .engine import device_packed
             yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
-            res = eng.fit_select_arma(yd, horizon, ar, diff, ma, pred_start, n_pred, **se_kw)
+            ref_kw = {"refit": refit, "joint_beta": joint_beta} if refit is not None else {}
+            res = eng.fit_select_arma(yd, horizon, ar, diff, ma, pred_start, n_pred, **se_kw, **ref_kw)
             pred, se = _host(res["pred"]), (_host(res["se"]) if want_se else None)
         elif ma is not None:
             from .engine import device_packed
@@ -553,10 +556,31 @@ def _estimator(estimator, ma, select, interval):
     return estimator
 
 
-def _joint_beta(joint_beta, estimator):
-    """validated ``joint_beta=``: True needs ``estimator="css"`` (DESIGN.md section 2 item 17)"""
+def _refit(refit, ma, estimator, select, interval):
+    """validated ``refit=``: None (the selection's Hannan-Rissanen winners, as before) or "css", the winner of the
+    (p, d, q) selection refit by conditional least squares (DESIGN.md section 2 item 18).  It needs candidate MA orders."""
+    if refit is None:
+        return None
+    if refit != "css":
+        raise ValueError(f"refit must be None or 'css', got {refit!r}")
+    if select is not None or interval is not None:
+        raise ValueError("refit= is not offered with select= or interval= (ARMA forecasts come without either)")
+    if estimator is not None:
+        raise ValueError(f"refit= is not offered with estimator= (estimator= chooses how a fixed ma=q is estimated, "
+                         f"refit= refits a selection's winner), got estimator={estimator!r}")
+    if not isinstance(ma, (list, tuple, np.ndarray)):
+        raise ValueError(f"refit= needs candidate MA orders ma=(0, ...) (it refits the winner of the (p, d, q) "
+                         f"selection), got ma={ma!r}")
+    return refit
+
+
+def _joint_beta(joint_beta, estimator, refit=None):
+    """validated ``joint_beta=``: True needs ``estimator="css"`` (DESIGN.md section 2 item 17) or ``refit="css"`` (item
+    18)"""
     if not joint_beta:
         return False
+    if refit == "css":
+        return True
     if estimator != "css":
         raise ValueError(f"joint_beta=True needs estimator='css' (beta joins the conditional least-squares fit), "
                          f"got estimator={estimator!r}")
@@ -680,7 +704,7 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
                     freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                     engine: ForecastEngine | None = None, pack: str = "host", select=None,
                     null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None, ma=None,
-                    conf_int=None, estimator=None, joint_beta=False) -> pd.DataFrame:
+                    conf_int=None, estimator=None, joint_beta=False, refit=None) -> pd.DataFrame:
     """Fit + forecast every group in ``pdf``; returns ``tuning_schema`` rows
     (keys..., Date, Demand, Demand_Fitted), groups in key order, dates ascending.
 
@@ -751,6 +775,11 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     (``ForecastEngine.fit_forecast_arma(..., joint_beta=True)``, DESIGN.md section 2 item 17: regression with ARIMA errors
     as SARIMAX fits it, by the conditional likelihood); schema unchanged, ``conf_int=`` works as above.  Refused without
     ``estimator="css"``.
+    ``refit="css"`` with candidate MA orders refits every series' winning (p, d, q) by conditional least squares, as the
+    reference fits its final model on the tuned order (``ForecastEngine.fit_select_arma(..., refit="css")``, DESIGN.md
+    section 2 item 18); ``joint_beta=True`` with it estimates beta jointly in that refit.  Schema unchanged, ``conf_int=``
+    works as above.  Refused with a fixed ``ma=``, with ``estimator=``, ``select=`` or ``interval=``, and for any value
+    other than ``"css"``.
     """
     eng = engine or default_engine()
     keys = list(keys)
@@ -758,7 +787,8 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     z = _z_of(interval)
     cz = _conf_z(conf_int, ar, select, interval)
     est = _estimator(estimator, ma, select, interval)
-    jb = _joint_beta(joint_beta, est)
+    ref = _refit(refit, ma, est, select, interval)
+    jb = _joint_beta(joint_beta, est, ref)
     if ma is None:
         diff = _diff_order(diff, ar, select, interval, mode)
         ar = _ar_orders_for(diff, ar, select, interval, mode)
@@ -773,7 +803,7 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     parts, lengths = [], []
     for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
                                                               pack == "device", z is not None, ar, diff, ma,
-                                                              cz is not None, est, jb):
+                                                              cz is not None, est, jb, ref):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n), n_pred)
         # key columns keep the dtype they came in with (no per-row string inference on N x T values)
@@ -865,7 +895,7 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
                    freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                    engine: ForecastEngine | None = None, pack: str = "host", select=None,
                    null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None, ma=None,
-                   conf_int=None, estimator=None, joint_beta=False):
+                   conf_int=None, estimator=None, joint_beta=False, refit=None):
     """Arrow ``Table``/``RecordBatch`` in -> Arrow ``Table`` with ``tuning_schema`` out (the ``mapInArrow``
     flavour of the boundary).  No pandas frame of the rows on either side: keys are dictionary-encoded on the way
     in and expanded from a dictionary on the way out, dates and values are NumPy views of Arrow buffers.
@@ -873,8 +903,8 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     ``tuning_schema(..., interval=True)``).  ``ar=p`` fits regression with AR(p) errors and ``ar=(0, 1, 2, 3, 4)`` chooses the order per series, as in
     ``forecast_groups``; ``diff=d`` with ``ar=p`` fits ARIMA(p, d, 0) errors as there, and ``ma=q`` ARIMA(p, d, q); tuples of ``ar``, ``diff`` and
     ``ma`` choose (p, d, q) per series.  ``conf_int=level`` adds the same two columns for those forecasts, and
-    ``estimator="css"`` refines a fixed ``ma=q``'s estimate and ``joint_beta=True`` adds beta to it, as in
-    ``forecast_groups``."""
+    ``estimator="css"`` refines a fixed ``ma=q``'s estimate and ``joint_beta=True`` adds beta to it, and ``refit="css"``
+    refits the selection's winners (with ``joint_beta=True``: beta jointly), as in ``forecast_groups``."""
     import pyarrow as pa
 
     if isinstance(table, pa.RecordBatch):
@@ -884,7 +914,8 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     z = _z_of(interval)
     cz = _conf_z(conf_int, ar, select, interval)
     est = _estimator(estimator, ma, select, interval)
-    jb = _joint_beta(joint_beta, est)
+    ref = _refit(refit, ma, est, select, interval)
+    jb = _joint_beta(joint_beta, est, ref)
     if ma is None:
         diff = _diff_order(diff, ar, select, interval, mode)
         ar = _ar_orders_for(diff, ar, select, interval, mode)
@@ -896,7 +927,7 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     parts, lengths = [], []
     for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
                                                               pack == "device", z is not None, ar, diff, ma,
-                                                              cz is not None, est, jb):
+                                                              cz is not None, est, jb, ref):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n, dtype=np.int32), n_pred)
         cols = []

@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define MMF_VERSION 113          /* 0.1.13 */
+#define MMF_VERSION 114          /* 0.1.14 */
 #define MMF_P 16                 /* design columns (zero-pad narrower designs) */
 #define MMF_PIVOT_TOL 1e-3f      /* per-series relative Cholesky pivot threshold */
 #define MMF_CAL_TOL 1e-10        /* aliasing threshold on the float64 calendar Gram */
@@ -465,6 +465,51 @@ int mmf_fit_select_arma_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_
                             float* out_cand_mse /* [n][n_diffs][n_mas][n_orders] */, float* out_phi, float* out_theta,
                             int32_t* out_order, int32_t* out_ma_order, float* out_sigma, int32_t* out_status,
                             mmf_stats* stats);
+
+/* ---- the (p, d, q) selection's winner refit by conditional least squares (DESIGN.md section 2 item 18) -----------------
+ * mmf_fit_select_arma_css_f32: mmf_fit_select_arma_f32, then every series' winner refit at its own (p, d, q) by
+ * mmf_fit_forecast_arma_css_f32's Levenberg-Marquardt, from the winner's Hannan-Rissanen (phi, theta).  The arguments are
+ * mmf_fit_select_arma_f32's, with max_iter and the nullable out_css_start, out_css, out_css_stop and out_iters [n] of
+ * mmf_fit_forecast_arma_css_f32.  Per row:
+ *   a winner with q >= 1 gets every output (pred, phi, theta, order, ma_order, sigma, status, css_start, css, css_stop,
+ *   iters) of mmf_fit_forecast_arma_css_f32 at its (p, d, q) with long_order = m_d (the selection's long order of its d),
+ *   the same max_iter and the same prediction window, bit for bit (such a winner passed the Hannan-Rissanen gate);
+ *   a winner with q = 0 keeps every output of mmf_fit_select_arma_f32 bit for bit, with css_start and css NaN and
+ *   css_stop and iters 0; so does a row with no eligible candidate.
+ * choice_p, choice_d, choice_q, mse and cand_mse are mmf_fit_select_arma_f32's bit for bit: the refit does not choose
+ * again, and mse stays the score of the Hannan-Rissanen winner.  max_iter outside [0, MMF_CSS_ITER_MAX] is MMF_E_INVALID,
+ * checked first; every other refusal is mmf_fit_select_arma_f32's, with its code and text.  Otherwise the contract of
+ * mmf_fit_select_arma_f32 (plans, device buffers only, any ld_out, enqueue-only unless `stats` is non-NULL, whose n_pending
+ * then also counts the refit's fits, mmf_config.kernel and assume_finite honoured, refused arguments write nothing).
+ * Scratch: per slab, that of mmf_fit_select_arma_f32 and 68 B per row (the winner's phi, theta, order, ma_order,
+ * choice_d and choice_q, written there when the caller passes NULL for them, and the list of the rows refit).
+ * replaces: the reference's final model (02:472-481), SARIMAX(order = the tuned order, exog) fitted on the training rows
+ * after the tuning loop, by the conditional likelihood. */
+int mmf_fit_select_arma_css_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
+                                const int32_t* orders, int32_t n_orders, const int32_t* diffs, int32_t n_diffs,
+                                const int32_t* mas, int32_t n_mas, int32_t long_order, int32_t max_iter,
+                                int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out,
+                                int32_t* out_choice_p, int32_t* out_choice_d, int32_t* out_choice_q, float* out_mse,
+                                float* out_cand_mse /* [n][n_diffs][n_mas][n_orders] */, float* out_phi,
+                                float* out_theta, int32_t* out_order, int32_t* out_ma_order, float* out_sigma,
+                                int32_t* out_status, float* out_css_start, float* out_css, int32_t* out_css_stop,
+                                int32_t* out_iters, mmf_stats* stats);
+
+/* mmf_fit_select_arma_joint_f32: mmf_fit_select_arma_css_f32 with each q >= 1 winner refit by
+ * mmf_fit_forecast_arma_joint_f32 (beta jointly with (phi, theta)) instead, every output of that call at the winner's
+ * (p, d, q), long_order = m_d, bit for bit; and the nullable out_beta [n][MMF_P]: the joint call's for a q >= 1 winner;
+ * for a q = 0 winner W gamma (+ c on the intercept) of the plain fit the winner builds on, in arma_joint's fp32 order
+ * (for d = 0 mmf_fit_forecast_f32's out_beta bit for bit; for d >= 1 the coefficients of Delta^d X); NaN for a row with
+ * no eligible candidate.  Otherwise mmf_fit_select_arma_css_f32's contract. */
+int mmf_fit_select_arma_joint_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
+                                  const int32_t* orders, int32_t n_orders, const int32_t* diffs, int32_t n_diffs,
+                                  const int32_t* mas, int32_t n_mas, int32_t long_order, int32_t max_iter,
+                                  int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out, float* out_beta,
+                                  int32_t* out_choice_p, int32_t* out_choice_d, int32_t* out_choice_q, float* out_mse,
+                                  float* out_cand_mse /* [n][n_diffs][n_mas][n_orders] */, float* out_phi,
+                                  float* out_theta, int32_t* out_order, int32_t* out_ma_order, float* out_sigma,
+                                  int32_t* out_status, float* out_css_start, float* out_css, int32_t* out_css_stop,
+                                  int32_t* out_iters, mmf_stats* stats);
 
 /* ---- standard errors of the ARIMA-family forecasts (DESIGN.md section 2 item 15) ----------------------------------------
  * mmf_arima_se_f32: a post-pass over the outputs of any ARIMA-family call (mmf_fit_forecast_ar_f32, _arima_f32, _arma_f32,

@@ -552,7 +552,7 @@ struct Tally {
 // arima_select_kernel; their d = 0 call (arima->d == 0) fits y itself with the mmf_plan_design plan; (p, d, q) selections
 // (hsel, with asel) add arma_select_kernel behind it.  ARMA calls (arma, with ar) run arma_kernel behind ar_kernel
 // (d = 0, no arima) or arima_kernel; CSS calls (css, with arma) add arma_css_kernel behind arma_kernel, joint calls (joint,
-// with css) arma_joint_kernel in its place.  Refit stages of a (p, d, q) selection (refit, with ar, arima, arma and css)
+// with css) arma_joint_kernel in its place, ML calls (ml, with css) arma_ml_kernel behind arma_css_kernel.  Refit stages of a (p, d, q) selection (refit, with ar, arima, arma and css)
 // run the fit of their d, refit_list_kernel and arma_css_list_kernel (joint: arma_joint_list_kernel).
 struct Call {
   const float* y = nullptr;
@@ -574,6 +574,7 @@ struct Call {
   std::optional<ArmaSelArgs> hsel;
   std::optional<CssArgs> css;
   std::optional<JointArgs> joint;
+  std::optional<MlArgs> ml;
   std::optional<RefitArgs> refit;
 
   // the same call on the rows from `off` on: every per-row output advanced by `off` rows (null stays null)
@@ -616,6 +617,12 @@ struct Call {
       c.css->iters = at(css->iters, 1);
     }
     if (joint) c.joint->beta = at(joint->beta, P);
+    if (ml) {
+      c.ml->loglik_start = at(ml->loglik_start, 1);
+      c.ml->loglik = at(ml->loglik, 1);
+      c.ml->stop = at(ml->stop, 1);
+      c.ml->iters = at(ml->iters, 1);
+    }
     if (refit) { c.refit->choice_d = at(refit->choice_d, 1); c.refit->choice_q = at(refit->choice_q, 1); }
     return c;
   }
@@ -759,6 +766,10 @@ int run_device_slab(mmf_ctx* ctx, const Plan& plan, const Call& c, int64_t n, Ta
         CU_TRY(c.joint ? launch_arma_joint(d, a, *c.ar, mh, *c.arma, *c.css, *c.joint, s)
                        : launch_arma_css(d, a, *c.ar, mh, *c.arma, *c.css, s));
         ++t.launches;
+        if (c.ml) {
+          CU_TRY(launch_arma_ml(d, a, *c.ar, mh, *c.arma, *c.ml, s));
+          ++t.launches;
+        }
       }
     }
   }
@@ -1620,13 +1631,14 @@ int mmf_fit_forecast_arima_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t 
 }
 
 // ---- regression with ARIMA(p, d, q) errors (DESIGN.md section 2 items 13, 16, 17) ----------------------------------------
-// The HR call (css == nullptr), the CSS call and the joint call (joint != nullptr, with css): the same checks, plans and
-// launches; the CSS call adds arma_css_kernel behind arma_kernel in every slab, the joint call arma_joint_kernel.
+// The HR call (css == nullptr), the CSS call, the joint call (joint != nullptr, with css) and the ML call (ml != nullptr,
+// with css): the same checks, plans and launches; the CSS call adds arma_css_kernel behind arma_kernel in every slab, the
+// joint call arma_joint_kernel, the ML call arma_ml_kernel behind arma_css_kernel.
 static int arma_call(mmf_ctx* ctx, const char* name, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
                      int32_t diff_order, int32_t ma_order, int32_t long_order, int32_t pred_start, int32_t n_pred,
                      float* out_pred, int64_t ld_out, float* out_phi, float* out_theta, int32_t* out_order,
                      int32_t* out_ma_order, float* out_sigma, int32_t* out_status, mmf_stats* stats,
-                     const CssArgs* css, const JointArgs* joint = nullptr) {
+                     const CssArgs* css, const JointArgs* joint = nullptr, const MlArgs* ml = nullptr) {
   if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
   GrowScope grow_scope(ctx);
   if (n < 0) return fail(MMF_E_INVALID, "n < 0");
@@ -1654,7 +1666,9 @@ static int arma_call(mmf_ctx* ctx, const char* name, const float* y, int64_t n, 
   CU_TRY(cudaSetDevice(ctx->device));
   if (!on_device({y, out_pred}, {out_phi, out_theta, out_order, out_ma_order, out_sigma, out_status,
                                  css ? css->css_start : nullptr, css ? css->css : nullptr, css ? css->css_stop : nullptr,
-                                 css ? css->iters : nullptr, joint ? joint->beta : nullptr}))
+                                 css ? css->iters : nullptr, joint ? joint->beta : nullptr,
+                                 ml ? ml->loglik_start : nullptr, ml ? ml->loglik : nullptr, ml ? ml->stop : nullptr,
+                                 ml ? ml->iters : nullptr}))
     return fail(MMF_E_UNSUPPORTED, "%s takes device buffers only", name);
   Call c = plain_call(y, ld_y, pred_start, n_pred, out_pred, ld_out, out_status);
   c.ar = ar_args(ar_order, out_phi, out_order, out_sigma, pl);
@@ -1666,6 +1680,7 @@ static int arma_call(mmf_ctx* ctx, const char* name, const float* y, int64_t n, 
   if (diff_order > 0) c.arima = arima_args(ld_y, ap.t_fit, diff_order);
   if (css) c.css = *css;
   if (joint) c.joint = *joint;
+  if (ml) c.ml = *ml;
   return enqueue(ctx, pl, {{&pl, c}}, n, stats);
 }
 
@@ -1713,6 +1728,25 @@ int mmf_fit_forecast_arma_joint_f32(mmf_ctx* ctx, const float* y, int64_t n, int
   return arma_call(ctx, "mmf_fit_forecast_arma_joint_f32", y, n, ld_y, ar_order, diff_order, ma_order, long_order,
                    pred_start, n_pred, out_pred, ld_out, out_phi, out_theta, out_order, out_ma_order, out_sigma,
                    out_status, stats, &css, &joint);
+}
+
+int mmf_fit_forecast_arma_ml_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
+                                 int32_t diff_order, int32_t ma_order, int32_t long_order, int32_t max_iter,
+                                 int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out, float* out_phi,
+                                 float* out_theta, int32_t* out_order, int32_t* out_ma_order, float* out_sigma,
+                                 int32_t* out_status, float* out_loglik_start, float* out_loglik, int32_t* out_ml_stop,
+                                 int32_t* out_iters, mmf_stats* stats) {
+  if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
+  if (max_iter < 0 || max_iter > MMF_CSS_ITER_MAX)
+    return fail(MMF_E_INVALID, "max_iter=%d outside [0,%d]", max_iter, MMF_CSS_ITER_MAX);
+  CssArgs css{};                           // the CSS call's start, its own columns unwritten
+  css.max_iter = max_iter == 0 ? MMF_CSS_ITER_DEFAULT : max_iter;
+  MlArgs ml{};
+  ml.max_iter = css.max_iter;
+  ml.loglik_start = out_loglik_start; ml.loglik = out_loglik; ml.stop = out_ml_stop; ml.iters = out_iters;
+  return arma_call(ctx, "mmf_fit_forecast_arma_ml_f32", y, n, ld_y, ar_order, diff_order, ma_order, long_order,
+                   pred_start, n_pred, out_pred, ld_out, out_phi, out_theta, out_order, out_ma_order, out_sigma,
+                   out_status, stats, &css, nullptr, &ml);
 }
 
 // ---- standard errors of the ARIMA-family forecasts (DESIGN.md section 2 item 15) ---------------------------------------

@@ -318,6 +318,19 @@ struct JointArgs {
 cudaError_t launch_arma_joint(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
                               const ArmaArgs& hr, const CssArgs& cs, const JointArgs& jt, cudaStream_t s);
 
+// ARIMA(p, d, q) errors by exact Gaussian likelihood (arma_ml.cu, DESIGN.md section 2 item 19): arma_ml_kernel runs
+// behind arma_css_kernel in the same slab, reads the CSS (phi, theta) from ArArgs::phi / ArmaArgs::theta and the gated
+// rows from ArmaArgs::ma_order (never null for this kernel), and overwrites the outputs of the rows that accepted a step
+struct MlArgs {
+  int32_t max_iter;                       // passes per series, 1 .. MMF_CSS_ITER_MAX (resolved: never 0)
+  float* loglik_start;                    // nullable [n]: the exact log-likelihood at the CSS estimate
+  float* loglik;                          // nullable [n]: ... at the shipped estimate
+  int32_t* stop;                          // nullable [n]: 1 converged, 2 stalled, 3 budget, 0 not refined
+  int32_t* iters;                         // nullable [n]: passes run
+};
+cudaError_t launch_arma_ml(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
+                           const ArmaArgs& hr, const MlArgs& ml, cudaStream_t s);
+
 // the refit of a (p, d, q) selection's winners (DESIGN.md section 2 item 18): one stage per listed d behind the
 // selection's stages, on that d's fit.  refit_list_kernel lists the slab's rows whose winner is (p, d, q >= 1) and writes
 // the refit outputs of the rows no refit kernel touches; arma_css_list_kernel / arma_joint_list_kernel run the fixed-order

@@ -603,15 +603,25 @@ class ForecastEngine:
         ARIMA errors, R's ``arima(xreg=, method="CSS")``).  The result adds ``beta`` [n, 16], the coefficients of the raw
         design columns the series ships (of the differenced design for ``diff_order`` >= 1; NaN for empty series).  With
         ``want_se=True`` the standard errors take the joint (phi, theta, sigma); beta's estimation uncertainty is not
-        included."""
+        included.
+
+        ``estimator="ml"`` (``mmf_fit_forecast_arma_ml_f32``, DESIGN.md section 2 item 19) runs ``estimator="css"``
+        and then refines every gated series' (phi, theta) on the exact Gaussian likelihood of its residuals: a Kalman
+        filter from the stationary start (missing rows predicted, not filled), the same Levenberg-Marquardt and
+        ``max_iter`` (R's ``arima(method="CSS-ML")`` on the differenced series).  A series that accepts no step keeps the
+        CSS outputs bit for bit; ``sigma`` is the ML estimate for every gated series.  The result adds ``loglik_start``
+        (the exact log-likelihood at the CSS estimate), ``loglik`` (at the shipped one), ``ml_stop`` (the CSS codes) and
+        ``iters`` (ML passes run).  ``want_se=True`` takes the ML (phi, theta, sigma).  Not with ``joint_beta=True``."""
         import torch
-        if estimator not in ("hr", "css"):
-            raise ValueError(f"estimator must be 'hr' or 'css', got {estimator!r}")
-        css = estimator == "css"
+        if estimator not in ("hr", "css", "ml"):
+            raise ValueError(f"estimator must be 'hr' or 'css' (or 'ml' for the exact likelihood), got {estimator!r}")
+        ml = estimator == "ml"
+        css = estimator == "css" or ml
         if not css and int(max_iter) != 0:
             raise ValueError("max_iter= is the pass budget of estimator='css'")
-        if joint_beta and not css:
-            raise ValueError("joint_beta=True needs estimator='css' (beta joins the conditional least-squares fit)")
+        if joint_beta and estimator != "css":
+            raise ValueError(f"joint_beta=True needs estimator='css' (beta joins the conditional least-squares fit), "
+                             f"got estimator={estimator!r}")
         if int(diff_order) >= 1:
             if getattr(self, "_arima", None) is None:
                 raise RuntimeError("plan_arima() (or plan_calendar(..., max_diff=d)) must be called first")
@@ -640,7 +650,14 @@ class ForecastEngine:
             css_end = torch.empty(n, device=dev, dtype=torch.float32)
             css_stop = torch.empty(n, device=dev, dtype=torch.int32)
             iters = torch.empty(n, device=dev, dtype=torch.int32)
-            if joint_beta:
+            if ml:
+                N.check(self._lib.mmf_fit_forecast_arma_ml_f32(
+                    self._h, yp, n, ld_y, int(ar_order), int(diff_order), int(ma_order), int(long_order),
+                    int(max_iter), int(pred_start), int(n_pred), out.data_ptr(), out.stride(0), phi.data_ptr(),
+                    theta.data_ptr(), order.data_ptr(), ma.data_ptr(), sigma.data_ptr(), status.data_ptr(),
+                    css_start.data_ptr(), css_end.data_ptr(), css_stop.data_ptr(), iters.data_ptr(),
+                    C.byref(st) if st is not None else None))
+            elif joint_beta:
                 beta = torch.empty((n, N.MMF_P), device=dev, dtype=torch.float32)
                 N.check(self._lib.mmf_fit_forecast_arma_joint_f32(
                     self._h, yp, n, ld_y, int(ar_order), int(diff_order), int(ma_order), int(long_order),
@@ -663,7 +680,9 @@ class ForecastEngine:
                                                         status.data_ptr(), C.byref(st) if st is not None else None))
         res = {"pred": out, "phi": phi, "theta": theta, "order": order, "ma_order": ma, "sigma": sigma,
                "status": status}
-        if css:
+        if ml:
+            res.update(loglik_start=css_start, loglik=css_end, ml_stop=css_stop, iters=iters)
+        elif css:
             res.update(css_start=css_start, css=css_end, css_stop=css_stop, iters=iters)
             if joint_beta:
                 res["beta"] = beta

@@ -540,12 +540,12 @@ def _arma_orders(ma, ar, diff, select, interval, mode="holdout"):
 
 
 def _estimator(estimator, ma, select, interval):
-    """validated ``estimator=`` of the fixed-order ARIMA(p, d, q) forecasts: None (Hannan-Rissanen, as before), "hr" or
-    "css" (DESIGN.md section 2 item 16).  It needs one MA order ``ma=q``."""
+    """validated ``estimator=`` of the fixed-order ARIMA(p, d, q) forecasts: None (Hannan-Rissanen, as before), "hr",
+    "css" (DESIGN.md section 2 item 16) or "ml" (item 19).  It needs one MA order ``ma=q``."""
     if estimator is None:
         return None
-    if estimator not in ("hr", "css"):
-        raise ValueError(f"estimator must be 'hr' or 'css', got {estimator!r}")
+    if estimator not in ("hr", "css", "ml"):
+        raise ValueError(f"estimator must be 'hr' or 'css' (or 'ml' for the exact likelihood), got {estimator!r}")
     if select is not None or interval is not None:
         raise ValueError("estimator= is not offered with select= or interval= (ARMA forecasts come without either)")
     if ma is None:
@@ -770,7 +770,9 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     ``estimator="css"`` with a fixed ``ma=q`` refines every gated series' Hannan-Rissanen (phi, theta) by conditional
     least squares (``ForecastEngine.fit_forecast_arma(..., estimator="css")``, DESIGN.md section 2 item 16); schema
     unchanged, ``conf_int=`` works as above.  ``estimator=None`` (or ``"hr"``) leaves everything as it was.  Refused
-    without ``ma=``, with candidate MA orders, ``select=`` or ``interval=``.
+    without ``ma=``, with candidate MA orders, ``select=`` or ``interval=``.  ``estimator="ml"`` refines that CSS
+    estimate by the exact Gaussian likelihood (``ForecastEngine.fit_forecast_arma(..., estimator="ml")``, DESIGN.md
+    section 2 item 19), with the same arguments, refusals, schema and ``conf_int=``.
     ``joint_beta=True`` with ``estimator="css"`` estimates the design's coefficients jointly with (phi, theta)
     (``ForecastEngine.fit_forecast_arma(..., joint_beta=True)``, DESIGN.md section 2 item 17: regression with ARIMA errors
     as SARIMAX fits it, by the conditional likelihood); schema unchanged, ``conf_int=`` works as above.  Refused without
@@ -903,7 +905,7 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     ``tuning_schema(..., interval=True)``).  ``ar=p`` fits regression with AR(p) errors and ``ar=(0, 1, 2, 3, 4)`` chooses the order per series, as in
     ``forecast_groups``; ``diff=d`` with ``ar=p`` fits ARIMA(p, d, 0) errors as there, and ``ma=q`` ARIMA(p, d, q); tuples of ``ar``, ``diff`` and
     ``ma`` choose (p, d, q) per series.  ``conf_int=level`` adds the same two columns for those forecasts, and
-    ``estimator="css"`` refines a fixed ``ma=q``'s estimate and ``joint_beta=True`` adds beta to it, and ``refit="css"``
+    ``estimator="css"`` (or ``"ml"``) refines a fixed ``ma=q``'s estimate and ``joint_beta=True`` adds beta to it, and ``refit="css"``
     refits the selection's winners (with ``joint_beta=True``: beta jointly), as in ``forecast_groups``."""
     import pyarrow as pa
 

@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define MMF_VERSION 114          /* 0.1.14 */
+#define MMF_VERSION 115          /* 0.1.15 */
 #define MMF_P 16                 /* design columns (zero-pad narrower designs) */
 #define MMF_PIVOT_TOL 1e-3f      /* per-series relative Cholesky pivot threshold */
 #define MMF_CAL_TOL 1e-10        /* aliasing threshold on the float64 calendar Gram */
@@ -355,7 +355,7 @@ int mmf_fit_forecast_arma_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t l
  * series sigma = sqrt(S / |C|) at the shipped point (the conditional MLE).  Series that fail the HR gate and empty
  * series get the HR call's outputs bit for bit.  out_css_start [n] (S(x0)), out_css [n] (S shipped), out_css_stop [n]
  * and out_iters [n] (passes run) are nullable; NaN, NaN, 0, 0 for fallback and empty series.  beta is not re-estimated;
- * this is not the exact (Kalman) likelihood.  Otherwise the contract of mmf_fit_forecast_arma_f32 (plans, device buffers
+ * this is not the exact (Kalman) likelihood (mmf_fit_forecast_arma_ml_f32 refines this call's estimate to it).  Otherwise the contract of mmf_fit_forecast_arma_f32 (plans, device buffers
  * only, any ld_out, enqueue-only unless `stats` is non-NULL, mmf_config.kernel and assume_finite honoured, refused
  * arguments write nothing); max_iter outside [0, MMF_CSS_ITER_MAX] is MMF_E_INVALID.  Scratch: per slab, 52 B per row
  * when out_phi, out_theta or out_ma_order is NULL.
@@ -393,6 +393,44 @@ int mmf_fit_forecast_arma_joint_f32(mmf_ctx* ctx, const float* y, int64_t n, int
                                     float* out_phi, float* out_theta, int32_t* out_order, int32_t* out_ma_order,
                                     float* out_sigma, int32_t* out_status, float* out_css_start, float* out_css,
                                     int32_t* out_css_stop, int32_t* out_iters, mmf_stats* stats);
+
+/* ---- ARIMA(p, d, q) errors by exact Gaussian likelihood (DESIGN.md section 2 item 19) ---------------------------------
+ * mmf_fit_forecast_arma_ml_f32: mmf_fit_forecast_arma_css_f32 with the same arguments and max_iter, then
+ * Levenberg-Marquardt refinement of every gated series' (phi, theta) on the exact Gaussian likelihood of its residuals
+ * (R's arima(method = "CSS-ML") on the differenced series):
+ *   model: e_s, s < T, the residual the CSS call models (y for d = 0, z' for d >= 1; beta not re-estimated) is a zero-mean
+ *   ARMA(p, q) in Harvey's state-space form: r = max(p, q + 1), T with phi in its first column and I on its
+ *   superdiagonal, R = (1, theta_1 .. theta_{r-1})', Z = (1, 0 .. 0), no observation noise, sigma^2 concentrated out;
+ *   start of the filter: a = 0 and P_{0|-1} the stationary state covariance, vec P = (I - T (x) T)^-1 vec(R R'), solved in
+ *   float64 on the r (r + 1) / 2 symmetric unknowns by Gaussian elimination with partial pivoting; a pivot |u_kk| <=
+ *   MMF_HR_PIVOT_TOL x max |A| fails the solve.  This is Gardner's start on the differenced series, not SARIMAX's
+ *   approximate-diffuse start over the levels;
+ *   filter over s in [0, T) in float64 from the fp32 residuals: on an observed row v_s = e_s - a_1, F_s = P_11, K = T P Z'
+ *   / F_s, a <- T a + K v_s, P <- T P T' + R R' - K K' F_s; on a missing row a <- T a, P <- T P T' + R R' (no steady-state
+ *   shortcut).  With n the number of observed rows (none conditioned on), S_w = sum v_s^2 / F_s:
+ *   L = n log(S_w / n) + sum log F_s, loglik = -(L + n (1 + log 2 pi)) / 2, sigma = sqrt(S_w / n);
+ *   optimiser: the CSS call's Levenberg-Marquardt (start, step, constants, accept, stops) on the scaled innovations r_s =
+ *   G v_s / sqrt(F_s), G = exp(sum log F_s / (2 n)), so that sum r_s^2 = G^2 S_w = n exp(L / n) is the objective and
+ *   MMF_CSS_RTOL applies to it.  The Jacobian is exact (forward-mode derivatives of a, P, K and P_0); G enters H and g
+ *   as a rank-2 correction.  The first pass is at x0 = the (phi, theta) the CSS call ships; a trial point whose P_0
+ *   solve fails counts as one that fails the step-down test (lambda <- 10 lambda, no pass).
+ * Outputs: a gated series that accepted no step keeps the CSS call's pred, phi, theta, order, ma_order and status bit for
+ * bit; one that did gets the recursion and level integration of the HR call with the shipped (phi, theta) (the library's
+ * predictor, not the Kalman filter's, so mmf_arima_se_f32 applies unchanged).  For every gated series sigma = sigma at
+ * the shipped point.  out_loglik_start [n] (loglik at x0), out_loglik [n] (at the shipped point, >= out_loglik_start),
+ * out_ml_stop [n] (the CSS call's codes, 0 not refined) and out_iters [n] (passes run) are nullable.  A gated series whose
+ * x0 fails the P_0 solve keeps every CSS output, with NaN, NaN, 0, 0.  Series that fail the HR gate and empty series get
+ * the HR call's outputs and NaN, NaN, 0, 0.  Otherwise the contract of mmf_fit_forecast_arma_css_f32 (plans, refusals
+ * with max_iter checked first, device buffers only, any ld_out, enqueue-only unless `stats`, mmf_config.kernel and
+ * assume_finite, scratch).
+ * replaces: SARIMAX(p, d, q) + exog fit of the reference's per-group model (02:441-450, 472-481), which maximises the
+ * exact likelihood. */
+int mmf_fit_forecast_arma_ml_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
+                                 int32_t diff_order, int32_t ma_order, int32_t long_order, int32_t max_iter,
+                                 int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out, float* out_phi,
+                                 float* out_theta, int32_t* out_order, int32_t* out_ma_order, float* out_sigma,
+                                 int32_t* out_status, float* out_loglik_start, float* out_loglik, int32_t* out_ml_stop,
+                                 int32_t* out_iters, mmf_stats* stats);
 
 /* ---- (p, d) selection by hold-out MSE on levels (DESIGN.md section 2 item 12) -----------------------------------------
  * mmf_fit_select_arima_f32: orders [n_orders] (1 .. MMF_ARSEL_MAX_CAND ascending distinct values in [0, MMF_AR_MAX]) and

@@ -5,9 +5,12 @@ alternates the HR call with the CSS call over several rounds after a warm-up, ti
 (median), ms per pass (the CSS call's extra time over the mean pass count), the distribution of passes and stop codes,
 the share of rows refined, in holdout mode the hold-out MSE of both, and the card's name and power limit.  ``--joint`` adds
 the joint call (mmf_fit_forecast_arma_joint_f32, beta estimated with (phi, theta)) to the alternation, with its ms per
-call and per pass, passes, stops, share refined and hold-out MSE.
+call and per pass, passes, stops, share refined and hold-out MSE.  ``--ml`` adds the exact-likelihood call
+(mmf_fit_forecast_arma_ml_f32, which runs the CSS call and refines it) the same way, its ms per pass being its extra time
+over the CSS call divided by its mean ML pass count.
 
-    python scripts/bench_arma_css.py [--series 1000000] [--steps 3] [--rounds 3] [--shapes ...] [--joint] [--out FILE]
+    python scripts/bench_arma_css.py [--series 1000000] [--steps 3] [--rounds 3] [--shapes ...] [--joint] [--ml]
+                                     [--out FILE]
 """
 import argparse
 import json
@@ -44,6 +47,7 @@ def main():
     ap.add_argument("--gaps", default="0,0.001")
     ap.add_argument("--orders", default=",".join(ORDERS))
     ap.add_argument("--joint", action="store_true")
+    ap.add_argument("--ml", action="store_true")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     name, limit = card()
@@ -66,10 +70,13 @@ def main():
                 css_call = lambda: eng.fit_forecast_arma(yf, p, q, d, ps, npred, estimator="css")  # noqa: E731
                 joint_call = lambda: eng.fit_forecast_arma(yf, p, q, d, ps, npred, estimator="css",  # noqa: E731
                                                            joint_beta=True)
+                ml_call = lambda: eng.fit_forecast_arma(yf, p, q, d, ps, npred, estimator="ml")  # noqa: E731
                 hr_call(), css_call()
                 if args.joint:
                     joint_call()
-                t_hr, t_css, t_joint = [], [], []
+                if args.ml:
+                    ml_call()
+                t_hr, t_css, t_joint, t_ml = [], [], [], []
                 for _ in range(args.rounds):
                     ms, hr = timed(hr_call, args.steps)
                     t_hr.append(ms)
@@ -78,6 +85,9 @@ def main():
                     if args.joint:
                         ms, jt = timed(joint_call, args.steps)
                         t_joint.append(ms)
+                    if args.ml:
+                        ms, ml = timed(ml_call, args.steps)
+                        t_ml.append(ms)
                 g = (cs["css_stop"] > 0).cpu().numpy()
                 it = cs["iters"].cpu().numpy()[g]
                 stop = cs["css_stop"].cpu().numpy()[g]
@@ -99,6 +109,16 @@ def main():
                                joint_stops=np.bincount(jt["css_stop"].cpu().numpy()[g], minlength=4)[1:].tolist())
                     rec["joint_ms_per_pass"] = (rec["joint_ms"] - rec["hr_ms"]) / max(rec["joint_iters_mean"], 1.0)
                     arms += (("joint", jt),)
+                if args.ml:
+                    itm = ml["iters"].cpu().numpy()[g]
+                    rec.update(ml_ms=float(np.median(t_ml)),
+                               ml_refined=float(((ml["phi"] != cs["phi"]).any(1) | (ml["theta"] != cs["theta"]).any(1))
+                                                .float().mean()),
+                               ml_iters_mean=float(itm.mean()) if itm.size else 0.0,
+                               ml_iters_pct=[float(v) for v in np.percentile(itm, [50, 90, 100])] if itm.size else [],
+                               ml_stops=np.bincount(ml["ml_stop"].cpu().numpy()[g], minlength=4).tolist())
+                    rec["ml_ms_per_pass"] = (rec["ml_ms"] - rec["css_ms"]) / max(rec["ml_iters_mean"], 1.0)
+                    arms += (("ml", ml),)
                 if mode == "holdout":
                     yh = yg[:, t_fit:t].float()
                     for k, r in arms:

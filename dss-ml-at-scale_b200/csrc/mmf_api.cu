@@ -552,7 +552,8 @@ struct Tally {
 // arima_select_kernel; their d = 0 call (arima->d == 0) fits y itself with the mmf_plan_design plan; (p, d, q) selections
 // (hsel, with asel) add arma_select_kernel behind it.  ARMA calls (arma, with ar) run arma_kernel behind ar_kernel
 // (d = 0, no arima) or arima_kernel; CSS calls (css, with arma) add arma_css_kernel behind arma_kernel, joint calls (joint,
-// with css) arma_joint_kernel in its place, ML calls (ml, with css) arma_ml_kernel behind arma_css_kernel.  Refit stages of a (p, d, q) selection (refit, with ar, arima, arma and css)
+// with css) arma_joint_kernel in its place, ML calls (ml, with css) arma_ml_kernel behind arma_css_kernel, Kalman-predictor
+// calls (kf, with ml) arma_kf_kernel behind arma_ml_kernel.  Refit stages of a (p, d, q) selection (refit, with ar, arima, arma and css)
 // run the fit of their d, refit_list_kernel and arma_css_list_kernel (joint: arma_joint_list_kernel).
 struct Call {
   const float* y = nullptr;
@@ -575,6 +576,7 @@ struct Call {
   std::optional<CssArgs> css;
   std::optional<JointArgs> joint;
   std::optional<MlArgs> ml;
+  std::optional<KfArgs> kf;
   std::optional<RefitArgs> refit;
 
   // the same call on the rows from `off` on: every per-row output advanced by `off` rows (null stays null)
@@ -623,6 +625,7 @@ struct Call {
       c.ml->stop = at(ml->stop, 1);
       c.ml->iters = at(ml->iters, 1);
     }
+    if (kf) c.kf->se = at(kf->se, kf->ld_se);
     if (refit) { c.refit->choice_d = at(refit->choice_d, 1); c.refit->choice_q = at(refit->choice_q, 1); }
     return c;
   }
@@ -770,6 +773,19 @@ int run_device_slab(mmf_ctx* ctx, const Plan& plan, const Call& c, int64_t n, Ta
           CU_TRY(launch_arma_ml(d, a, *c.ar, mh, *c.arma, *c.ml, s));
           ++t.launches;
         }
+        if (c.kf) {
+          if (c.kf->se) {            // every row's se of the library's predictor; arma_kf_kernel overwrites its rows
+            ArimaSeArgs sa{};
+            sa.y = c.y; sa.ld_y = c.ld_y; sa.t_fit = mh.t_fit; sa.diff_order = mh.d;
+            sa.phi = c.ar->phi; sa.order = c.ar->order; sa.theta = c.arma->theta; sa.ma_order = c.arma->ma_order;
+            sa.sigma = c.ar->sigma; sa.pred_start = c.pred_start; sa.n_pred = c.n_pred;
+            sa.out = c.kf->se; sa.ld_se = c.kf->ld_se; sa.n = n;
+            CU_TRY(launch_arima_se(sa, ctx->sm_count, s));
+            ++t.launches;
+          }
+          CU_TRY(launch_arma_kf(d, a, *c.ar, mh, *c.arma, *c.kf, s));
+          ++t.launches;
+        }
       }
     }
   }
@@ -827,11 +843,14 @@ int run_device(mmf_ctx* ctx, const Plan& slab_plan, const std::vector<Stage>& st
                uint32_t* slab_pending = nullptr) {
   const cudaStream_t s = ctx->stream;
   const int64_t slab = slab_rows(slab_plan, n);
-  // CSS and joint calls read the HR (phi, theta, ma_order) back: what the caller did not ask for goes to per-slab scratch
+  // CSS and joint calls read the HR (phi, theta, ma_order) back: what the caller did not ask for goes to per-slab scratch;
+  // Kalman-predictor calls with standard errors also read order and sigma back
   const Call& c0 = stages[0].call;
+  const bool kf_se = c0.kf && c0.kf->se != nullptr;
   float* hr = nullptr;
-  if (c0.css && (c0.ar->phi == nullptr || c0.arma->theta == nullptr || c0.arma->ma_order == nullptr)) {
-    const size_t per_row = (MMF_AR_MAX + MMF_MA_MAX + 1) * sizeof(float);
+  if (c0.css && (c0.ar->phi == nullptr || c0.arma->theta == nullptr || c0.arma->ma_order == nullptr ||
+                 (kf_se && (c0.ar->order == nullptr || c0.ar->sigma == nullptr)))) {
+    const size_t per_row = (MMF_AR_MAX + MMF_MA_MAX + 1 + (kf_se ? 2 : 0)) * sizeof(float);
     int rc = grow((void**)&ctx->d_css_hr, &ctx->css_hr_cap, (size_t)slab * per_row);
     if (rc != MMF_OK) return rc;
     hr = ctx->d_css_hr;
@@ -853,6 +872,9 @@ int run_device(mmf_ctx* ctx, const Plan& slab_plan, const std::vector<Stage>& st
         if (!c.ar->phi) c.ar->phi = hr;
         if (!c.arma->theta) c.arma->theta = hr + (size_t)slab * MMF_AR_MAX;
         if (!c.arma->ma_order) c.arma->ma_order = reinterpret_cast<int32_t*>(hr + (size_t)slab * (MMF_AR_MAX + MMF_MA_MAX));
+        if (kf_se && !c.ar->order)
+          c.ar->order = reinterpret_cast<int32_t*>(hr + (size_t)slab * (MMF_AR_MAX + MMF_MA_MAX + 1));
+        if (kf_se && !c.ar->sigma) c.ar->sigma = hr + (size_t)slab * (MMF_AR_MAX + MMF_MA_MAX + 2);
       }
       if (rs != nullptr) {
         auto or_scratch = [](auto*& p, int32_t* w) { if (!p) p = reinterpret_cast<decltype(p + 0)>(w); };
@@ -1638,7 +1660,8 @@ static int arma_call(mmf_ctx* ctx, const char* name, const float* y, int64_t n, 
                      int32_t diff_order, int32_t ma_order, int32_t long_order, int32_t pred_start, int32_t n_pred,
                      float* out_pred, int64_t ld_out, float* out_phi, float* out_theta, int32_t* out_order,
                      int32_t* out_ma_order, float* out_sigma, int32_t* out_status, mmf_stats* stats,
-                     const CssArgs* css, const JointArgs* joint = nullptr, const MlArgs* ml = nullptr) {
+                     const CssArgs* css, const JointArgs* joint = nullptr, const MlArgs* ml = nullptr,
+                     const KfArgs* kf = nullptr) {
   if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
   GrowScope grow_scope(ctx);
   if (n < 0) return fail(MMF_E_INVALID, "n < 0");
@@ -1661,6 +1684,8 @@ static int arma_call(mmf_ctx* ctx, const char* name, const float* y, int64_t n, 
     return fail(MMF_E_INVALID, "long_order=%d outside {0} and [%d,%d]", long_order, lmin, MMF_HR_LONG_MAX);
   if (ld_y < T) return fail(MMF_E_INVALID, "ld_y=%lld < t_fit=%d", (long long)ld_y, T);
   if (int rc = check_window(pred_start, n_pred, n_rows, ld_out)) return rc;
+  if (kf && kf->se && kf->ld_se < n_pred)
+    return fail(MMF_E_INVALID, "ld_se=%lld < n_pred=%d", (long long)kf->ld_se, n_pred);
   if (stats) memset(stats, 0, sizeof(*stats));
   if (n == 0) return MMF_OK;
   CU_TRY(cudaSetDevice(ctx->device));
@@ -1668,7 +1693,7 @@ static int arma_call(mmf_ctx* ctx, const char* name, const float* y, int64_t n, 
                                  css ? css->css_start : nullptr, css ? css->css : nullptr, css ? css->css_stop : nullptr,
                                  css ? css->iters : nullptr, joint ? joint->beta : nullptr,
                                  ml ? ml->loglik_start : nullptr, ml ? ml->loglik : nullptr, ml ? ml->stop : nullptr,
-                                 ml ? ml->iters : nullptr}))
+                                 ml ? ml->iters : nullptr, kf ? kf->se : nullptr}))
     return fail(MMF_E_UNSUPPORTED, "%s takes device buffers only", name);
   Call c = plain_call(y, ld_y, pred_start, n_pred, out_pred, ld_out, out_status);
   c.ar = ar_args(ar_order, out_phi, out_order, out_sigma, pl);
@@ -1681,6 +1706,7 @@ static int arma_call(mmf_ctx* ctx, const char* name, const float* y, int64_t n, 
   if (css) c.css = *css;
   if (joint) c.joint = *joint;
   if (ml) c.ml = *ml;
+  if (kf) c.kf = *kf;
   return enqueue(ctx, pl, {{&pl, c}}, n, stats);
 }
 
@@ -1747,6 +1773,28 @@ int mmf_fit_forecast_arma_ml_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_
   return arma_call(ctx, "mmf_fit_forecast_arma_ml_f32", y, n, ld_y, ar_order, diff_order, ma_order, long_order,
                    pred_start, n_pred, out_pred, ld_out, out_phi, out_theta, out_order, out_ma_order, out_sigma,
                    out_status, stats, &css, nullptr, &ml);
+}
+
+int mmf_fit_forecast_arma_ml_kf_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
+                                    int32_t diff_order, int32_t ma_order, int32_t long_order, int32_t max_iter,
+                                    int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out, float* out_phi,
+                                    float* out_theta, int32_t* out_order, int32_t* out_ma_order, float* out_sigma,
+                                    int32_t* out_status, float* out_loglik_start, float* out_loglik,
+                                    int32_t* out_ml_stop, int32_t* out_iters, float* out_se, int64_t ld_se,
+                                    mmf_stats* stats) {
+  if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
+  if (max_iter < 0 || max_iter > MMF_CSS_ITER_MAX)
+    return fail(MMF_E_INVALID, "max_iter=%d outside [0,%d]", max_iter, MMF_CSS_ITER_MAX);
+  CssArgs css{};                           // the ML call's stages, then the predictor
+  css.max_iter = max_iter == 0 ? MMF_CSS_ITER_DEFAULT : max_iter;
+  MlArgs ml{};
+  ml.max_iter = css.max_iter;
+  ml.loglik_start = out_loglik_start; ml.loglik = out_loglik; ml.stop = out_ml_stop; ml.iters = out_iters;
+  KfArgs kf{};
+  kf.se = out_se; kf.ld_se = ld_se;
+  return arma_call(ctx, "mmf_fit_forecast_arma_ml_kf_f32", y, n, ld_y, ar_order, diff_order, ma_order, long_order,
+                   pred_start, n_pred, out_pred, ld_out, out_phi, out_theta, out_order, out_ma_order, out_sigma,
+                   out_status, stats, &css, nullptr, &ml, &kf);
 }
 
 // ---- standard errors of the ARIMA-family forecasts (DESIGN.md section 2 item 15) ---------------------------------------

@@ -331,6 +331,16 @@ struct MlArgs {
 cudaError_t launch_arma_ml(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
                            const ArmaArgs& hr, const MlArgs& ml, cudaStream_t s);
 
+// the Kalman predictor of the ML fit (arma_kf.cu, DESIGN.md section 2 item 20): arma_kf_kernel runs behind arma_ml_kernel
+// in the same slab (and behind arima_se_kernel over the slab's rows when se is given), reads the shipped (phi, theta)
+// and the gated rows as arma_ml_kernel does, and overwrites pred (and se) of every gated row whose P_0 solves there
+struct KfArgs {
+  float* se;                              // nullable [n, ld_se]: the standard errors of the predictions
+  int64_t ld_se;
+};
+cudaError_t launch_arma_kf(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
+                           const ArmaArgs& hr, const KfArgs& kf, cudaStream_t s);
+
 // the refit of a (p, d, q) selection's winners (DESIGN.md section 2 item 18): one stage per listed d behind the
 // selection's stages, on that d's fit.  refit_list_kernel lists the slab's rows whose winner is (p, d, q >= 1) and writes
 // the refit outputs of the rows no refit kernel touches; arma_css_list_kernel / arma_joint_list_kernel run the fixed-order

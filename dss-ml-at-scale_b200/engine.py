@@ -578,7 +578,8 @@ class ForecastEngine:
 
     def fit_forecast_arma(self, y, ar_order: int, ma_order: int, diff_order: int = 0, pred_start: int = 0,
                           n_pred: int | None = None, long_order: int = 0, want_stats: bool = False,
-                          want_se: bool = False, estimator: str = "hr", max_iter: int = 0, joint_beta: bool = False):
+                          want_se: bool = False, estimator: str = "hr", max_iter: int = 0, joint_beta: bool = False,
+                          predictor: str = "recursion"):
         """Regression with ARIMA(``ar_order``, ``diff_order``, ``ma_order``) errors (``mmf_fit_forecast_arma_f32``,
         DESIGN.md section 2 item 13): the plain fit (on the differenced series and design for ``diff_order`` >= 1),
         then Hannan-Rissanen on its residuals -- a long AR of order ``long_order`` (0: the default) gives innovation
@@ -611,10 +612,24 @@ class ForecastEngine:
         ``max_iter`` (R's ``arima(method="CSS-ML")`` on the differenced series).  A series that accepts no step keeps the
         CSS outputs bit for bit; ``sigma`` is the ML estimate for every gated series.  The result adds ``loglik_start``
         (the exact log-likelihood at the CSS estimate), ``loglik`` (at the shipped one), ``ml_stop`` (the CSS codes) and
-        ``iters`` (ML passes run).  ``want_se=True`` takes the ML (phi, theta, sigma).  Not with ``joint_beta=True``."""
+        ``iters`` (ML passes run).  ``want_se=True`` takes the ML (phi, theta, sigma).  Not with ``joint_beta=True``.
+
+        ``predictor="kalman"`` with ``estimator="ml"`` (``mmf_fit_forecast_arma_ml_kf_f32``, DESIGN.md section 2 item
+        20) predicts every gated series whose stationary start solves at the shipped (phi, theta) with the Kalman filter
+        of the exact likelihood, as SARIMAX's ``predict()`` / ``get_forecast()`` do: one step ahead in sample from the
+        observed rows before each row, the dynamic forecast beyond t_fit.  Every other output, and every row the filter
+        does not cover, is ``estimator="ml"``'s bit for bit.  ``want_se=True`` takes the call's own standard errors
+        (the variance of this predictor's error, gaps included).  The default ``predictor="recursion"`` is the
+        library's recursion."""
         import torch
         if estimator not in ("hr", "css", "ml"):
             raise ValueError(f"estimator must be 'hr' or 'css' (or 'ml' for the exact likelihood), got {estimator!r}")
+        if predictor not in ("recursion", "kalman"):
+            raise ValueError(f"predictor must be 'recursion' or 'kalman', got {predictor!r}")
+        kalman = predictor == "kalman"
+        if kalman and estimator != "ml":
+            raise ValueError(f"predictor='kalman' needs estimator='ml' (the filter of the exact-likelihood fit), "
+                             f"got estimator={estimator!r}")
         ml = estimator == "ml"
         css = estimator == "css" or ml
         if not css and int(max_iter) != 0:
@@ -650,7 +665,16 @@ class ForecastEngine:
             css_end = torch.empty(n, device=dev, dtype=torch.float32)
             css_stop = torch.empty(n, device=dev, dtype=torch.int32)
             iters = torch.empty(n, device=dev, dtype=torch.int32)
-            if ml:
+            if kalman:
+                se = torch.empty((n, n_pred), device=dev, dtype=torch.float32) if want_se else None
+                N.check(self._lib.mmf_fit_forecast_arma_ml_kf_f32(
+                    self._h, yp, n, ld_y, int(ar_order), int(diff_order), int(ma_order), int(long_order),
+                    int(max_iter), int(pred_start), int(n_pred), out.data_ptr(), out.stride(0), phi.data_ptr(),
+                    theta.data_ptr(), order.data_ptr(), ma.data_ptr(), sigma.data_ptr(), status.data_ptr(),
+                    css_start.data_ptr(), css_end.data_ptr(), css_stop.data_ptr(), iters.data_ptr(),
+                    se.data_ptr() if se is not None else None, se.stride(0) if se is not None else 0,
+                    C.byref(st) if st is not None else None))
+            elif ml:
                 N.check(self._lib.mmf_fit_forecast_arma_ml_f32(
                     self._h, yp, n, ld_y, int(ar_order), int(diff_order), int(ma_order), int(long_order),
                     int(max_iter), int(pred_start), int(n_pred), out.data_ptr(), out.stride(0), phi.data_ptr(),
@@ -686,7 +710,9 @@ class ForecastEngine:
             res.update(css_start=css_start, css=css_end, css_stop=css_stop, iters=iters)
             if joint_beta:
                 res["beta"] = beta
-        if want_se:
+        if want_se and kalman:
+            res["se"] = se
+        elif want_se:
             self._add_se(res, y, t_fit, pred_start, n_pred, int(diff_order))
         if st is not None:
             self.launches += st.kernel_launches

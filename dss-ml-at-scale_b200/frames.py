@@ -339,7 +339,7 @@ def _host(x):
 
 
 def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, interval=False, ar=None, diff=None,
-                 ma=None, want_se=False, estimator=None, joint_beta=False, refit=None):
+                 ma=None, want_se=False, estimator=None, joint_beta=False, refit=None, predictor=None):
     """Run the engine over every bucket: yields (bucket, out_days, n_pred, y_host, pred_host, se_host or None).
     ``interval``: prediction standard errors too (``fit_forecast_se``), one call per calendar bucket.
     ``ar``: regression with AR(ar) errors (``fit_forecast_ar``), one call per calendar bucket; a tuple of orders
@@ -354,7 +354,9 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
     ``estimator``: the fixed-order ARIMA(p, d, q) call's estimator (None: the engine's default, Hannan-Rissanen);
     ``joint_beta``: with ``estimator="css"``, beta estimated jointly with (phi, theta).
     ``refit``: with candidate MA orders, the winner refit by conditional least squares (``joint_beta`` with it: beta
-    jointly)."""
+    jointly).
+    ``predictor``: with ``estimator="ml"``, "kalman" predicts with the filter of the exact likelihood (None: the
+    recursion)."""
     se_kw = {"want_se": True} if want_se else {}
     if interval and select is not None:
         raise ValueError("interval= is not offered with select= (model selection returns point forecasts)")
@@ -382,6 +384,8 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
             est_kw = {"estimator": estimator} if estimator is not None else {}
             if joint_beta:
                 est_kw["joint_beta"] = True
+            if predictor is not None:
+                est_kw["predictor"] = predictor
             res = eng.fit_forecast_arma(yd, ar, ma, diff or 0, pred_start, n_pred, **se_kw, **est_kw)
             pred, se = _host(res["pred"]), (_host(res["se"]) if want_se else None)
         elif isinstance(diff, tuple):
@@ -574,6 +578,19 @@ def _refit(refit, ma, estimator, select, interval):
     return refit
 
 
+def _predictor(predictor, estimator):
+    """validated ``predictor=``: None (the recursion, as before), "recursion", or "kalman" with ``estimator="ml"``
+    (DESIGN.md section 2 item 20)"""
+    if predictor is None:
+        return None
+    if predictor not in ("recursion", "kalman"):
+        raise ValueError(f"predictor must be 'recursion' or 'kalman', got {predictor!r}")
+    if predictor == "kalman" and estimator != "ml":
+        raise ValueError(f"predictor='kalman' needs estimator='ml' (the filter of the exact-likelihood fit), "
+                         f"got estimator={estimator!r}")
+    return predictor
+
+
 def _joint_beta(joint_beta, estimator, refit=None):
     """validated ``joint_beta=``: True needs ``estimator="css"`` (DESIGN.md section 2 item 17) or ``refit="css"`` (item
     18)"""
@@ -704,7 +721,7 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
                     freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                     engine: ForecastEngine | None = None, pack: str = "host", select=None,
                     null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None, ma=None,
-                    conf_int=None, estimator=None, joint_beta=False, refit=None) -> pd.DataFrame:
+                    conf_int=None, estimator=None, joint_beta=False, refit=None, predictor=None) -> pd.DataFrame:
     """Fit + forecast every group in ``pdf``; returns ``tuning_schema`` rows
     (keys..., Date, Demand, Demand_Fitted), groups in key order, dates ascending.
 
@@ -772,7 +789,10 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     unchanged, ``conf_int=`` works as above.  ``estimator=None`` (or ``"hr"``) leaves everything as it was.  Refused
     without ``ma=``, with candidate MA orders, ``select=`` or ``interval=``.  ``estimator="ml"`` refines that CSS
     estimate by the exact Gaussian likelihood (``ForecastEngine.fit_forecast_arma(..., estimator="ml")``, DESIGN.md
-    section 2 item 19), with the same arguments, refusals, schema and ``conf_int=``.
+    section 2 item 19), with the same arguments, refusals, schema and ``conf_int=``.  ``predictor="kalman"`` with
+    ``estimator="ml"`` predicts with that likelihood's Kalman filter (``ForecastEngine.fit_forecast_arma(...,
+    predictor="kalman")``, DESIGN.md section 2 item 20: SARIMAX's ``predict()`` / ``get_forecast()``), ``conf_int=``
+    bands from its own standard errors; refused with any other estimator.
     ``joint_beta=True`` with ``estimator="css"`` estimates the design's coefficients jointly with (phi, theta)
     (``ForecastEngine.fit_forecast_arma(..., joint_beta=True)``, DESIGN.md section 2 item 17: regression with ARIMA errors
     as SARIMAX fits it, by the conditional likelihood); schema unchanged, ``conf_int=`` works as above.  Refused without
@@ -789,6 +809,7 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     z = _z_of(interval)
     cz = _conf_z(conf_int, ar, select, interval)
     est = _estimator(estimator, ma, select, interval)
+    pr = _predictor(predictor, est)
     ref = _refit(refit, ma, est, select, interval)
     jb = _joint_beta(joint_beta, est, ref)
     if ma is None:
@@ -805,7 +826,7 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     parts, lengths = [], []
     for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
                                                               pack == "device", z is not None, ar, diff, ma,
-                                                              cz is not None, est, jb, ref):
+                                                              cz is not None, est, jb, ref, pr):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n), n_pred)
         # key columns keep the dtype they came in with (no per-row string inference on N x T values)
@@ -897,7 +918,7 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
                    freq="W-MON", horizon=FORECAST_HORIZON, mode="holdout", design="trend_season_exog",
                    engine: ForecastEngine | None = None, pack: str = "host", select=None,
                    null_keys_on_gaps: bool = False, interval=None, ar=None, diff=None, ma=None,
-                   conf_int=None, estimator=None, joint_beta=False, refit=None):
+                   conf_int=None, estimator=None, joint_beta=False, refit=None, predictor=None):
     """Arrow ``Table``/``RecordBatch`` in -> Arrow ``Table`` with ``tuning_schema`` out (the ``mapInArrow``
     flavour of the boundary).  No pandas frame of the rows on either side: keys are dictionary-encoded on the way
     in and expanded from a dictionary on the way out, dates and values are NumPy views of Arrow buffers.
@@ -906,7 +927,8 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     ``forecast_groups``; ``diff=d`` with ``ar=p`` fits ARIMA(p, d, 0) errors as there, and ``ma=q`` ARIMA(p, d, q); tuples of ``ar``, ``diff`` and
     ``ma`` choose (p, d, q) per series.  ``conf_int=level`` adds the same two columns for those forecasts, and
     ``estimator="css"`` (or ``"ml"``) refines a fixed ``ma=q``'s estimate and ``joint_beta=True`` adds beta to it, and ``refit="css"``
-    refits the selection's winners (with ``joint_beta=True``: beta jointly), as in ``forecast_groups``."""
+    refits the selection's winners (with ``joint_beta=True``: beta jointly), and ``predictor="kalman"`` with
+    ``estimator="ml"`` predicts with the Kalman filter, as in ``forecast_groups``."""
     import pyarrow as pa
 
     if isinstance(table, pa.RecordBatch):
@@ -916,6 +938,7 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     z = _z_of(interval)
     cz = _conf_z(conf_int, ar, select, interval)
     est = _estimator(estimator, ma, select, interval)
+    pr = _predictor(predictor, est)
     ref = _refit(refit, ma, est, select, interval)
     jb = _joint_beta(joint_beta, est, ref)
     if ma is None:
@@ -929,7 +952,7 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     parts, lengths = [], []
     for b, out_days, n_pred, y_host, pred, se in _fit_buckets(buckets, eng, freq, horizon, mode, design, select,
                                                               pack == "device", z is not None, ar, diff, ma,
-                                                              cz is not None, est, jb, ref):
+                                                              cz is not None, est, jb, ref, pr):
         n = y_host.shape[0]
         row_of = np.repeat(np.arange(n, dtype=np.int32), n_pred)
         cols = []

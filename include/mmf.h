@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define MMF_VERSION 115          /* 0.1.15 */
+#define MMF_VERSION 116          /* 0.1.16 */
 #define MMF_P 16                 /* design columns (zero-pad narrower designs) */
 #define MMF_PIVOT_TOL 1e-3f      /* per-series relative Cholesky pivot threshold */
 #define MMF_CAL_TOL 1e-10        /* aliasing threshold on the float64 calendar Gram */
@@ -416,7 +416,8 @@ int mmf_fit_forecast_arma_joint_f32(mmf_ctx* ctx, const float* y, int64_t n, int
  *   solve fails counts as one that fails the step-down test (lambda <- 10 lambda, no pass).
  * Outputs: a gated series that accepted no step keeps the CSS call's pred, phi, theta, order, ma_order and status bit for
  * bit; one that did gets the recursion and level integration of the HR call with the shipped (phi, theta) (the library's
- * predictor, not the Kalman filter's, so mmf_arima_se_f32 applies unchanged).  For every gated series sigma = sigma at
+ * predictor, not the Kalman filter's, so mmf_arima_se_f32 applies unchanged; mmf_fit_forecast_arma_ml_kf_f32 predicts with
+ * the filter).  For every gated series sigma = sigma at
  * the shipped point.  out_loglik_start [n] (loglik at x0), out_loglik [n] (at the shipped point, >= out_loglik_start),
  * out_ml_stop [n] (the CSS call's codes, 0 not refined) and out_iters [n] (passes run) are nullable.  A gated series whose
  * x0 fails the P_0 solve keeps every CSS output, with NaN, NaN, 0, 0.  Series that fail the HR gate and empty series get
@@ -431,6 +432,39 @@ int mmf_fit_forecast_arma_ml_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_
                                  float* out_theta, int32_t* out_order, int32_t* out_ma_order, float* out_sigma,
                                  int32_t* out_status, float* out_loglik_start, float* out_loglik, int32_t* out_ml_stop,
                                  int32_t* out_iters, mmf_stats* stats);
+
+/* ---- the Kalman predictor of the exact-likelihood fit (DESIGN.md section 2 item 20) -----------------------------------
+ * mmf_fit_forecast_arma_ml_kf_f32: mmf_fit_forecast_arma_ml_f32 with the same arguments, then the predictions of every
+ * covered series (a gated series whose P_0 solves at the shipped (phi, theta), including one that accepted no ML step)
+ * from the Kalman filter of that call's model, evaluated in float64 at the shipped fp32 (phi, theta):
+ *   e: a_s the filter's predicted state of z-row s (the residual of y for d = 0, of z' for d >= 1), from a = 0 and P_0;
+ *   for s < T it uses the observed rows before s only (a missing row predicted and not updated, as in the likelihood),
+ *   for s >= T it is the dynamic forecast a_{T+h} = T^h a_T.  The prediction of e_s is a_{s,1};
+ *   levels: zhat_s = fitted_s + a_{s,1} (fp32), integrated to levels as mmf_fit_forecast_arma_f32 integrates its zhat
+ *   (a missing level filled with its prediction).  This is the ML call's pred with the recursion's prediction replaced;
+ *   out_se [n, ld_se] (nullable; ld_se >= n_pred): se_t = sigma sqrt(Var(y_t - yhat_t)) with the fitted model taken as
+ *   true and no estimation uncertainty (mmf_arima_se_f32's definition applied to this predictor).  The error state is
+ *   (alpha_s - a_s, the errors of the d previous filled levels); its alpha block is the filter's P, and its full
+ *   covariance moves with the filter (alpha - a <- (T - K Z)(alpha - a) + R eps on an update, T (alpha - a) + R eps on a
+ *   missing row; the level error of row t is Z (alpha_s - a_s) plus the integration of the previous level errors, 0
+ *   where y_t is observed).  On a gap-free fit window se = sigma sqrt(F_s) in sample.  NaN where mmf_arima_se_f32 gives
+ *   NaN (rows t < d, a level chain without an anchor), +Inf where the float64 variance overflowed.
+ * Every other output (phi, theta, order, ma_order, sigma, status, loglik_start, loglik, ml_stop, iters) is the ML call's
+ * bit for bit on every row.  Series the predictor does not cover (HR-gate fallbacks, empty series, a P_0 that fails at
+ * the shipped point) keep every output of the ML call bit for bit, and their out_se is mmf_arima_se_f32 of the call's
+ * outputs bit for bit.  Otherwise the contract of mmf_fit_forecast_arma_ml_f32 (plans, refusals with max_iter checked
+ * first, device buffers only, any ld_out, enqueue-only unless `stats`, mmf_config.kernel and assume_finite); ld_se <
+ * n_pred with out_se given is MMF_E_INVALID.  Scratch: per slab, 60 B per row when out_se is given and out_phi,
+ * out_theta, out_order, out_ma_order or out_sigma is NULL (52 B as the CSS call otherwise).
+ * replaces: SARIMAX predict() / get_forecast() of the reference's fitted per-group model (02:453-457, 484-488): the
+ * Kalman filter's one-step predictions in sample, its dynamic forecast beyond, and their standard errors. */
+int mmf_fit_forecast_arma_ml_kf_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t ar_order,
+                                    int32_t diff_order, int32_t ma_order, int32_t long_order, int32_t max_iter,
+                                    int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out, float* out_phi,
+                                    float* out_theta, int32_t* out_order, int32_t* out_ma_order, float* out_sigma,
+                                    int32_t* out_status, float* out_loglik_start, float* out_loglik,
+                                    int32_t* out_ml_stop, int32_t* out_iters, float* out_se, int64_t ld_se,
+                                    mmf_stats* stats);
 
 /* ---- (p, d) selection by hold-out MSE on levels (DESIGN.md section 2 item 12) -----------------------------------------
  * mmf_fit_select_arima_f32: orders [n_orders] (1 .. MMF_ARSEL_MAX_CAND ascending distinct values in [0, MMF_AR_MAX]) and

@@ -7,9 +7,11 @@ the share of rows refined, in holdout mode the hold-out MSE of both, and the car
 the joint call (mmf_fit_forecast_arma_joint_f32, beta estimated with (phi, theta)) to the alternation, with its ms per
 call and per pass, passes, stops, share refined and hold-out MSE.  ``--ml`` adds the exact-likelihood call
 (mmf_fit_forecast_arma_ml_f32, which runs the CSS call and refines it) the same way, its ms per pass being its extra time
-over the CSS call divided by its mean ML pass count.
+over the CSS call divided by its mean ML pass count.  ``--kalman`` (with ``--ml``) adds the ML call with the Kalman
+predictor (mmf_fit_forecast_arma_ml_kf_f32): its ms, the predictor stage's cost (its extra time over the ML call) in
+total and per series, and its hold-out MSE.
 
-    python scripts/bench_arma_css.py [--series 1000000] [--steps 3] [--rounds 3] [--shapes ...] [--joint] [--ml]
+    python scripts/bench_arma_css.py [--series 1000000] [--steps 3] [--rounds 3] [--shapes ...] [--joint] [--ml] [--kalman]
                                      [--out FILE]
 """
 import argparse
@@ -48,6 +50,7 @@ def main():
     ap.add_argument("--orders", default=",".join(ORDERS))
     ap.add_argument("--joint", action="store_true")
     ap.add_argument("--ml", action="store_true")
+    ap.add_argument("--kalman", action="store_true")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     name, limit = card()
@@ -71,12 +74,16 @@ def main():
                 joint_call = lambda: eng.fit_forecast_arma(yf, p, q, d, ps, npred, estimator="css",  # noqa: E731
                                                            joint_beta=True)
                 ml_call = lambda: eng.fit_forecast_arma(yf, p, q, d, ps, npred, estimator="ml")  # noqa: E731
+                kf_call = lambda: eng.fit_forecast_arma(yf, p, q, d, ps, npred, estimator="ml",  # noqa: E731
+                                                        predictor="kalman")
                 hr_call(), css_call()
                 if args.joint:
                     joint_call()
                 if args.ml:
                     ml_call()
-                t_hr, t_css, t_joint, t_ml = [], [], [], []
+                if args.kalman:
+                    kf_call()
+                t_hr, t_css, t_joint, t_ml, t_kf = [], [], [], [], []
                 for _ in range(args.rounds):
                     ms, hr = timed(hr_call, args.steps)
                     t_hr.append(ms)
@@ -88,6 +95,9 @@ def main():
                     if args.ml:
                         ms, ml = timed(ml_call, args.steps)
                         t_ml.append(ms)
+                    if args.kalman:
+                        ms, kf = timed(kf_call, args.steps)
+                        t_kf.append(ms)
                 g = (cs["css_stop"] > 0).cpu().numpy()
                 it = cs["iters"].cpu().numpy()[g]
                 stop = cs["css_stop"].cpu().numpy()[g]
@@ -119,6 +129,11 @@ def main():
                                ml_stops=np.bincount(ml["ml_stop"].cpu().numpy()[g], minlength=4).tolist())
                     rec["ml_ms_per_pass"] = (rec["ml_ms"] - rec["css_ms"]) / max(rec["ml_iters_mean"], 1.0)
                     arms += (("ml", ml),)
+                if args.kalman:
+                    rec.update(kf_ms=float(np.median(t_kf)))
+                    rec["kf_stage_ms"] = rec["kf_ms"] - rec["ml_ms"]
+                    rec["kf_stage_ns_per_series"] = rec["kf_stage_ms"] * 1e6 / args.series
+                    arms += (("kf", kf),)
                 if mode == "holdout":
                     yh = yg[:, t_fit:t].float()
                     for k, r in arms:

@@ -36,7 +36,8 @@ EXPORTS = (
     "mmf_fit_forecast_f32", "mmf_fit_forecast_int", "mmf_fit_forecast_se_f32", "mmf_fit_forecast_ar_f32",
     "mmf_fit_select_ar_f32", "mmf_plan_arima", "mmf_fit_forecast_arima_f32", "mmf_fit_select_arima_f32",
     "mmf_fit_forecast_arma_f32", "mmf_fit_forecast_arma_css_f32", "mmf_fit_forecast_arma_joint_f32",
-    "mmf_fit_forecast_arma_ml_f32", "mmf_fit_forecast_arma_ml_kf_f32", "mmf_fit_select_arma_f32", "mmf_fit_select_arma_css_f32", "mmf_fit_select_arma_joint_f32", "mmf_arima_se_f32",
+    "mmf_fit_forecast_arma_ml_f32", "mmf_fit_forecast_arma_ml_kf_f32", "mmf_fit_select_arma_f32", "mmf_fit_select_arma_css_f32", "mmf_fit_select_arma_joint_f32",
+    "mmf_fit_select_arma_ml_f32", "mmf_fit_select_arma_ml_kf_f32", "mmf_arima_se_f32",
     "mmf_plan_calendars", "mmf_fit_forecast_ragged_f32",
     "mmf_plan_backtest", "mmf_backtest_f32",
     "mmf_fit_forecast_bcast_f32", "mmf_fit_select_forecast_f32", "mmf_pack_hash_utf8", "mmf_pack_hash_i32",
@@ -174,6 +175,9 @@ def load() -> C.CDLL:
     sel_tail = [C.c_void_p] * 15 + [C.POINTER(MmfStats)]
     lib.mmf_fit_select_arma_css_f32.argtypes = sel_head + sel_tail
     lib.mmf_fit_select_arma_joint_f32.argtypes = sel_head + [C.c_void_p] + sel_tail
+    # the ML refit: the four ML outputs in the CSS outputs' place; with the predictor out_se and ld_se before stats
+    lib.mmf_fit_select_arma_ml_f32.argtypes = sel_head + sel_tail
+    lib.mmf_fit_select_arma_ml_kf_f32.argtypes = sel_head + [C.c_void_p] * 15 + [C.c_void_p, C.c_int64, C.POINTER(MmfStats)]
     lib.mmf_arima_se_f32.argtypes = [
         C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
         C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.POINTER(MmfStats),

@@ -554,7 +554,9 @@ struct Tally {
 // (d = 0, no arima) or arima_kernel; CSS calls (css, with arma) add arma_css_kernel behind arma_kernel, joint calls (joint,
 // with css) arma_joint_kernel in its place, ML calls (ml, with css) arma_ml_kernel behind arma_css_kernel, Kalman-predictor
 // calls (kf, with ml) arma_kf_kernel behind arma_ml_kernel.  Refit stages of a (p, d, q) selection (refit, with ar, arima, arma and css)
-// run the fit of their d, refit_list_kernel and arma_css_list_kernel (joint: arma_joint_list_kernel).
+// run the fit of their d, refit_list_kernel and arma_css_list_kernel (joint: arma_joint_list_kernel); with ml they add
+// refit_ml_cols_kernel and arma_ml_list_kernel, with kf arma_kf_list_kernel (kf_list), and se_pass runs arima_se_kernel
+// over the slab with the per-series d behind them; kf_only stages run the fit, the list and arma_kf_list_kernel alone.
 struct Call {
   const float* y = nullptr;
   int64_t ld_y = 0;
@@ -578,6 +580,7 @@ struct Call {
   std::optional<MlArgs> ml;
   std::optional<KfArgs> kf;
   std::optional<RefitArgs> refit;
+  bool kf_list = false, se_pass = false, kf_only = false;   // refit stages of the ML + Kalman call (DESIGN.md 4.25)
 
   // the same call on the rows from `off` on: every per-row output advanced by `off` rows (null stays null)
   Call slice(int64_t off) const {
@@ -748,9 +751,30 @@ int run_device_slab(mmf_ctx* ctx, const Plan& plan, const Call& c, int64_t n, Ta
     CU_TRY(cudaMemsetAsync(c.refit->count, 0, sizeof(uint32_t), s));
     const JointArgs jt = c.joint ? *c.joint : JointArgs{};
     CU_TRY(launch_refit_list(d, a, ma, *c.css, jt, *c.refit, s));
-    CU_TRY(c.joint ? launch_arma_joint_list(d, a, *c.ar, ma, *c.arma, *c.css, jt, *c.refit, s)
-                   : launch_arma_css_list(d, a, *c.ar, ma, *c.arma, *c.css, *c.refit, s));
-    t.launches += 2;
+    ++t.launches;
+    if (!c.kf_only) {
+      CU_TRY(c.joint ? launch_arma_joint_list(d, a, *c.ar, ma, *c.arma, *c.css, jt, *c.refit, s)
+                     : launch_arma_css_list(d, a, *c.ar, ma, *c.arma, *c.css, *c.refit, s));
+      ++t.launches;
+    }
+    if (c.ml && !c.kf_only) {       // the ML refit from the CSS refit's estimate; the ML columns of the other rows
+      CU_TRY(launch_refit_ml_cols(a, ma, *c.ml, *c.refit, s));
+      CU_TRY(launch_arma_ml_list(d, a, *c.ar, ma, *c.arma, *c.ml, *c.refit, s));
+      t.launches += 2;
+    }
+    if (c.se_pass) {                // every row's se of the library's predictor, each row at its own d, once every d's
+      ArimaSeArgs sa{};             // ML refit has run; the Kalman stages behind overwrite the rows they cover
+      sa.y = c.y; sa.ld_y = c.ld_y; sa.t_fit = ma.t_fit; sa.diffs = c.refit->choice_d;
+      sa.phi = c.ar->phi; sa.order = c.ar->order; sa.theta = c.arma->theta; sa.ma_order = c.arma->ma_order;
+      sa.sigma = c.ar->sigma; sa.pred_start = c.pred_start; sa.n_pred = c.n_pred;
+      sa.out = c.kf->se; sa.ld_se = c.kf->ld_se; sa.n = n;
+      CU_TRY(launch_arima_se(sa, ctx->sm_count, s));
+      ++t.launches;
+    }
+    if (c.kf_list) {
+      CU_TRY(launch_arma_kf_list(d, a, *c.ar, ma, *c.arma, *c.kf, *c.refit, s));
+      ++t.launches;
+    }
   } else if (c.ar) {
     CU_TRY(c.asel    ? launch_arima_select(d, a, *c.ar, ma, *c.asel, s)
            : c.arima ? launch_arima(d, a, *c.ar, ma, s)
@@ -856,10 +880,12 @@ int run_device(mmf_ctx* ctx, const Plan& slab_plan, const std::vector<Stage>& st
     hr = ctx->d_css_hr;
   }
   // selections with refit stages: the refit reads the winner back (phi, theta, order, ma_order, choice_d, choice_q), so
-  // what the caller did not ask for goes to per-slab scratch in every stage; the row list and its length live there too
+  // what the caller did not ask for goes to per-slab scratch in every stage; the row list and its length live there too.
+  // The ML + Kalman refit with standard errors also reads sigma back (the se pass and arma_kf_list_kernel)
   int32_t* rs = nullptr;
+  const bool sig_slot = stages.back().call.kf && stages.back().call.kf->se != nullptr && stages[0].call.ar->sigma == nullptr;
   if (stages.back().call.refit) {
-    const size_t words = (size_t)slab * (MMF_AR_MAX + MMF_MA_MAX + 5) + 1;
+    const size_t words = (size_t)slab * (MMF_AR_MAX + MMF_MA_MAX + 5 + (sig_slot ? 1 : 0)) + 1;
     int rc = grow((void**)&ctx->d_refit, &ctx->refit_cap, words * sizeof(int32_t));
     if (rc != MMF_OK) return rc;
     rs = ctx->d_refit;
@@ -886,6 +912,7 @@ int run_device(mmf_ctx* ctx, const Plan& slab_plan, const std::vector<Stage>& st
         int32_t* choice_d = w;  w += slab;
         int32_t* choice_q = w;  w += slab;
         int32_t* rows = w;      w += slab;
+        if (sig_slot) { or_scratch(c.ar->sigma, w); w += slab; }
         or_scratch(c.ar->phi, phi);
         or_scratch(c.ar->order, order);
         if (c.hsel) {
@@ -1831,10 +1858,13 @@ int mmf_arima_se_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int3
   return stats_tail(ctx, stats, n, Tally{1, MMF_KERNEL_WARP});
 }
 
-// ---- (p, d) and (p, d, q) selection by hold-out MSE on levels (DESIGN.md section 2 items 12, 14, 18) --------------------
+// ---- (p, d) and (p, d, q) selection by hold-out MSE on levels (DESIGN.md section 2 items 12, 14, 18, 21) ----------------
 // The MA arguments (mas .. out_ma_order) are those of mmf_fit_select_arma_f32 (with_q); mmf_fit_select_arima_f32 passes
-// none and launches no arma_select_kernel.  The refit calls (css, with_q; joint with css) add one refit stage per listed
-// d behind the selection's stages.
+// none and launches no arma_select_kernel.  The refit calls (css, with_q; joint with css; ml with css, kf with ml) add one
+// refit stage per listed d behind the selection's stages.  The ML + Kalman call with standard errors (kf->se) cannot run
+// the predictor inside those stages: the se pass must see every d's ML refit first, and arma_kf_list_kernel then
+// overwrites the rows it covers.  So the last refit stage runs the se pass (per-series d), and one Kalman stage per listed
+// d follows (that d's fit again, its list, arma_kf_list_kernel).  Without se the predictor runs in the refit stage.
 static int select_arima_call(mmf_ctx* ctx, const char* name, bool with_q, const float* y, int64_t n, int64_t ld_y,
                              int32_t n_hold, const int32_t* orders, int32_t n_orders, const int32_t* diffs,
                              int32_t n_diffs, const int32_t* mas, int32_t n_mas, int32_t long_order, int32_t pred_start,
@@ -1842,7 +1872,7 @@ static int select_arima_call(mmf_ctx* ctx, const char* name, bool with_q, const 
                              int32_t* out_choice_d, int32_t* out_choice_q, float* out_mse, float* out_cand_mse,
                              float* out_phi, float* out_theta, int32_t* out_order, int32_t* out_ma_order,
                              float* out_sigma, int32_t* out_status, mmf_stats* stats, const CssArgs* css = nullptr,
-                             const JointArgs* joint = nullptr) {
+                             const JointArgs* joint = nullptr, const MlArgs* ml = nullptr, const KfArgs* kf = nullptr) {
   if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
   GrowScope grow_scope(ctx);
   if (n < 0) return fail(MMF_E_INVALID, "n < 0");
@@ -1886,13 +1916,17 @@ static int select_arima_call(mmf_ctx* ctx, const char* name, bool with_q, const 
   if (ld_y < (int64_t)T + n_hold)
     return fail(MMF_E_INVALID, "ld_y=%lld < t_fit + n_hold=%lld", (long long)ld_y, (long long)T + n_hold);
   if (int rc = check_window(pred_start, n_pred, n_rows, ld_out)) return rc;
+  if (kf && kf->se && kf->ld_se < n_pred)
+    return fail(MMF_E_INVALID, "ld_se=%lld < n_pred=%d", (long long)kf->ld_se, n_pred);
   if (stats) memset(stats, 0, sizeof(*stats));
   if (n == 0) return MMF_OK;
   CU_TRY(cudaSetDevice(ctx->device));
   if (!on_device({y, out_pred}, {out_choice_p, out_choice_d, out_mse, out_cand_mse, out_phi, out_order, out_sigma,
                                  out_status, out_choice_q, out_theta, out_ma_order, css ? css->css_start : nullptr,
                                  css ? css->css : nullptr, css ? css->css_stop : nullptr, css ? css->iters : nullptr,
-                                 joint ? joint->beta : nullptr}))
+                                 joint ? joint->beta : nullptr, ml ? ml->loglik_start : nullptr,
+                                 ml ? ml->loglik : nullptr, ml ? ml->stop : nullptr, ml ? ml->iters : nullptr,
+                                 kf ? kf->se : nullptr}))
     return fail(MMF_E_UNSUPPORTED, "%s takes device buffers only", name);
 
   // (p, d, q) selection: the (p, q >= 1) pairs q-major, and their row sets R(q, L = max(p, q)) in order of appearance
@@ -1967,10 +2001,25 @@ static int select_arima_call(mmf_ctx* ctx, const char* name, bool with_q, const 
     c.arma = hr;
     c.css = *css;
     if (joint) c.joint = *joint;
+    if (ml) c.ml = *ml;
+    if (kf) {
+      c.kf = *kf;
+      c.kf_list = kf->se == nullptr;
+      c.se_pass = kf->se != nullptr && k == n_diffs - 1;
+    }
     RefitArgs rf{};
     rf.choice_d = out_choice_d; rf.choice_q = out_choice_q; rf.first = k == 0;
     c.refit = rf;
     stages.push_back({&plan, c});
+  }
+  // the Kalman stages of a call with standard errors: per listed d, the refit stage's fit and list again (the scratch
+  // holds the last d's), then arma_kf_list_kernel over the ML refit's outputs
+  for (int k = 0; kf && kf->se && k < n_diffs; ++k) {
+    Stage st = stages[n_diffs + k];
+    st.call.ml.reset();
+    st.call.kf_list = true; st.call.se_pass = false; st.call.kf_only = true;
+    st.call.refit->first = 0;
+    stages.push_back(st);
   }
   return enqueue(ctx, level_plan, std::move(stages), n, stats);
 }
@@ -2039,6 +2088,53 @@ int mmf_fit_select_arma_joint_f32(mmf_ctx* ctx, const float* y, int64_t n, int64
                            n_diffs, mas, n_mas, long_order, pred_start, n_pred, out_pred, ld_out, out_choice_p,
                            out_choice_d, out_choice_q, out_mse, out_cand_mse, out_phi, out_theta, out_order,
                            out_ma_order, out_sigma, out_status, stats, &css, &joint);
+}
+
+int mmf_fit_select_arma_ml_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
+                               const int32_t* orders, int32_t n_orders, const int32_t* diffs, int32_t n_diffs,
+                               const int32_t* mas, int32_t n_mas, int32_t long_order, int32_t max_iter,
+                               int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out,
+                               int32_t* out_choice_p, int32_t* out_choice_d, int32_t* out_choice_q, float* out_mse,
+                               float* out_cand_mse, float* out_phi, float* out_theta, int32_t* out_order,
+                               int32_t* out_ma_order, float* out_sigma, int32_t* out_status, float* out_loglik_start,
+                               float* out_loglik, int32_t* out_ml_stop, int32_t* out_iters, mmf_stats* stats) {
+  if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
+  if (max_iter < 0 || max_iter > MMF_CSS_ITER_MAX)
+    return fail(MMF_E_INVALID, "max_iter=%d outside [0,%d]", max_iter, MMF_CSS_ITER_MAX);
+  CssArgs css{};                           // the CSS refit's start, its own columns unwritten
+  css.max_iter = max_iter == 0 ? MMF_CSS_ITER_DEFAULT : max_iter;
+  MlArgs ml{};
+  ml.max_iter = css.max_iter;
+  ml.loglik_start = out_loglik_start; ml.loglik = out_loglik; ml.stop = out_ml_stop; ml.iters = out_iters;
+  return select_arima_call(ctx, "mmf_fit_select_arma_ml_f32", true, y, n, ld_y, n_hold, orders, n_orders, diffs,
+                           n_diffs, mas, n_mas, long_order, pred_start, n_pred, out_pred, ld_out, out_choice_p,
+                           out_choice_d, out_choice_q, out_mse, out_cand_mse, out_phi, out_theta, out_order,
+                           out_ma_order, out_sigma, out_status, stats, &css, nullptr, &ml);
+}
+
+int mmf_fit_select_arma_ml_kf_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
+                                  const int32_t* orders, int32_t n_orders, const int32_t* diffs, int32_t n_diffs,
+                                  const int32_t* mas, int32_t n_mas, int32_t long_order, int32_t max_iter,
+                                  int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out,
+                                  int32_t* out_choice_p, int32_t* out_choice_d, int32_t* out_choice_q, float* out_mse,
+                                  float* out_cand_mse, float* out_phi, float* out_theta, int32_t* out_order,
+                                  int32_t* out_ma_order, float* out_sigma, int32_t* out_status,
+                                  float* out_loglik_start, float* out_loglik, int32_t* out_ml_stop, int32_t* out_iters,
+                                  float* out_se, int64_t ld_se, mmf_stats* stats) {
+  if (!ctx) return fail(MMF_E_INVALID, "ctx is NULL");
+  if (max_iter < 0 || max_iter > MMF_CSS_ITER_MAX)
+    return fail(MMF_E_INVALID, "max_iter=%d outside [0,%d]", max_iter, MMF_CSS_ITER_MAX);
+  CssArgs css{};                           // the ML refit's stages, then the predictor
+  css.max_iter = max_iter == 0 ? MMF_CSS_ITER_DEFAULT : max_iter;
+  MlArgs ml{};
+  ml.max_iter = css.max_iter;
+  ml.loglik_start = out_loglik_start; ml.loglik = out_loglik; ml.stop = out_ml_stop; ml.iters = out_iters;
+  KfArgs kf{};
+  kf.se = out_se; kf.ld_se = ld_se;
+  return select_arima_call(ctx, "mmf_fit_select_arma_ml_kf_f32", true, y, n, ld_y, n_hold, orders, n_orders, diffs,
+                           n_diffs, mas, n_mas, long_order, pred_start, n_pred, out_pred, ld_out, out_choice_p,
+                           out_choice_d, out_choice_q, out_mse, out_cand_mse, out_phi, out_theta, out_order,
+                           out_ma_order, out_sigma, out_status, stats, &css, nullptr, &ml, &kf);
 }
 
 // ---- ragged batches: many calendars, one launch ------------------------------------------------------------------

@@ -360,6 +360,15 @@ cudaError_t launch_arma_css_list(const DesignView& d, const FitArgs& a, const Ar
 cudaError_t launch_arma_joint_list(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
                                    const ArmaArgs& hr, const CssArgs& cs, const JointArgs& jt, const RefitArgs& rf,
                                    cudaStream_t s);
+// the ML refit and its Kalman predictor (arma_ml.cu, arma_kf.cu, DESIGN.md section 2 item 21): arma_ml_list_kernel and
+// arma_kf_list_kernel run arma_ml_kernel / arma_kf_kernel over the refit stage's list as arma_css_list_kernel runs
+// arma_css_kernel; refit_ml_cols_kernel writes the ML columns of the rows refit_list_kernel leaves out, by its rule
+cudaError_t launch_arma_ml_list(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
+                                const ArmaArgs& hr, const MlArgs& ml, const RefitArgs& rf, cudaStream_t s);
+cudaError_t launch_refit_ml_cols(const FitArgs& a, const ArimaArgs& ma, const MlArgs& ml, const RefitArgs& rf,
+                                 cudaStream_t s);
+cudaError_t launch_arma_kf_list(const DesignView& d, const FitArgs& a, const ArArgs& ar, const ArimaArgs& ma,
+                                const ArmaArgs& hr, const KfArgs& kf, const RefitArgs& rf, cudaStream_t s);
 
 // per-series (p, d, q) selection by hold-out MSE on levels (arma_select.cu, DESIGN.md section 2 item 14): one launch per
 // listed d, right behind that d's arima_select_kernel (same fit, z', gamma / c and running best), for the q >= 1 blocks.

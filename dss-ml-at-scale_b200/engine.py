@@ -831,7 +831,8 @@ class ForecastEngine:
 
     def fit_select_arma(self, y, n_hold: int, orders=(0, 1, 2, 3, 4), diffs=(0, 1, 2), mas=(0, 1, 2, 3, 4),
                         pred_start: int = 0, n_pred: int | None = None, long_order: int = 0, want_stats: bool = False,
-                        want_se: bool = False, refit: str | None = None, joint_beta: bool = False, max_iter: int = 0):
+                        want_se: bool = False, refit: str | None = None, joint_beta: bool = False, max_iter: int = 0,
+                        predictor: str = "recursion"):
         """Regression with ARIMA(p, d, q) errors, (p, d, q) chosen per series by hold-out MSE on levels
         (``mmf_fit_select_arma_f32``, DESIGN.md section 2 item 14).  The candidates are every triple of ``orders``,
         ``diffs`` and ``mas`` (ascending, distinct, 0 .. MMF_MA_MAX, ``mas[0] == 0``), d, then q, then p ascending:
@@ -850,14 +851,31 @@ class ForecastEngine:
         refit).  ``joint_beta=True`` (``mmf_fit_select_arma_joint_f32``) refits the q >= 1 winners with beta estimated
         jointly (``fit_forecast_arma(..., joint_beta=True)``) and adds ``beta`` [n, 16]: the joint call's for those, W
         gamma of the winner's plain fit for q = 0 winners, NaN where no candidate is eligible.  With ``want_se=True`` the
-        standard errors take the refit's (phi, theta, sigma)."""
+        standard errors take the refit's (phi, theta, sigma).
+
+        ``refit="ml"`` (``mmf_fit_select_arma_ml_f32``, DESIGN.md section 2 item 21) refines that CSS refit by exact
+        likelihood: a winner with q >= 1 gets every output of ``fit_forecast_arma(p, q, d, long_order=m_d,
+        estimator="ml", max_iter=max_iter)`` bit for bit, and the result adds ``loglik_start``, ``loglik``, ``ml_stop``
+        and ``iters`` (NaN, NaN, 0, 0 where nothing was refit) in place of the CSS columns.  ``predictor="kalman"``
+        with it (``mmf_fit_select_arma_ml_kf_f32``) predicts those winners with the likelihood's Kalman filter, as
+        ``fit_forecast_arma(..., estimator="ml", predictor="kalman")`` does, and ``want_se=True`` then returns the
+        call's own standard errors.  ``joint_beta=True`` is not offered with ``refit="ml"``."""
         import torch
-        if refit not in (None, "css"):
-            raise ValueError(f"refit must be None or 'css', got {refit!r}")
+        if refit not in (None, "css", "ml"):
+            raise ValueError(f"refit must be None or 'css' (or 'ml' for the exact likelihood), got {refit!r}")
         if refit is None and int(max_iter) != 0:
-            raise ValueError("max_iter= is the pass budget of refit='css'")
+            raise ValueError("max_iter= is the pass budget of refit='css' (or 'ml')")
         if joint_beta and refit is None:
             raise ValueError("joint_beta=True needs refit='css' (beta joins the conditional least-squares refit)")
+        if joint_beta and refit == "ml":
+            raise ValueError("joint_beta=True needs refit='css' (beta joins the conditional least-squares refit; joint "
+                             "beta by the exact likelihood is not offered), got refit='ml'")
+        if predictor not in ("recursion", "kalman"):
+            raise ValueError(f"predictor must be 'recursion' or 'kalman', got {predictor!r}")
+        kalman = predictor == "kalman"
+        if kalman and refit != "ml":
+            raise ValueError(f"predictor='kalman' needs estimator='ml' (or refit='ml' for a selection: the filter of "
+                             f"the exact-likelihood fit), got refit={refit!r}")
         orders = [int(m) for m in orders]
         diffs = [int(d) for d in diffs]
         mas = [int(q) for q in mas]
@@ -903,6 +921,25 @@ class ForecastEngine:
         if refit is None:
             N.check(self._lib.mmf_fit_select_arma_f32(*head, int(pred_start), int(n_pred), out.data_ptr(), out.stride(0),
                                                       *tail, C.byref(st) if st is not None else None))
+        elif refit == "ml":
+            res.update(loglik_start=torch.empty(n, device=dev, dtype=torch.float32),
+                       loglik=torch.empty(n, device=dev, dtype=torch.float32),
+                       ml_stop=torch.empty(n, device=dev, dtype=torch.int32),
+                       iters=torch.empty(n, device=dev, dtype=torch.int32))
+            ml_out = (res["loglik_start"].data_ptr(), res["loglik"].data_ptr(), res["ml_stop"].data_ptr(),
+                      res["iters"].data_ptr())
+            sp = C.byref(st) if st is not None else None
+            if kalman:
+                se = torch.empty((n, n_pred), device=dev, dtype=torch.float32) if want_se else None
+                N.check(self._lib.mmf_fit_select_arma_ml_kf_f32(*head, int(max_iter), int(pred_start), int(n_pred),
+                                                                out.data_ptr(), out.stride(0), *tail, *ml_out,
+                                                                se.data_ptr() if se is not None else None,
+                                                                se.stride(0) if se is not None else 0, sp))
+                if se is not None:
+                    res["se"] = se
+            else:
+                N.check(self._lib.mmf_fit_select_arma_ml_f32(*head, int(max_iter), int(pred_start), int(n_pred),
+                                                             out.data_ptr(), out.stride(0), *tail, *ml_out, sp))
         else:
             res.update(css_start=torch.empty(n, device=dev, dtype=torch.float32),
                        css=torch.empty(n, device=dev, dtype=torch.float32),
@@ -918,7 +955,7 @@ class ForecastEngine:
             else:
                 N.check(self._lib.mmf_fit_select_arma_css_f32(*head, int(max_iter), int(pred_start), int(n_pred),
                                                               out.data_ptr(), out.stride(0), *tail, *css_out))
-        if want_se:
+        if want_se and "se" not in res:
             self._add_se(res, y, t_fit, pred_start, n_pred, 0, diffs=choice_d)
         if st is not None:
             self.launches += st.kernel_launches

@@ -354,9 +354,9 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
     ``estimator``: the fixed-order ARIMA(p, d, q) call's estimator (None: the engine's default, Hannan-Rissanen);
     ``joint_beta``: with ``estimator="css"``, beta estimated jointly with (phi, theta).
     ``refit``: with candidate MA orders, the winner refit by conditional least squares (``joint_beta`` with it: beta
-    jointly).
-    ``predictor``: with ``estimator="ml"``, "kalman" predicts with the filter of the exact likelihood (None: the
-    recursion)."""
+    jointly), or "ml" by exact likelihood.
+    ``predictor``: with ``estimator="ml"`` or ``refit="ml"``, "kalman" predicts with the filter of the exact likelihood
+    (None: the recursion)."""
     se_kw = {"want_se": True} if want_se else {}
     if interval and select is not None:
         raise ValueError("interval= is not offered with select= (model selection returns point forecasts)")
@@ -376,6 +376,8 @@ def _fit_buckets(buckets, eng, freq, horizon, mode, design, select, on_device, i
             from .engine import device_packed
             yd = b.y if (on_device or not isinstance(eng, ForecastEngine)) else device_packed(b.y)
             ref_kw = {"refit": refit, "joint_beta": joint_beta} if refit is not None else {}
+            if predictor is not None:                # only when given: engines without predictor= keep working
+                ref_kw["predictor"] = predictor
             res = eng.fit_select_arma(yd, horizon, ar, diff, ma, pred_start, n_pred, **se_kw, **ref_kw)
             pred, se = _host(res["pred"]), (_host(res["se"]) if want_se else None)
         elif ma is not None:
@@ -561,12 +563,13 @@ def _estimator(estimator, ma, select, interval):
 
 
 def _refit(refit, ma, estimator, select, interval):
-    """validated ``refit=``: None (the selection's Hannan-Rissanen winners, as before) or "css", the winner of the
-    (p, d, q) selection refit by conditional least squares (DESIGN.md section 2 item 18).  It needs candidate MA orders."""
+    """validated ``refit=``: None (the selection's Hannan-Rissanen winners, as before), "css", the winner of the
+    (p, d, q) selection refit by conditional least squares (DESIGN.md section 2 item 18), or "ml", that refit refined by
+    exact likelihood (item 21).  It needs candidate MA orders."""
     if refit is None:
         return None
-    if refit != "css":
-        raise ValueError(f"refit must be None or 'css', got {refit!r}")
+    if refit not in ("css", "ml"):
+        raise ValueError(f"refit must be None or 'css' (or 'ml' for the exact likelihood), got {refit!r}")
     if select is not None or interval is not None:
         raise ValueError("refit= is not offered with select= or interval= (ARMA forecasts come without either)")
     if estimator is not None:
@@ -578,16 +581,16 @@ def _refit(refit, ma, estimator, select, interval):
     return refit
 
 
-def _predictor(predictor, estimator):
+def _predictor(predictor, estimator, refit=None):
     """validated ``predictor=``: None (the recursion, as before), "recursion", or "kalman" with ``estimator="ml"``
-    (DESIGN.md section 2 item 20)"""
+    (DESIGN.md section 2 item 20) or ``refit="ml"`` (item 21)"""
     if predictor is None:
         return None
     if predictor not in ("recursion", "kalman"):
         raise ValueError(f"predictor must be 'recursion' or 'kalman', got {predictor!r}")
-    if predictor == "kalman" and estimator != "ml":
-        raise ValueError(f"predictor='kalman' needs estimator='ml' (the filter of the exact-likelihood fit), "
-                         f"got estimator={estimator!r}")
+    if predictor == "kalman" and estimator != "ml" and refit != "ml":
+        raise ValueError(f"predictor='kalman' needs estimator='ml' (or refit='ml' for a selection: the filter of the "
+                         f"exact-likelihood fit), got estimator={estimator!r}, refit={refit!r}")
     return predictor
 
 
@@ -598,6 +601,9 @@ def _joint_beta(joint_beta, estimator, refit=None):
         return False
     if refit == "css":
         return True
+    if refit == "ml":
+        raise ValueError("joint_beta=True needs estimator='css' or refit='css' (joint beta by the exact likelihood is "
+                         "not offered), got refit='ml'")
     if estimator != "css":
         raise ValueError(f"joint_beta=True needs estimator='css' (beta joins the conditional least-squares fit), "
                          f"got estimator={estimator!r}")
@@ -801,7 +807,10 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     reference fits its final model on the tuned order (``ForecastEngine.fit_select_arma(..., refit="css")``, DESIGN.md
     section 2 item 18); ``joint_beta=True`` with it estimates beta jointly in that refit.  Schema unchanged, ``conf_int=``
     works as above.  Refused with a fixed ``ma=``, with ``estimator=``, ``select=`` or ``interval=``, and for any value
-    other than ``"css"``.
+    other than ``"css"`` or ``"ml"``.  ``refit="ml"`` refines that refit by exact likelihood
+    (``ForecastEngine.fit_select_arma(..., refit="ml")``, DESIGN.md section 2 item 21), and ``predictor="kalman"`` with
+    it predicts with the likelihood's Kalman filter, ``conf_int=`` bands from its own standard errors: the reference's
+    final model and its ``predict()``.  ``joint_beta=True`` is refused with ``refit="ml"``.
     """
     eng = engine or default_engine()
     keys = list(keys)
@@ -809,7 +818,7 @@ def forecast_groups(pdf, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Deman
     z = _z_of(interval)
     cz = _conf_z(conf_int, ar, select, interval)
     est = _estimator(estimator, ma, select, interval)
-    pr = _predictor(predictor, est)
+    pr = _predictor(predictor, est, refit)
     ref = _refit(refit, ma, est, select, interval)
     jb = _joint_beta(joint_beta, est, ref)
     if ma is None:
@@ -927,8 +936,8 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     ``forecast_groups``; ``diff=d`` with ``ar=p`` fits ARIMA(p, d, 0) errors as there, and ``ma=q`` ARIMA(p, d, q); tuples of ``ar``, ``diff`` and
     ``ma`` choose (p, d, q) per series.  ``conf_int=level`` adds the same two columns for those forecasts, and
     ``estimator="css"`` (or ``"ml"``) refines a fixed ``ma=q``'s estimate and ``joint_beta=True`` adds beta to it, and ``refit="css"``
-    refits the selection's winners (with ``joint_beta=True``: beta jointly), and ``predictor="kalman"`` with
-    ``estimator="ml"`` predicts with the Kalman filter, as in ``forecast_groups``."""
+    (or ``"ml"``) refits the selection's winners (with ``joint_beta=True``: beta jointly), and ``predictor="kalman"`` with
+    ``estimator="ml"`` or ``refit="ml"`` predicts with the Kalman filter, as in ``forecast_groups``."""
     import pyarrow as pa
 
     if isinstance(table, pa.RecordBatch):
@@ -938,7 +947,7 @@ def forecast_table(table, *, keys=DEFAULT_KEYS, date_col="Date", value_col="Dema
     z = _z_of(interval)
     cz = _conf_z(conf_int, ar, select, interval)
     est = _estimator(estimator, ma, select, interval)
-    pr = _predictor(predictor, est)
+    pr = _predictor(predictor, est, refit)
     ref = _refit(refit, ma, est, select, interval)
     jb = _joint_beta(joint_beta, est, ref)
     if ma is None:

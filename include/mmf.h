@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define MMF_VERSION 116          /* 0.1.16 */
+#define MMF_VERSION 117          /* 0.1.17 */
 #define MMF_P 16                 /* design columns (zero-pad narrower designs) */
 #define MMF_PIVOT_TOL 1e-3f      /* per-series relative Cholesky pivot threshold */
 #define MMF_CAL_TOL 1e-10        /* aliasing threshold on the float64 calendar Gram */
@@ -582,6 +582,54 @@ int mmf_fit_select_arma_joint_f32(mmf_ctx* ctx, const float* y, int64_t n, int64
                                   float* out_theta, int32_t* out_order, int32_t* out_ma_order, float* out_sigma,
                                   int32_t* out_status, float* out_css_start, float* out_css, int32_t* out_css_stop,
                                   int32_t* out_iters, mmf_stats* stats);
+
+/* ---- the (p, d, q) selection's winner refit by exact likelihood, and its Kalman predictor (DESIGN.md section 2 item 21)
+ * mmf_fit_select_arma_ml_f32: mmf_fit_select_arma_css_f32, then every q >= 1 winner refined by
+ * mmf_fit_forecast_arma_ml_f32's maximum likelihood from the CSS refit's (phi, theta).  The arguments are
+ * mmf_fit_select_arma_css_f32's with that call's four CSS columns replaced by the nullable out_loglik_start, out_loglik,
+ * out_ml_stop and out_iters [n] of mmf_fit_forecast_arma_ml_f32 (the CSS columns are not returned).  Per row:
+ *   a winner with q >= 1 gets every output (pred, phi, theta, order, ma_order, sigma, status, loglik_start, loglik,
+ *   ml_stop, iters) of mmf_fit_forecast_arma_ml_f32 at its (p, d, q) with long_order = m_d, the same max_iter and the
+ *   same prediction window, bit for bit;
+ *   a winner with q = 0, and a row with no eligible candidate, keeps every output of mmf_fit_select_arma_f32 bit for bit,
+ *   with loglik_start and loglik NaN and ml_stop and iters 0 (q = 0 winners are not refit).
+ * choice_p, choice_d, choice_q, mse and cand_mse are mmf_fit_select_arma_f32's bit for bit.  max_iter outside [0,
+ * MMF_CSS_ITER_MAX] is MMF_E_INVALID, checked first; every other refusal is mmf_fit_select_arma_f32's, with its code and
+ * text.  Otherwise mmf_fit_select_arma_css_f32's contract, scratch included (68 B per row).
+ * replaces: the reference's final model (02:472-481), SARIMAX(order = the tuned order, exog) fitted on the training rows
+ * after the tuning loop, by the exact likelihood. */
+int mmf_fit_select_arma_ml_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
+                               const int32_t* orders, int32_t n_orders, const int32_t* diffs, int32_t n_diffs,
+                               const int32_t* mas, int32_t n_mas, int32_t long_order, int32_t max_iter,
+                               int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out,
+                               int32_t* out_choice_p, int32_t* out_choice_d, int32_t* out_choice_q, float* out_mse,
+                               float* out_cand_mse /* [n][n_diffs][n_mas][n_orders] */, float* out_phi,
+                               float* out_theta, int32_t* out_order, int32_t* out_ma_order, float* out_sigma,
+                               int32_t* out_status, float* out_loglik_start, float* out_loglik, int32_t* out_ml_stop,
+                               int32_t* out_iters, mmf_stats* stats);
+
+/* mmf_fit_select_arma_ml_kf_f32: mmf_fit_select_arma_ml_f32 with the same arguments and out_se / ld_se of
+ * mmf_fit_forecast_arma_ml_kf_f32.  Per row:
+ *   a winner with q >= 1 gets every output of mmf_fit_forecast_arma_ml_kf_f32 at its (p, d, q) with long_order = m_d,
+ *   the same max_iter and the same prediction window, out_se included, bit for bit;
+ *   every other row keeps mmf_fit_select_arma_ml_f32's outputs, and its out_se is mmf_arima_se_f32 of the call's outputs
+ *   with the per-series d (diffs = choice_d) bit for bit (NaN for a row with no eligible candidate).
+ * ld_se < n_pred with out_se given is MMF_E_INVALID.  Otherwise mmf_fit_select_arma_ml_f32's contract.  With out_se the
+ * call runs each listed d's fit once more (the predictor follows the se pass over every row), so n_pending counts
+ * 3 n_diffs fits per row; without it 2 n_diffs.  Scratch: per slab, 72 B per row when out_se is given and out_sigma is
+ * NULL (the winner's sigma as well), 68 B otherwise.
+ * replaces: the reference's final model and its predict() (02:472-488): SARIMAX fitted at the tuned order by exact
+ * likelihood, then the Kalman filter's predictions in sample, its dynamic forecast beyond, and their standard errors. */
+int mmf_fit_select_arma_ml_kf_f32(mmf_ctx* ctx, const float* y, int64_t n, int64_t ld_y, int32_t n_hold,
+                                  const int32_t* orders, int32_t n_orders, const int32_t* diffs, int32_t n_diffs,
+                                  const int32_t* mas, int32_t n_mas, int32_t long_order, int32_t max_iter,
+                                  int32_t pred_start, int32_t n_pred, float* out_pred, int64_t ld_out,
+                                  int32_t* out_choice_p, int32_t* out_choice_d, int32_t* out_choice_q, float* out_mse,
+                                  float* out_cand_mse /* [n][n_diffs][n_mas][n_orders] */, float* out_phi,
+                                  float* out_theta, int32_t* out_order, int32_t* out_ma_order, float* out_sigma,
+                                  int32_t* out_status, float* out_loglik_start, float* out_loglik,
+                                  int32_t* out_ml_stop, int32_t* out_iters, float* out_se, int64_t ld_se,
+                                  mmf_stats* stats);
 
 /* ---- standard errors of the ARIMA-family forecasts (DESIGN.md section 2 item 15) ----------------------------------------
  * mmf_arima_se_f32: a post-pass over the outputs of any ARIMA-family call (mmf_fit_forecast_ar_f32, _arima_f32, _arma_f32,

@@ -11,7 +11,13 @@ several rounds after a warm-up, timed with CUDA events around work that ends in 
 Prints ms per call (median and spread), the refit rows' passes (mean, p50, p90) and stop shares, the share of rows
 refit and refined, the hold-out MSE of the selection against each refit (NaN-aware), and the card's name and power limit.
 
+--refit ml (mmf_fit_select_arma_ml_f32, DESIGN.md section 2 item 21) times select, css, ml (fit_select_arma(refit="ml"))
+and, with --kalman, mlkf (refit="ml", predictor="kalman"); compose is then the composition of the last of them (the
+fixed-order call with estimator="ml", and predictor="kalman" with --kalman).  The ML arms' pass statistics are those of
+the ML refinement (iters, ml_stop).
+
     python scripts/bench_arma_select_css.py [--series 1000000] [--steps 1] [--rounds 3] [--shapes ...] [--out FILE]
+                                            [--refit css|ml] [--kalman]
 """
 import argparse
 import json
@@ -46,8 +52,9 @@ def long_order(t_fit, d):
     return min(32, max(2 * max(max(GRID[0]), max(GRID[2])), int(math.floor(lt * lt))))
 
 
-def compose(eng, y, t_fit, h, ps, npred):
-    """the selection, then the fixed-order CSS call per winning class on its gathered rows, scattered back"""
+def compose(eng, y, t_fit, h, ps, npred, **fixed):
+    """the selection, then the fixed-order call (CSS, or `fixed`) per winning class on its gathered rows, scattered
+    back"""
     res = eng.fit_select_arma(y, h, *GRID, ps, npred)
     cp, cd, cq = res["choice_p"], res["choice_d"], res["choice_q"]
     key = (cp * 100 + cd * 10 + cq)[cq >= 1]
@@ -58,7 +65,7 @@ def compose(eng, y, t_fit, h, ps, npred):
         sub = torch.empty((len(idx), ld), device=y.device)
         sub[:, :t_fit] = y[idx, :t_fit]
         r = eng.fit_forecast_arma(sub[:, :t_fit], p, q, d, ps, npred, long_order=long_order(t_fit, d),
-                                  estimator="css")
+                                  **(fixed or {"estimator": "css"}))
         for name, v in r.items():
             if name in res:
                 res[name][idx] = v
@@ -76,7 +83,10 @@ def main():
     ap.add_argument("--shapes", default="C4_holdout,weekly157")
     ap.add_argument("--gaps", default="0,0.001")
     ap.add_argument("--out", default=None)
+    ap.add_argument("--refit", choices=("css", "ml"), default="css")
+    ap.add_argument("--kalman", action="store_true", help="with --refit ml: also the Kalman predictor's arm")
     args = ap.parse_args()
+    ml = args.refit == "ml"
     name, limit = card()
     rows = []
     for shape in args.shapes.split(","):
@@ -96,6 +106,14 @@ def main():
                 "joint": lambda: eng.fit_select_arma(yg, h, *GRID, ps, npred, refit="css", joint_beta=True),
                 "compose": lambda: compose(eng, yg, t_fit, h, ps, npred),
             }
+            if ml:
+                kf = dict(predictor="kalman") if args.kalman else {}
+                del arms["joint"]
+                arms = {"select": arms["select"], "css": arms["css"],
+                        "ml": lambda: eng.fit_select_arma(yg, h, *GRID, ps, npred, refit="ml"),
+                        **({"mlkf": lambda: eng.fit_select_arma(yg, h, *GRID, ps, npred, refit="ml", **kf)}
+                           if args.kalman else {}),
+                        "compose": lambda: compose(eng, yg, t_fit, h, ps, npred, estimator="ml", **kf)}
             for fn in arms.values():                          # warm-up: every shape the timed window uses
                 fn()
                 torch.cuda.synchronize()
@@ -106,21 +124,24 @@ def main():
                     torch.cuda.empty_cache()
                     ms, last[k] = timed(fn, args.steps)
                     times[k].append(ms)
-            sel, cs, jt, cm = last["select"], last["css"], last["joint"], last["compose"]
+            sel, cs, cm = last["select"], last["css"], last["compose"]
             refit = (cs["choice_q"] >= 1).cpu().numpy()
             rec = dict(shape=shape, gaps=gap, series=args.series, refit_share=float(refit.mean()))
             for k in arms:
                 rec[f"{k}_ms"] = float(np.median(times[k]))
                 rec[f"{k}_ms_range"] = [float(min(times[k])), float(max(times[k]))]
-            same_bits = all(torch.equal(cs[k].view(torch.int32) if cs[k].is_floating_point() else cs[k],
+            top = "css" if not ml else ("mlkf" if args.kalman else "ml")   # the arm compose stands in for
+            cols = (("css", "css_start", "css_stop") if not ml else ("loglik", "loglik_start", "ml_stop"))
+            same_bits = all(torch.equal(last[top][k].view(torch.int32) if cm[k].is_floating_point() else last[top][k],
                                         cm[k].view(torch.int32) if cm[k].is_floating_point() else cm[k])
-                            for k in ("pred", "phi", "theta", "sigma", "css", "css_start", "css_stop", "iters"))
-            rec["css_equals_compose"] = bool(same_bits)
+                            for k in ("pred", "phi", "theta", "sigma", "iters") + cols)
+            rec[f"{top}_equals_compose"] = bool(same_bits)
             yh = yg[:, t_fit:t].float()
-            for k, r in (("select", sel), ("css", cs), ("joint", jt)):
+            for k in [k for k in arms if k != "compose"]:
+                r = last[k]
                 if k != "select":
                     it = r["iters"].cpu().numpy()[refit]
-                    stop = r["css_stop"].cpu().numpy()[refit]
+                    stop = r["ml_stop" if k in ("ml", "mlkf") else "css_stop"].cpu().numpy()[refit]
                     refined = ((r["phi"] != sel["phi"]).any(1) | (r["theta"] != sel["theta"]).any(1)).cpu().numpy()
                     rec[f"{k}_passes"] = ([float(it.mean()), float(np.percentile(it, 50)), float(np.percentile(it, 90))]
                                           if it.size else [])
@@ -131,7 +152,7 @@ def main():
                 rec[f"mse_{k}"] = float((torch.where(ok, e, 0.0) ** 2).sum() / ok.sum())
             rows.append(rec)
             print(json.dumps(rec), flush=True)
-            del last, sel, cs, jt, cm
+            del last, sel, cs, cm
             torch.cuda.empty_cache()
         eng.close()
         del y
